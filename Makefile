@@ -1,6 +1,6 @@
-# Builds the product library (sm_100a only) and the CPU oracle (test infrastructure).
+# Builds the product library (sm_90a only) and the CPU oracle (test infrastructure).
 NVCC ?= /usr/local/cuda/bin/nvcc
-ARCH  = -gencode arch=compute_100a,code=sm_100a
+ARCH  = -gencode arch=compute_90a,code=sm_90a
 NVFLAGS = $(ARCH) -O3 -std=c++17 -lineinfo -Xcompiler -fPIC,-Wall,-Wno-unused-function -Xptxas -v --expt-relaxed-constexpr
 SRC = $(wildcard tinysql_b200/csrc/*.cu)
 OBJ = $(patsubst tinysql_b200/csrc/%.cu,build/%.o,$(SRC))

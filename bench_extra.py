@@ -1,4 +1,4 @@
-"""bench.py --workload {expr,agg}: the secondary BASELINE configs on one B200 (benchmark infrastructure, like bench.py:
+"""bench.py --workload {expr,agg}: the secondary BASELINE configs on one H100 (benchmark infrastructure, like bench.py:
 the cpu_baseline legs load the oracle; the product package tinysql_b200/ never does).
   expr = C2: vectorized LT + Plus (builtin_compare_vec / builtin_arithmetic_vec) over 1e8 int64 rows
   agg  = C4: 1e8-row GROUP BY int64 key with SUM(float64), COUNT(*), 1e6 groups
@@ -208,7 +208,7 @@ def run_agg(args, lib, peak, peak_src, sampler_cls):
         "warmup": args.warmup, "ms_per_step": ms_step, "higher_is_better": True, "scaling": "weak", "vs_baseline": None, "dtype": "f64/int64", "data": "synthetic",
         "config": {"workload": f"C4: {n}-row GROUP BY int64 key, SUM(float64) + COUNT(*) + firstrow(key), {groups} groups, uniform keys", "groups_out": int(g),
                    "l2": "input 1.6 GB exceeds L2; the 1e6-group state (~50 MB) is L2-resident by design"},
-        "roofline": {"bound": "hbm", "kernel": "update pipeline of one batch, timed together: k_scatter_aos (radix scatter by key hash) + k_agg_preagg (shared-memory pre-aggregation per partition) + k_agg_update over the partial rows; below 4 input rows per group, or between 1e4 and 1.5e5 groups, k_agg_update alone", "achieved": achieved, "peak": peak, "unit": "GB/s", "frac": achieved / peak, "traffic": None,
+        "roofline": {"bound": "hbm", "kernel": "update pipeline of one batch, timed together: k_scatter_aos (radix scatter by key hash) + k_agg_preagg (shared-memory pre-aggregation per partition) + k_agg_update over the partial rows; below 4 input rows per group, or between 4.8e3 and 3.07e5 groups, k_agg_update alone", "achieved": achieved, "peak": peak, "unit": "GB/s", "frac": achieved / peak, "traffic": None,
                      "peak_source": peak_src, "algorithmic_bytes_per_row": 16, "kernel_ms": upd_s * 1e3},
         "e2e": {"value": n / e2e_s, "unit": "rows/s", "h2d_bytes_per_step": 16 * n, "d2h_bytes_per_step": int(g_host) * 24 + 3 * (int(g_host) // 8), "ms_per_step": e2e_s * 1e3},
         "gpu_launches": int(l2 - l1), "clocks": clocks, "verified": verified,

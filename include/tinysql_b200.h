@@ -1,5 +1,5 @@
 /*
- * tinysql_b200.h — C-ABI of the B200-native vectorized execution path for TinySQL.
+ * tinysql_b200.h — C-ABI of the H100-native vectorized execution path for TinySQL.
  *
  * This is the drop-in boundary: exactly the calls a cgo shim inside TinySQL's
  * `executor`, `expression` and `util/chunk` packages would bind (see INTEGRATION.md
@@ -11,7 +11,7 @@
  * (the reference calls Next from a single goroutine per operator instance,
  * executor/executor.go:155-162).
  *
- * Reference citations are relative to /root/reference (pingcap-incubator/tinysql).
+ * Reference citations are relative to the root of pingcap-incubator/tinysql.
  */
 #ifndef TINYSQL_B200_H
 #define TINYSQL_B200_H
@@ -33,7 +33,7 @@ enum {
   TQ_ERR_OVERFLOW_DOUBLE = 5,       /* types.ErrOverflow "DOUBLE"           builtin_arithmetic_vec.go:52 */
   TQ_ERR_DIVISION_BY_ZERO = 6,      /* handleDivisionByZeroError in strict mode, builtin_arithmetic_vec.go:369-375 */
   TQ_ERR_CUDA = 7,                  /* device fault / launch failure (generic internal error) */
-  TQ_ERR_NO_DEVICE = 8,             /* no usable sm_100 device: there is NO CPU fallback */
+  TQ_ERR_NO_DEVICE = 8,             /* no usable sm_90 device: there is NO CPU fallback */
   TQ_ERR_OOM = 9,
   TQ_ERR_STATE = 10                 /* call out of protocol order (e.g. probe before finalize_build) */
 };
@@ -79,7 +79,7 @@ typedef struct tq_column {
 
 /* ------------------------------------------------------------------ library */
 /* Select the CUDA device for this process (one process per GPU).  Fails with
- * TQ_ERR_NO_DEVICE when no sm_100 GPU is visible. */
+ * TQ_ERR_NO_DEVICE when no sm_90 GPU is visible. */
 int32_t tq_init(int32_t device_ordinal);
 int32_t tq_shutdown(void);
 /* Copies the calling thread's last error text (NUL-terminated) into buf. */

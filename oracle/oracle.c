@@ -3,7 +3,7 @@
  *
  * TEST INFRASTRUCTURE ONLY (see oracle.h).  Written for obviousness, not speed.
  * Compile with -fwrapv: Go integer arithmetic wraps, C's is undefined.
- * Paths in comments are relative to /root/reference.
+ * Paths in comments are relative to the reference repository (pingcap-incubator/tinysql).
  */
 #include "oracle.h"
 #include <math.h>

@@ -4,7 +4,7 @@
  * Only tests/, __graft_entry__.smoke() and bench.py's cpu_baseline / --impl reference
  * legs may load this library; the product (libtinysql_b200.so) never links or calls it.
  * Each function cites the reference file:line it restates (paths relative to
- * /root/reference).  Parity status: pinned against the reference's own known-answer
+ * the reference repository).  Parity status: pinned against the reference's own known-answer
  * tests re-expressed in tests/test_oracle_golden.py, test_oracle_sort_merge.py (+ sort_cases.py),
  * test_oracle_final_agg.py and test_oracle_strnum.py (+ strnum_cases.py) (the Go reference cannot be
  * built here: no Go toolchain, and the join/agg hot functions are course stubs).

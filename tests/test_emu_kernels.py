@@ -4,7 +4,7 @@ they use (one OS thread per CUDA thread, pthread barriers for __syncthreads and 
 cuda_runtime.h) into libtq_emu.so, which exports the same C-ABI entry points.  The host-side mirror (tinysql_b200/executor.py,
 chunk.py) is pointed at that library and the bodies of the GPU parity tests run against the oracle.  This checks the code's
 LOGIC (indexing, ranking, masks, searches, the host orchestration); timing, memory-model and launch behaviour are what the
-`-m gpu` tests of the same names check on the B200."""
+`-m gpu` tests of the same names check on the H100."""
 import ctypes as C
 import os
 import subprocess

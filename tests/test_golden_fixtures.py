@@ -128,7 +128,7 @@ ENGINES = [pytest.param(OracleEngine(), id="oracle"), pytest.param(GpuEngine(), 
 def engine(request):
     eng = request.param
     if eng.name == "gpu":
-        request.getfixturevalue("lib")  # loads libtinysql_b200.so and needs a B200
+        request.getfixturevalue("lib")  # loads libtinysql_b200.so and needs an H100
     return eng
 
 

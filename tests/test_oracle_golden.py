@@ -1,6 +1,6 @@
 """CPU suite, part 1: the oracle (oracle/oracle.c) pinned against the known-answer tests the reference's own
 test-suite holds for this path, re-expressed (the Go tests cannot run here: no Go toolchain, hot functions
-are course stubs).  Each case cites the reference test it restates (paths relative to /root/reference)."""
+are course stubs).  Each case cites the reference test it restates (paths relative to the reference repository)."""
 import ctypes as C
 
 import numpy as np

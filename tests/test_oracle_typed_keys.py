@@ -1,5 +1,5 @@
 """CPU suite: the oracle's restatement of FLOAT / var-len key encoding, string GROUP BY and string / FLOAT aggregate
-arguments, pinned against the reference's own known answers (paths relative to /root/reference) and against an independent
+arguments, pinned against the reference's own known answers (paths relative to the reference repository) and against an independent
 pure-Python restatement."""
 import ctypes as C
 from collections import defaultdict

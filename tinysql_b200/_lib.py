@@ -1,6 +1,6 @@
 """ctypes binding of libtinysql_b200.so — the C-ABI declared in include/tinysql_b200.h.
 
-The product path is the CUDA library: if it is missing or no sm_100 GPU is visible every call
+The product path is the CUDA library: if it is missing or no sm_90 GPU is visible every call
 fails loudly (TQ_ERR_NO_DEVICE); there is no CPU fallback anywhere in this package.
 """
 import ctypes as C

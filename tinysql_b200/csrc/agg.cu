@@ -719,15 +719,13 @@ static int32_t agg_try_preagg(tq_agg *a, const DCol *cols, int64_t n, bool *done
   int pbits = 0;
   while (((int64_t)PRE_MAX_GROUPS_PER_PART << pbits) < g_est) pbits++;
   if (pbits > 12) return TQ_OK;
-  // Measured (B200, 5e7 rows, SUM(f64)+COUNT): one table per CTA (<= 2400 groups) 0.69 ms vs 1.27 ms on the general path;
-  // with radix partitioning (3e4 / 1e6 groups) 1.65 / 1.69 ms vs 1.00 / 1.63 ms — the 64-bit shared-memory atomics cost
-  // more than the L2 atomics they replace, so the partitioned variant stays opt-in until that kernel is reworked.
+  // One table per CTA (<= 2400 groups) beats the general path; with radix partitioning the 64-bit shared-memory atomics can
+  // cost more than the L2 atomics they replace, so the partitioned variant is taken only where it wins (below).
   if (pbits > 0 && !a->pre_partitioned) return TQ_OK;
-  // Measured on a B200 (5e7 rows, SUM(f64) + COUNT, scripts/agg_pre_probe.py; partitioned vs general path): 3e3 groups 0.98 vs
-  // 1.29 ms, 3e4: 1.38 vs 1.14, 3e5: 1.46 vs 1.43, 1e6: 1.58 vs 1.88, 5e6: 4.09 vs 8.40 — the middle range, where the general
-  // table is still cache-friendly and the scatter is pure overhead, stays on the general path.
+  // Partitioned vs general path (scripts/agg_pre_probe.py, H100): in the middle range (4 to 128 partitions, up to 307,200
+  // groups) the general table is still cache-friendly and the scatter is pure overhead, so it stays on the general path.
   static const bool force_part = [] { const char *e = getenv("TQ_AGG_PREAGG_PART"); return e && e[0] == '1'; }();
-  if (pbits >= 2 && pbits <= 6 && !force_part) return TQ_OK;
+  if (pbits >= 2 && pbits <= 7 && !force_part) return TQ_OK;
   Runtime &r = rt();
   cudaStream_t s = r.compute;
   const int P = 1 << pbits;

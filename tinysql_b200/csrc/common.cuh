@@ -1,4 +1,4 @@
-// common.cuh — shared host runtime + device helpers for libtinysql_b200.so (sm_100a only).
+// common.cuh — shared host runtime + device helpers for libtinysql_b200.so (sm_90a only).
 #pragma once
 #include <cuda_runtime.h>
 
@@ -128,7 +128,7 @@ __host__ __device__ __forceinline__ uint64_t mix64(uint64_t k) {
 
 // Bucket / partition hash of the join tables: ONE 64-bit multiply.  Top bits = the high bits of a multiplicative
 // (Fibonacci) hash, which choose the partition; the low 32 bits are lo32 ^ hi32 of the product, which choose the slot inside
-// the partition.  The probe pipeline is instruction-issue-bound (ncu: profiles/), and mix64's two 64-bit multiplies were a
+// the partition.  The probe pipeline is instruction-issue-bound, and mix64's two 64-bit multiplies were a
 // quarter of its instructions.  Like mix64 it only places rows — equality is always decided on the key itself.
 __host__ __device__ __forceinline__ uint64_t hash_key(uint64_t k) {
   k ^= k >> 32;

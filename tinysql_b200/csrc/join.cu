@@ -43,7 +43,7 @@ static bool g_force_global_table = false;                // TQ_JOIN_FORCE_GLOBAL
 static const bool g_old_fast = false;                    // the round-1 PK-FK kernels instead of the streaming pipeline: measured slower, kept only for the paths that still call them
 static bool g_debug_sums = false;                        // TQ_JOIN_DEBUG_SUMS=1: print per-stage row counts / column checksums of the streaming pipeline (diagnostics)
 static bool g_no_tma = false;                            // TQ_JOIN_NO_TMA=1: plain loads instead of TMA bulk copies in the AoS scatter (diagnostics)
-static const int g_scatter_tile = 2048;                  // rows per tile of the AoS scatter (1024 / 4096 measured slower: DESIGN §5)
+static const int g_scatter_tile = 2048;                  // rows per tile of the AoS scatter
 
 // key_mode: how (flag, raw bytes) equality (util/codec/codec.go:212-240,363-382) maps onto raw 8-byte equality
 //   0: flags always agree (both signed, both unsigned, or both DOUBLE)  -> raw equality
@@ -1092,8 +1092,9 @@ __device__ __forceinline__ EntryPair ld_pair(const uint64_t *tbl, uint32_t loc_e
   if (smem) {
     e.a = *reinterpret_cast<const ulonglong2 *>(p);
     e.b = *reinterpret_cast<const ulonglong2 *>(p + 2);
-  } else {  // one 256-bit load = one sector
-    asm volatile("ld.global.v4.u64 {%0, %1, %2, %3}, [%4];" : "=l"(e.a.x), "=l"(e.a.y), "=l"(e.b.x), "=l"(e.b.y) : "l"(p));
+  } else {  // two 128-bit loads of the same 32-byte sector (sm_90 has no 256-bit global load)
+    asm volatile("ld.global.v2.u64 {%0, %1}, [%2];" : "=l"(e.a.x), "=l"(e.a.y) : "l"(p));
+    asm volatile("ld.global.v2.u64 {%0, %1}, [%2];" : "=l"(e.b.x), "=l"(e.b.y) : "l"(p + 2));
   }
   return e;
 }
@@ -1702,7 +1703,7 @@ static int32_t try_stream_build(tq_join *j, bool *done) {
   bp.n_parts = P;
   bp.key_col = j->build_key;
   {
-    int64_t split = (int64_t)(mean / 4096.0);   // ~4K rows per CTA: a dozen partitions are live across the 148 SMs
+    int64_t split = (int64_t)(mean / 4096.0);   // ~4K rows per CTA: about a dozen partitions are live across the 132 SMs
     bp.split = (int)(split < 1 ? 1 : (split > 256 ? 256 : split));
   }
   {

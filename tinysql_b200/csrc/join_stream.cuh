@@ -70,9 +70,9 @@ __host__ __device__ constexpr int sa_occ(int nc) {  // resident CTAs per SM the 
   return sa_smem_bytes<T>(nc, 130) <= 72 * 1024 ? 3 : (sa_smem_bytes<T>(nc, 130) <= 110 * 1024 ? 2 : 1);
 }
 
-// One tile = T rows.  Measured on a B200 (scripts/ub/rank.cu): ranking a row inside its bin with a shared-memory
-// atomicAdd-with-return costs no more than reading the key (0.12 ms per 1e8 rows), warp ballots over the bin bits or
-// match.any cost 4x that — so the rank is the atomic's return value.
+// One tile = T rows.  Ranking a row inside its bin with a shared-memory atomicAdd-with-return costs about as much as
+// reading the key, warp ballots over the bin bits or match.any several times that (scripts/ub/rank.cu measures the three)
+// — so the rank is the atomic's return value.
 // PLAIN: no outerSideFilter bytes and every key can match (same key type on both sides) — the foreign-key join; the general
 // instantiation pays a few runtime-uniform branches per row for `selected`, the signed/unsigned rule and the outer-join bin.
 template <int NC, int T, bool PLAIN>
@@ -471,8 +471,7 @@ __global__ void __launch_bounds__((CW + 1) * 32, OCC) k_probe_pos(const ProbePos
     }
     // The stage may be refilled (a TMA write) as soon as every warp has released it, so the values must have LEFT shared
     // memory first.  An issued LDS is not a completed one: SASS showed LDS.128 x4, WARPSYNC, SYNCS.ARRIVE with no scoreboard
-    // wait in between, and on a B200 the refill then tore rows (first 16 bytes of one tile, last 16 of another, ~50 rows in
-    // half the runs of a 1.5M-row probe).  The register scoreboard is per warp, so ONE instruction that reads every loaded
+    // wait in between, and the refill then tore rows (first 16 bytes of one tile, last 16 of another).  The register scoreboard is per warp, so ONE instruction that reads every loaded
     // register waits for the whole warp's loads: lane 0 stores their XOR to a sink word before it arrives on the barrier.
     uint64_t dep = 0;
 #pragma unroll
@@ -550,9 +549,8 @@ struct ProbePosVariant {
 };
 template <int NP, int NB>
 static ProbePosVariant probe_pos_variant() {
-  // Measured on the C3 shape (B200): 2 rows per lane x 12 consumer warps x 3 CTAs per SM (1.85 ms probe pipeline) beats 4 rows x 8
-  // warps x 3 (1.94, spills), 2 x 16 x 2 and 2 x 8 x 4: more warps in flight hide the L2 latency of the table gathers better than
-  // more loads per warp.  The losing shapes were deleted.
+  // 2 rows per lane x 12 consumer warps x 3 CTAs per SM: more warps in flight hide the L2 latency of the table gathers better
+  // than more loads per warp (4 rows per lane spills at 3 CTAs per SM).
   return {k_probe_pos<NP, NB, 2, 12, 3>, 12 * 32 * 2, 13 * 32};
 }
 template <int NP>

@@ -1,5 +1,5 @@
 // othercond.cuh — HashJoinExec OtherConditions on the device (EXPERIMENTAL: written in round 1 after the GPU budget was
-// spent; parity tests exist but are gated behind TQ_RUN_EXPERIMENTS until they have run on a B200).
+// spent; parity tests exist but are gated behind TQ_RUN_EXPERIMENTS until they have run on the GPU).
 //
 // Reference: joiner.tryToMatchInners builds the joined rows of one outer row, baseJoiner.filter keeps those for which every
 // condition is true, and an outer row none of whose joined rows survive is emitted once with a NULL inner side by

@@ -51,8 +51,8 @@ static int32_t init_device(int ordinal) {
   }
   cudaDeviceProp p;
   TQ_CUDA(cudaGetDeviceProperties(&p, ordinal));
-  if (p.major != 10) {
-    set_error("device %d is sm_%d%d; this library carries sm_100a code only", ordinal, p.major, p.minor);
+  if (p.major != 9 || p.minor != 0) {
+    set_error("device %d is sm_%d%d; this library carries sm_90a code only", ordinal, p.major, p.minor);
     return TQ_ERR_NO_DEVICE;
   }
   TQ_CUDA(cudaSetDevice(ordinal));
@@ -118,7 +118,7 @@ struct BlockCache {
   }
 };
 // leaked on purpose: DevBuf/PinBuf objects with static storage release into these during exit
-static BlockCache &dev_cache() { static BlockCache *c = new BlockCache((size_t)96 << 30); return *c; }
+static BlockCache &dev_cache() { static BlockCache *c = new BlockCache((size_t)40 << 30); return *c; }  // half of an H100's 80 GB
 static BlockCache &pin_cache() { static BlockCache *c = new BlockCache((size_t)24 << 30); return *c; }
 
 int32_t DevBuf::reserve(size_t bytes) {
@@ -382,7 +382,7 @@ int32_t tq_last_error(char *buf, int32_t buf_len) {
   return TQ_OK;
 }
 
-const char *tq_version(void) { return "tinysql_b200 0.1 (sm_100a)"; }
+const char *tq_version(void) { return "tinysql_b200 0.1 (sm_90a)"; }
 
 int32_t tq_pinned_alloc(size_t bytes, void **out) {
   if (!out) return TQ_ERR_INVALID_ARG;
@@ -501,7 +501,7 @@ int32_t tq_flush_l2(void) {
   TQ_TRY(ensure_init());
   Runtime &r = rt();
   std::lock_guard<std::recursive_mutex> lk(r.mu);
-  const size_t bytes = 256u << 20;  // 2x the 126 MB L2
+  const size_t bytes = 256u << 20;  // 5x the 50 MB L2
   if (!r.l2_scratch) {
     TQ_CUDA(cudaMalloc(&r.l2_scratch, bytes));
     r.l2_scratch_bytes = bytes;

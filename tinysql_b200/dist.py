@@ -493,7 +493,7 @@ def dist_workload_config(world, n_b, n_p, n_chunks=None):
            "build_rows_per_gpu": n_b, "probe_rows_per_gpu": n_p, "global_build_rows": N_b, "global_probe_rows": N_p,
            "exchange": "fused scatter + push into per-source regions of the peers' receive buffers (CUDA IPC peer stores over NVLink), device-side epoch "
                        "flags instead of host barriers; local join reads the regions as one segmented batch",
-           "l2": "inputs and outputs exceed the 126 MB L2; no flush needed"}
+           "l2": "inputs and outputs exceed the 50 MB L2; no flush needed"}
     if n_chunks is not None:
         cfg["parallelism"] = f"key-hash partitions over {world} ranks, {n_chunks} probe chunks pipelined (push of chunk c+1 overlaps the join of chunk c)"
     return cfg
@@ -513,7 +513,7 @@ def bench_distributed_join(args, rank, world, local_rank, dist_mod, peak, peak_s
     bk, bv, pk, pv = (torch.from_numpy(x).to(dev) for x in (bk_h, bv_h, pk_h, pv_h))
     del bk_h, bv_h, pv_h
     torch.cuda.synchronize()
-    n_chunks = max(1, int(os.environ.get("TQ_DIST_CHUNKS", "2")))   # measured at N=2: 2 chunks 5.87 ms, 3: 6.12, 4: 6.28, 8: 10.0 per step
+    n_chunks = max(1, int(os.environ.get("TQ_DIST_CHUNKS", "2")))   # probe chunks per step: fewer chunks, fewer exchanges
     rj = RegionJoin(lib, L, world, rank, n_b, n_p, n_chunks)
 
     def step(keep=False):
@@ -618,8 +618,8 @@ def bench_distributed_join(args, rank, world, local_rank, dist_mod, peak, peak_s
         "data": "synthetic",
         "config": dist_workload_config(world, n_b, n_p, n_chunks),
         "roofline": {"bound": "nvlink", "kernel": "push of this rank's probe rows (7/8 of them cross NVLink at 8 GPUs), overlapped with the local join",
-                     "achieved": push_bytes / (ms_per_step * 1e-3) / 1e9, "peak": 770.0, "unit": "GB/s", "frac": push_bytes / (ms_per_step * 1e-3) / 1e9 / 770.0,
-                     "traffic": None, "peak_source": "B200_PROFILING.md: measured peer copy 770 GB/s per direction per GPU",
+                     "achieved": push_bytes / (ms_per_step * 1e-3) / 1e9, "peak": 450.0, "unit": "GB/s", "frac": push_bytes / (ms_per_step * 1e-3) / 1e9 / 450.0,
+                     "traffic": None, "peak_source": "H100 SXM data sheet: NVLink 900 GB/s per GPU, 450 GB/s per direction",
                      "note": "whole-step time charged against the NVLink bytes one GPU must send; local probe pipeline of rank 0: "
                              f"{probe_s * 1e3:.3f} ms per chunk batch, build {statistics.mean(build_ns) * 1e-6:.3f} ms"},
         "e2e": {"value": value, "unit": "joined rows/s", "h2d_bytes_per_step": 0, "d2h_bytes_per_step": 0,
@@ -687,7 +687,7 @@ def one_gpu_reference(lib, L, dev, world, n_b, n_p, steps=2):
             L.check(lib.tq_timer_stop(C.byref(ms)))
             best = ms.value if best is None else min(best, ms.value)
     return {"ms_per_step": best, "rows": int(rows), "value": rows / (best * 1e-3), "build_rows": N_b, "probe_rows": n_p * world,
-            "note": "one B200, all inputs resident in HBM before the timed region, probe fed in device batches of one shard each; best of the timed repetitions"}
+            "note": "one GPU, all inputs resident in HBM before the timed region, probe fed in device batches of one shard each; best of the timed repetitions"}
 
 
 def _mix64_mod_torch(gid, mod):
