@@ -248,7 +248,8 @@ def test_join_partitioned_smem_tables(lib, monkeypatch):
 @pytest.mark.parametrize("no_fast", ["0", "1"])
 def test_join_partitioned_unique_pk_fk(lib, monkeypatch, no_fast):
     """the C3 shape at 1/20 scale: unique build keys, every probe row matches exactly once
-    (no_fast=0: the template-specialised PK-FK kernel; 1: the generic unique-key kernel)"""
+    (no_fast=0: the streaming build and the positional probe k_probe_pos; 1: the general build and the generic unique-key
+    kernel)"""
     monkeypatch.setenv("TQ_JOIN_NO_FAST", no_fast)
     rng = np.random.default_rng(3)
     nb, npr = 500000, 5000000
@@ -272,7 +273,8 @@ def test_join_partitioned_unique_pk_fk(lib, monkeypatch, no_fast):
 
 @pytest.mark.parametrize("nbc,npc", [(1, 1), (3, 2), (4, 4), (2, 3)])
 def test_join_fast_kernel_shapes(lib, nbc, npc):
-    """row-table fast path across column counts (16- and 32-byte entries), incl. misses and the empty-marker key"""
+    """the positional probe k_probe_pos across column counts (16- and 32-byte entries), incl. misses and the empty-marker key
+    (a build row with that key hands the table over from the streaming build to the general build)"""
     rng = np.random.default_rng(nbc * 10 + npc)
     nb, npr = 400000, 1500000
     s = np.int64(np.uint64(0xA5C3F00DDEADBEEF).astype(np.int64))

@@ -10,9 +10,14 @@
 //   CSR mode (duplicate keys or wide rows): word1 = (offset | count << 32) into build rows packed
 //       row-major in key order; duplicates keep build insertion order (rowHashMap.Get, hash_table.go:259-272).
 //       Build: insert+count, exclusive scan, fill, sort duplicate segments, gather rows.
+//   Large NOT NULL build sides that fit an entry first try the streaming build (try_stream_build, gated by stream_build_ok):
+//       k_scatter_aos into AoS slabs, then k_build_cluster builds each partition's tables in cluster shared memory.
 // Probe.  Small build (one table): k_probe, ordered output (probe row asc, build insertion asc) via
-//   ticketed tiles + decoupled look-back.  Large build: k_probe_part_hist -> scan -> k_probe_scatter
-//   (shared-memory counting sort of 8192-row tiles, coalesced full-sector stores) -> k_probe_part(_uniq).
+//   ticketed tiles + decoupled look-back.
+//   Large build, PK-FK shape (stream_probe_ok, no probe NULL bitmap): the streaming positional path of join_stream.cuh
+//   (launch_probe_stream): k_scatter_aos -> k_part_bases -> k_probe_pos -> hole filling; the result is a multiset.
+//   Any other large build: k_probe_part_hist (only after a slab overflow) -> scan -> k_probe_scatter(_fast) (shared-memory
+//   counting sort of 4096-row tiles, coalesced full-sector stores) -> k_probe_part_fast / k_probe_part(_uniq).
 #include <cstdlib>
 #include <deque>
 #include <memory>
@@ -37,13 +42,7 @@ static constexpr uint64_t PART_MAX_SMEM_BYTES = 128 << 10;  // a partition table
 static const int64_t g_tiles_per_cta = 8;
 static int64_t g_part_target_rows = 150000;              // build rows per partition: a partition table ~ 4-8 MB, a few live ones fit in L2
 static const int64_t g_max_load_pct = 50;                // partition-table load-factor bound (pair probing keeps chains short)
-static bool g_exact_scatter = false;                     // TQ_JOIN_EXACT_SCATTER=1: always run the probe-side histogram pass
 static bool g_no_fast_kernel = false;                    // TQ_JOIN_NO_FAST=1: use the generic kernels (tests)
-static bool g_force_global_table = false;                // TQ_JOIN_FORCE_GLOBAL=1: A/B switch for profiling
-static const bool g_old_fast = false;                    // the round-1 PK-FK kernels instead of the streaming pipeline: measured slower, kept only for the paths that still call them
-static bool g_debug_sums = false;                        // TQ_JOIN_DEBUG_SUMS=1: print per-stage row counts / column checksums of the streaming pipeline (diagnostics)
-static bool g_no_tma = false;                            // TQ_JOIN_NO_TMA=1: plain loads instead of TMA bulk copies in the AoS scatter (diagnostics)
-static const int g_scatter_tile = 2048;                  // rows per tile of the AoS scatter
 
 // key_mode: how (flag, raw bytes) equality (util/codec/codec.go:212-240,363-382) maps onto raw 8-byte equality
 //   0: flags always agree (both signed, both unsigned, or both DOUBLE)  -> raw equality
@@ -615,6 +614,13 @@ __global__ void k_init_slabs(uint32_t *lo, uint32_t *cursor, uint32_t *lim, int 
   cursor[i] = start;
   lim[i] = (i < n_parts) ? start + slab : start + tail_rows;
 }
+// Rows per partition slab of the optimistic (histogram-free) scatter of n rows into P partitions: hash partitions of a batch
+// are near-uniform, so the mean plus 25% and 4096 rows.  AoS slabs are rounded up to 32 rows so that every slab starts
+// 16-byte aligned whatever the row width, as the bulk copies of the positional probe require.
+static uint64_t slab_rows(int64_t n, int P, bool aos) {
+  const uint64_t slab = (uint64_t)n / P + (uint64_t)n / P / 4 + 4096;
+  return aos ? (slab + 31) & ~31ull : slab;
+}
 
 // ---- probe-side radix scatter -------------------------------------------------------------------------
 static constexpr int SCAT_THREADS = 256;
@@ -889,7 +895,7 @@ int32_t scatter_rows_by_hash(const DCol *cols, int n_cols, int key_col, int64_t 
   ScatterKernel kern = scatter_fast_kernel(n_cols);
   if (!kern || pbits < 1 || pbits > PART_MAX_BITS || n <= 0 || n > 0xFFFFFFF0ll) { set_error("internal: scatter_rows_by_hash arguments"); return TQ_ERR_INVALID_ARG; }
   const int P = 1 << pbits, n_bins = P + 1;
-  const uint64_t slab = (uint64_t)n / P + (uint64_t)n / P / 4 + 4096;
+  const uint64_t slab = slab_rows(n, P, false);
   if (slab * P > 0xFFFFFFF0ull) { set_error("batch too large for 32-bit partition offsets"); return TQ_ERR_INVALID_ARG; }
   out.resize(n_cols);
   ScatterParams sp{};
@@ -1341,37 +1347,47 @@ __global__ void __launch_bounds__(PROBE_THREADS) k_probe_part(const ProbeParams 
 #include "join_stream.cuh"
 namespace tq {
 
-// scatter.cuh: the streaming AoS scatter for other operators (HashAgg pre-aggregation)
-int32_t scatter_rows_by_hash_aos(const DCol *cols, int n_cols, int key_col, int64_t n, int pbits, DevBuf &aos, DevBuf &lo, DevBuf &hi, DevBuf &lim,
-                                 unsigned long long *d_overflow, cudaStream_t s) {
-  if (n_cols < 1 || n_cols > 4 || pbits < 1 || pbits > SA_MAX_PBITS || n <= 0 || n > 0xFFFFFFF0ll) { set_error("internal: scatter_rows_by_hash_aos arguments"); return TQ_ERR_INVALID_ARG; }
+// The optimistic AoS scatter of one batch.  The caller describes the input in q (columns, key, key_mode, selected, pbits, n,
+// overflow flag, segments); this sizes the slabs (slab_rows), reserves them and lo / hi / lim, initialises the slab bounds
+// and launches k_scatter_aos — with TMA bulk copies when every input column is 16-byte aligned, plain loads otherwise.
+static int32_t scatter_aos(ScatterAosParams &q, DevBuf &aos, DevBuf &lo, DevBuf &hi, DevBuf &lim, cudaStream_t s) {
+  const int nc = q.sp.n_cols, pbits = q.sp.pbits;
+  const int64_t n = q.sp.n;
+  if (nc < 1 || nc > 4 || pbits < 1 || pbits > SA_MAX_PBITS || n <= 0 || n > 0xFFFFFFF0ll) { set_error("internal: AoS scatter arguments"); return TQ_ERR_INVALID_ARG; }
   const int P = 1 << pbits;
-  const uint64_t slab = ((uint64_t)n / P + (uint64_t)n / P / 4 + 4096 + 31) & ~31ull;
+  const uint64_t slab = slab_rows(n, P, true);
   if (slab * P > 0xFFFFFFF0ull) { set_error("batch too large for 32-bit partition offsets"); return TQ_ERR_INVALID_ARG; }
-  TQ_TRY(aos.reserve((size_t)slab * P * n_cols * 8 + 256));
+  TQ_TRY(aos.reserve((size_t)slab * P * nc * 8 + 256));
   TQ_TRY(lo.reserve((size_t)(P + 3) * 4));
   TQ_TRY(hi.reserve((size_t)(P + 3) * 4));
   TQ_TRY(lim.reserve((size_t)(P + 3) * 4));
   k_init_slabs<<<(P + 1 + 255) / 256, 256, 0, s>>>(lo.as<uint32_t>(), hi.as<uint32_t>(), lim.as<uint32_t>(), P, (uint32_t)slab, 0u);
   count_launch();
-  ScatterAosParams q{};
-  q.sp.n_cols = n_cols;
-  q.use_tma = g_no_tma ? 0 : 1;
-  for (int c = 0; c < n_cols; c++) {
-    q.sp.in[c] = cols[c];
-    if ((reinterpret_cast<uintptr_t>(cols[c].data) & 15) != 0) q.use_tma = 0;
+  auto aligned = [](const void *ptr) { return (reinterpret_cast<uintptr_t>(ptr) & 15) == 0; };
+  q.use_tma = 1;
+  for (int c = 0; c < nc; c++) {
+    if (!aligned(q.sp.in[c].data)) q.use_tma = 0;
+    for (int g = 0; g < q.n_segs; g++)
+      if (!aligned(q.seg_in[g][c])) q.use_tma = 0;
   }
-  q.sp.selected = nullptr;
-  q.sp.key_col = key_col;
-  q.sp.key_mode = KEYMODE_RAW;
-  q.sp.is_outer = 0;
-  q.sp.pbits = pbits;
-  q.sp.n = n;
   q.sp.part_cursor = hi.as<uint32_t>();
   q.sp.part_lim = lim.as<uint32_t>();
-  q.sp.overflow = d_overflow;
   q.out = aos.as<uint64_t>();
-  return launch_scatter_aos(q, n_cols, s);
+  return launch_scatter_aos(q, nc, s);
+}
+
+// scatter.cuh: the streaming AoS scatter for other operators (HashAgg pre-aggregation)
+int32_t scatter_rows_by_hash_aos(const DCol *cols, int n_cols, int key_col, int64_t n, int pbits, DevBuf &aos, DevBuf &lo, DevBuf &hi, DevBuf &lim,
+                                 unsigned long long *d_overflow, cudaStream_t s) {
+  ScatterAosParams q{};
+  q.sp.n_cols = n_cols;
+  for (int c = 0; c < n_cols && c < 4; c++) q.sp.in[c] = cols[c];
+  q.sp.key_col = key_col;
+  q.sp.key_mode = KEYMODE_RAW;
+  q.sp.pbits = pbits;
+  q.sp.n = n;
+  q.sp.overflow = d_overflow;
+  return scatter_aos(q, aos, lo, hi, lim, s);
 }
 
 // ------------------------------------------------------------------ host side
@@ -1636,6 +1652,21 @@ static int32_t key_source(tq_join *j, bool build, int i, const std::vector<DCol>
   return TQ_OK;
 }
 
+// Whether the build side may try the streaming build (try_stream_build): a large NOT NULL build side whose rows fit a table
+// entry and whose keys can match at all.  Unlike stream_probe_ok this does not depend on the join type: a stream-built table
+// also serves outer joins, through the general partitioned probe.
+static bool stream_build_ok(const tq_join *j) {
+  return j->n_build >= PART_MIN_BUILD_ROWS && !g_no_fast_kernel && !j->build_has_nulls && j->n_build_cols <= 4 && j->key_mode != KEYMODE_NEVER;
+}
+
+// Whether probe batches may take the streaming positional path (launch_probe_stream) as far as the operator and its table
+// decide: a partitioned ROW-mode table with unique NOT NULL build rows, an inner join without OtherConditions, at most 4
+// columns per side, and optimistic slabs (no slab has overflowed yet).  The callers add what depends on the batch.
+static bool stream_probe_ok(const tq_join *j) {
+  return j->pbits > 0 && j->pbits <= SA_MAX_PBITS && j->row_mode && j->join_type == TQ_JOIN_INNER && !j->build_has_nulls && j->optimistic_scatter &&
+         j->n_probe_cols <= 4 && j->n_build_cols <= 4 && !j->has_oc && !g_no_fast_kernel;
+}
+
 // Partition-local build (join_stream.cuh): scatter the build rows into AoS partition slabs, then one thread-block cluster
 // per partition builds its sub-tables in distributed shared memory (k_build_cluster).  The table has 2^(pbits + sbits)
 // sub-tables; the probe side keeps the 2^pbits coarse partitions.  Covers the PK-FK shape — NOT NULL build columns that fit
@@ -1650,7 +1681,7 @@ static int32_t try_stream_build(tq_join *j, bool *done) {
   if (pbits > SA_MAX_PBITS) pbits = SA_MAX_PBITS;
   if (pbits < 1) return TQ_OK;
   const int P = 1 << pbits;
-  const uint64_t slab = ((uint64_t)n / P + (uint64_t)n / P / 4 + 4096 + 31) & ~31ull;
+  const uint64_t slab = slab_rows(n, P, true);
   if (slab * P > 0xFFFFFFF0ull) return TQ_OK;
   // Table capacity from the row count alone (no host round trip for the partition histogram): hash partitions of m rows hold
   // m +- a few sqrt(m); a sub-table that turns out fuller than the load limit allows is flagged by the build kernel and the
@@ -1695,30 +1726,17 @@ static int32_t try_stream_build(tq_join *j, bool *done) {
   }
   cfg.dynamicSmemBytes = (size_t)slice_bytes;
   DevBuf &off = j->part_off[0], &hi = j->part_cursor[0], &lim = j->part_lim[0];
-  TQ_TRY(off.reserve((size_t)(P + 3) * 4));
-  TQ_TRY(hi.reserve((size_t)(P + 3) * 4));
-  TQ_TRY(lim.reserve((size_t)(P + 3) * 4));
-  TQ_TRY(j->b_aos.reserve((size_t)slab * P * NB * 8 + 256));
   unsigned long long *cur = j->cursors.as<unsigned long long>();
   TQ_CUDA(cudaMemsetAsync(cur, 0, 64, s));
-  k_init_slabs<<<(P + 1 + 255) / 256, 256, 0, s>>>(off.as<uint32_t>(), hi.as<uint32_t>(), lim.as<uint32_t>(), P, (uint32_t)slab, 0u);
-  count_launch();
   ScatterAosParams q{};
   q.sp.n_cols = NB;
-  q.use_tma = g_no_tma ? 0 : 1;
-  for (int c = 0; c < NB; c++) {
-    q.sp.in[c] = j->b_view[c];
-    if ((reinterpret_cast<uintptr_t>(j->b_view[c].data) & 15) != 0) q.use_tma = 0;
-  }
+  for (int c = 0; c < NB; c++) q.sp.in[c] = j->b_view[c];
   q.sp.key_col = j->build_key;
   q.sp.key_mode = j->key_mode;   // rows whose key can never match are dropped here (hash_table.go:161-163 skips NULL keys; none here)
   q.sp.pbits = pbits;
   q.sp.n = n;
-  q.sp.part_cursor = hi.as<uint32_t>();
-  q.sp.part_lim = lim.as<uint32_t>();
   q.sp.overflow = cur + 2;
-  q.out = j->b_aos.as<uint64_t>();
-  TQ_TRY(launch_scatter_aos(q, NB, s));
+  TQ_TRY(scatter_aos(q, j->b_aos, off, hi, lim, s));
   TQ_TRY(j->slots.reserve(((n_slots + 1) << shift) * 8));  // (+ the side entry of the empty-marker key, unused on this path)
   uint64_t *words = j->slots.as<uint64_t>();
   BuildClusterParams bp{};
@@ -1782,8 +1800,7 @@ static int32_t join_build(tq_join *j) {
   TQ_CUDA(cudaMemsetAsync(counters, 0, 64, s));
   j->build_has_nulls = false;
   for (int c = 0; c < j->n_build_cols; c++) j->build_has_nulls |= (j->b_view[c].bm != nullptr);
-  if (n >= PART_MIN_BUILD_ROWS && !g_force_global_table && !g_no_fast_kernel && !g_old_fast && !j->build_has_nulls && j->n_build_cols <= 4 &&
-      j->key_mode != KEYMODE_NEVER) {
+  if (stream_build_ok(j)) {
     bool done = false;
     TQ_TRY(try_stream_build(j, &done));
     j->b_aos.release();
@@ -1806,7 +1823,7 @@ static int32_t join_build(tq_join *j) {
   // Partitioning: ~g_part_target_rows build rows per partition table; small build sides keep ONE table.
   uint64_t n_slots = 64, cap = 0;
   int pbits = 0;
-  if (n >= PART_MIN_BUILD_ROWS && !g_force_global_table) {
+  if (n >= PART_MIN_BUILD_ROWS) {
     uint64_t P = 1;
     while (P * (uint64_t)g_part_target_rows < (uint64_t)n) P <<= 1;
     while ((1ull << pbits) < P) pbits++;
@@ -2022,101 +2039,36 @@ __global__ void __launch_bounds__(256) k_hole_move_pads(const HoleMoveDevParams 
   }
 }
 
-// ---- diagnostics (TQ_JOIN_DEBUG_SUMS=1): wrapping sums of 8-byte words over strided ranges
-__global__ void k_dbg_sum(const uint64_t *base, int64_t n, int stride, unsigned long long *out) {
-  unsigned long long acc = 0;
-  for (int64_t i = (int64_t)blockIdx.x * blockDim.x + threadIdx.x; i < n; i += (int64_t)gridDim.x * blockDim.x) acc += base[i * stride];
-  atomicAdd(out, acc);
-}
-__global__ void k_dbg_sum_slab(const uint64_t *slab, const uint32_t *lo, const uint32_t *hi, int n_parts, int nc, int c, unsigned long long *out) {
-  unsigned long long acc = 0, cnt = 0;
-  for (int q = blockIdx.x; q < n_parts; q += gridDim.x)
-    for (int64_t r = lo[q] + threadIdx.x; r < (int64_t)hi[q]; r += blockDim.x) { acc += slab[r * nc + c]; cnt++; }
-  atomicAdd(out, acc);
-  atomicAdd(out + 1, cnt);
-}
-__global__ void k_dbg_sum_valid(const uint64_t *col, const uint32_t *valid, const unsigned long long *cur, unsigned long long *out) {
-  const int64_t S = (int64_t)cur[3];
-  unsigned long long acc = 0, cnt = 0;
-  for (int64_t i = (int64_t)blockIdx.x * blockDim.x + threadIdx.x; i < S; i += (int64_t)gridDim.x * blockDim.x)
-    if ((valid[i >> 5] >> (i & 31)) & 1u) { acc += col[i]; cnt++; }
-  atomicAdd(out, acc);
-  atomicAdd(out + 1, cnt);
-}
-static void dbg_report(const char *what, int c, const unsigned long long *d_out, cudaStream_t s) {
-  unsigned long long h[2] = {0, 0};
-  cudaMemcpyAsync(h, d_out, 16, cudaMemcpyDeviceToHost, s);
-  cudaStreamSynchronize(s);
-  fprintf(stderr, "[tq debug] %-28s col %d  sum=%016llx  rows=%llu\n", what, c, h[0], h[1]);
-}
-
 // scatter (AoS, TMA-fed) -> partition bases -> positional probe -> device-driven hole filling
 static int32_t launch_probe_stream(tq_join *j, const ProbeParams &p, const std::vector<DCol> &probe, const uint8_t *d_selected, int64_t n,
                                    unsigned long long *cur, int slot, uint64_t alloc_rows) {
   cudaStream_t s = rt().compute;
   const int P = 1 << j->pbits, NP = j->n_probe_cols, NB = j->n_build_cols;
-  const uint64_t slab = ((uint64_t)n / P + (uint64_t)n / P / 4 + 4096 + 31) & ~31ull;
-  if (slab * P > 0xFFFFFFF0ull) { set_error("probe batch too large for 32-bit partition offsets"); return TQ_ERR_INVALID_ARG; }
   DevBuf &off = j->part_off[slot], &cur_b = j->part_cursor[slot], &lim = j->part_lim[slot];
-  TQ_TRY(off.reserve((size_t)(P + 3) * 4));
-  TQ_TRY(cur_b.reserve((size_t)(P + 3) * 4));
-  TQ_TRY(lim.reserve((size_t)(P + 3) * 4));
   TQ_TRY(j->pos_base[slot].reserve((size_t)(P + 2) * 4));
-  TQ_TRY(j->part_aos[slot].reserve((size_t)slab * P * NP * 8 + 256));
   const int64_t n_words_max = (int64_t)(alloc_rows >> 5) + 1;
   TQ_TRY(j->pos_valid[slot].reserve((size_t)(n_words_max + 2) * 4));
   TQ_TRY(j->hole_pos[slot].reserve((size_t)(32 * (P + 2)) * 4));   // at most 31 pad slots per partition
   TQ_TRY(j->hole_src[slot].reserve((size_t)(32 * (P + 2)) * 4));
-  static const bool poison = [] { const char *e = getenv("TQ_JOIN_DEBUG_POISON"); return e && e[0] == '1'; }();
-  if (poison) {  // diagnostics: stale bytes become recognisable (0xEE.. = slab never written, 0xDD.. = result slot never written)
-    TQ_CUDA(cudaMemsetAsync(j->part_aos[slot].p, 0xEE, (size_t)slab * P * NP * 8, s));
-    for (int c = 0; c < NP; c++) TQ_CUDA(cudaMemsetAsync(p.out_probe[c].data, 0xDD, (size_t)alloc_rows * 8, s));
-    for (int c = 0; c < NB; c++) TQ_CUDA(cudaMemsetAsync(p.out_build[c].data, 0xDD, (size_t)alloc_rows * 8, s));
-  }
-  k_init_slabs<<<(P + 1 + 255) / 256, 256, 0, s>>>(off.as<uint32_t>(), cur_b.as<uint32_t>(), lim.as<uint32_t>(), P, (uint32_t)slab, 0u);
-  count_launch();
   ScatterAosParams q{};
   q.sp.n_cols = NP;
-  q.use_tma = g_no_tma ? 0 : 1;
-  for (int c = 0; c < NP; c++) {
-    q.sp.in[c] = probe[c];
-    if ((reinterpret_cast<uintptr_t>(probe[c].data) & 15) != 0) q.use_tma = 0;
-  }
+  for (int c = 0; c < NP; c++) q.sp.in[c] = probe[c];
   if (j->seg.n) {  // regions filled by the peers' push kernels; row counts live on the device
     const int T = scatter_aos_tile(NP, P + 2);
     q.n_segs = j->seg.n;
     q.seg_tiles = (int)((j->seg.cap + T - 1) / T);
     for (int g = 0; g < j->seg.n; g++) {
       q.seg_cnt[g] = j->seg.cnt[g];
-      for (int c = 0; c < NP; c++) {
-        q.seg_in[g][c] = j->seg.col[g][c];
-        if ((reinterpret_cast<uintptr_t>(j->seg.col[g][c]) & 15) != 0) q.use_tma = 0;
-      }
+      for (int c = 0; c < NP; c++) q.seg_in[g][c] = j->seg.col[g][c];
     }
   }
   q.sp.selected = d_selected;
   q.sp.key_col = j->probe_key;
   q.sp.key_mode = j->key_mode;
-  q.sp.is_outer = 0;
   q.sp.pbits = j->pbits;
   q.sp.n = n;
-  q.sp.part_cursor = cur_b.as<uint32_t>();
-  q.sp.part_lim = lim.as<uint32_t>();
   q.sp.overflow = cur + 2;
-  q.out = j->part_aos[slot].as<uint64_t>();
-  TQ_TRY(launch_scatter_aos(q, NP, s));
-  DevBuf dbg;
-  if (g_debug_sums && !j->seg.n) {
-    TQ_TRY(dbg.reserve(64));
-    for (int c = 0; c < NP; c++) {
-      cudaMemsetAsync(dbg.p, 0, 16, s);
-      k_dbg_sum<<<296, 256, 0, s>>>(probe[c].data, n, 1, dbg.as<unsigned long long>());
-      dbg_report("probe input", c, dbg.as<unsigned long long>(), s);
-      cudaMemsetAsync(dbg.p, 0, 16, s);
-      k_dbg_sum_slab<<<P, 256, 0, s>>>(j->part_aos[slot].as<uint64_t>(), off.as<uint32_t>(), cur_b.as<uint32_t>(), P, NP, c, dbg.as<unsigned long long>());
-      dbg_report("slabs after scatter", c, dbg.as<unsigned long long>(), s);
-    }
-  }
+  TQ_TRY(scatter_aos(q, j->part_aos[slot], off, cur_b, lim, s));
   k_part_bases<<<1, PART_BASES_THREADS, 0, s>>>(off.as<uint32_t>(), cur_b.as<uint32_t>(), lim.as<uint32_t>(), P, j->pos_base[slot].as<uint32_t>(), cur + 3);
   count_launch();
   ProbePosParams pp{};
@@ -2141,13 +2093,6 @@ static int32_t launch_probe_stream(tq_join *j, const ProbeParams &p, const std::
   pv.k<<<(unsigned)(P * split), pv.threads, smem, s>>>(pp, j->table);
   count_launch();
   TQ_TRY(check_launch("k_probe_pos"));
-  if (g_debug_sums) {
-    for (int c = 0; c < NP; c++) {
-      cudaMemsetAsync(dbg.p, 0, 16, s);
-      k_dbg_sum_valid<<<296, 256, 0, s>>>(p.out_probe[c].data, pp.valid, cur, dbg.as<unsigned long long>());
-      dbg_report("probe output (valid slots)", c, dbg.as<unsigned long long>(), s);
-    }
-  }
   // holes: the padding of every partition to 32 slots (filled here) + probe rows without a match (finalize_pending)
   k_hole_pads<<<1, HOLE_PAD_THREADS, 0, s>>>(off.as<uint32_t>(), cur_b.as<uint32_t>(), lim.as<uint32_t>(), j->pos_base[slot].as<uint32_t>(), P, cur,
                                             j->hole_pos[slot].as<uint32_t>(), j->hole_src[slot].as<uint32_t>());
@@ -2162,17 +2107,6 @@ static int32_t launch_probe_stream(tq_join *j, const ProbeParams &p, const std::
   count_launch(2);
   j->probe_launches += 3;
   TQ_TRY(check_launch("k_hole_move_pads"));
-  if (g_debug_sums) {
-    unsigned long long h_cur[8];
-    cudaMemcpyAsync(h_cur, cur, 64, cudaMemcpyDeviceToHost, s);
-    cudaStreamSynchronize(s);
-    fprintf(stderr, "[tq debug] probe: M=%llu span=%llu pad_holes=%llu rows_in_slabs=%llu\n", h_cur[0], h_cur[3], h_cur[5], h_cur[6]);
-    for (int c = 0; c < NP; c++) {
-      cudaMemsetAsync(dbg.p, 0, 16, s);
-      k_dbg_sum<<<296, 256, 0, s>>>(p.out_probe[c].data, (int64_t)h_cur[0], 1, dbg.as<unsigned long long>());
-      dbg_report("result probe column [0,M)", c, dbg.as<unsigned long long>(), s);
-    }
-  }
   j->probe_launches += 3;
   return TQ_OK;
 }
@@ -2245,12 +2179,11 @@ static int32_t launch_probe(tq_join *j, const std::vector<DCol> &probe, const ui
     p.tile_state = ts.as<unsigned long long>();
     p.ticket = reinterpret_cast<unsigned *>(ts.as<unsigned long long>() + n_tiles);
   }
-  // The streaming PK-FK pipeline (join_stream.cuh): unique build keys held in the table entries, inner join, no NULL bitmap
-  // on either side, optimistic slabs.  Its result is positional: room for the padding of every partition to 32 rows.
+  // The streaming PK-FK pipeline (join_stream.cuh) when the operator allows it and this batch has no probe NULL bitmap.  Its
+  // result is positional: room for the padding of every partition to 32 rows.
   bool any_in_bm = false;
   for (int c = 0; c < j->n_probe_cols; c++) any_in_bm |= (probe[c].bm != nullptr);
-  const bool pos_path = j->pbits > 0 && j->pbits <= SA_MAX_PBITS && j->row_mode && !p.is_outer && !any_in_bm && !j->build_has_nulls && !g_no_fast_kernel &&
-                        !g_old_fast && j->optimistic_scatter && !g_exact_scatter && j->n_probe_cols <= 4 && j->n_build_cols <= 4 && !j->has_oc;
+  const bool pos_path = stream_probe_ok(j) && !any_in_bm;
   const uint64_t alloc_rows = capacity + (pos_path ? 32ull * ((1ull << j->pbits) + 2) : 0);
   for (int c = 0; c < ncols; c++) {
     TQ_TRY(rb->cols[c].data.reserve((size_t)(alloc_rows ? alloc_rows : 1) * 8));
@@ -2322,11 +2255,10 @@ static int32_t launch_probe(tq_join *j, const std::vector<DCol> &probe, const ui
     sp.n = n;
     sp.part_cnt = cnt.as<uint32_t>();
     sp.part_cursor = cur_b.as<uint32_t>();
-    // Optimistic slabs: hash partitions of a probe batch are near-uniform, so every partition gets a fixed slab of
-    // n/P * 1.25 + 4096 rows and the histogram pass (a full extra read of the key column) is skipped; the scatter
-    // flags a slab that would overflow and finalize_pending re-runs the batch on the exact path.
-    const bool optimistic = j->optimistic_scatter && !g_exact_scatter;
-    const uint64_t slab = (uint64_t)n / P + (uint64_t)n / P / 4 + 4096;
+    // Optimistic slabs: every partition gets a fixed slab (slab_rows) and the histogram pass (a full extra read of the key
+    // column) is skipped; the scatter flags a slab that would overflow and finalize_pending re-runs the batch on the exact path.
+    const bool optimistic = j->optimistic_scatter;
+    const uint64_t slab = slab_rows(n, P, false);
     const uint64_t part_rows = optimistic ? slab * P + (p.is_outer ? (uint64_t)n : 0) : (uint64_t)n;
     if (part_rows > 0xFFFFFFF0ull) { set_error("probe batch too large for 32-bit partition offsets"); return TQ_ERR_INVALID_ARG; }
     for (int c = 0; c < j->n_probe_cols; c++) {
@@ -2370,8 +2302,6 @@ static int32_t launch_probe(tq_join *j, const std::vector<DCol> &probe, const ui
     }
     const int64_t scat_tiles = (n + SCAT_TILE - 1) / SCAT_TILE;
     const int64_t scat_cap = (int64_t)rt().sm_count * 4;
-    bool any_in_bm = false;
-    for (int c = 0; c < j->n_probe_cols; c++) any_in_bm |= (probe[c].bm != nullptr);
     ScatterKernel sfast = (!any_in_bm && !g_no_fast_kernel) ? scatter_fast_kernel(j->n_probe_cols) : nullptr;
     if (sfast) {
       static bool sattr[5] = {};
@@ -2695,11 +2625,7 @@ int32_t tq_join_create(const tq_join_desc *d, tq_join **out) {
   // LeftOuter keeps the left child as the outer side, RightOuter the right child (builder.go:451-477)
   if (d->join_type == TQ_JOIN_LEFT_OUTER && d->outer_is_right) { set_error("left outer join needs outer_is_right == 0"); return TQ_ERR_INVALID_ARG; }
   if (d->join_type == TQ_JOIN_RIGHT_OUTER && !d->outer_is_right) { set_error("right outer join needs outer_is_right == 1"); return TQ_ERR_INVALID_ARG; }
-  { const char *e = getenv("TQ_JOIN_FORCE_GLOBAL"); g_force_global_table = e && e[0] == '1'; }
   { const char *e = getenv("TQ_JOIN_NO_FAST"); g_no_fast_kernel = e && e[0] == '1'; }
-  { const char *e = getenv("TQ_JOIN_NO_TMA"); g_no_tma = e && e[0] == '1'; }
-  { const char *e = getenv("TQ_JOIN_DEBUG_SUMS"); g_debug_sums = e && e[0] == '1'; }
-  { const char *e = getenv("TQ_JOIN_EXACT_SCATTER"); g_exact_scatter = e && e[0] == '1'; }
   { const char *e = getenv("TQ_JOIN_PART_ROWS"); if (e && atoll(e) > 0) g_part_target_rows = atoll(e); }
   tq_join *j = new (std::nothrow) tq_join();
   if (!j) return TQ_ERR_OOM;
@@ -3070,9 +2996,9 @@ int32_t tq_join_put_probe_segments(tq_join *j, int32_t n_segs, const tq_column *
   TQ_TRY(ensure_init());
   if (j->state != tq_join::PROBING) { set_error("put_probe before finalize_build"); return TQ_ERR_STATE; }
   if (j->probe_eof) { set_error("put_probe after probe_eof"); return TQ_ERR_STATE; }
-  const bool eligible = j->pbits > 0 && j->pbits <= SA_MAX_PBITS && j->row_mode && j->join_type == TQ_JOIN_INNER && !j->build_has_nulls && !j->key_hidden &&
-                        !j->any_ind && !j->has_oc && j->n_probe_cols <= 4 && j->n_build_cols <= 4 && j->optimistic_scatter && !g_no_fast_kernel && !g_old_fast;
-  if (!eligible) {
+  // segmented input can only run the streaming path (k_scatter_aos alone reads the regions), and it has no pass that would
+  // encode a hidden key column or FLOAT / var-len columns
+  if (!stream_probe_ok(j) || j->key_hidden || j->any_ind) {
     set_error("segmented probe batches need the streaming PK-FK path (inner join, unique NOT NULL build side >= 2^18 rows, <= 4 columns per side)");
     return TQ_ERR_UNSUPPORTED_TYPE;
   }

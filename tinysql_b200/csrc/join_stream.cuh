@@ -274,11 +274,9 @@ static ScatterAosKernel scatter_aos_kernel_t(int nc) {
   }
   return nullptr;
 }
-// tile size: TQ_JOIN_SCATTER_TILE (1024 / 2048 / 4096) if its shared-memory image fits an SM, else the next smaller one
+// tile size: 2048 rows if that shared-memory image fits an SM, else 1024
 static int scatter_aos_tile(int nc, int bins) {
-  if (g_scatter_tile >= 4096 && sa_smem_bytes<4096>(nc, bins) <= 220 * 1024) return 4096;
-  if (g_scatter_tile >= 2048 && sa_smem_bytes<2048>(nc, bins) <= 220 * 1024) return 2048;
-  return 1024;
+  return sa_smem_bytes<2048>(nc, bins) <= 220 * 1024 ? 2048 : 1024;
 }
 static int32_t launch_scatter_aos(const ScatterAosParams &q, int nc, cudaStream_t s) {
   const int bins = scatter_bins(q.sp) + 1;
@@ -286,8 +284,7 @@ static int32_t launch_scatter_aos(const ScatterAosParams &q, int nc, cudaStream_
   const bool plain = !q.sp.selected && q.sp.key_mode == KEYMODE_RAW;
   ScatterAosKernel k;
   int smem, per_sm;
-  if (T == 4096) { k = plain ? scatter_aos_kernel_t<4096, true>(nc) : scatter_aos_kernel_t<4096, false>(nc); smem = sa_smem_bytes<4096>(nc, bins); per_sm = sa_occ<4096>(nc); }
-  else if (T == 2048) { k = plain ? scatter_aos_kernel_t<2048, true>(nc) : scatter_aos_kernel_t<2048, false>(nc); smem = sa_smem_bytes<2048>(nc, bins); per_sm = sa_occ<2048>(nc); }
+  if (T == 2048) { k = plain ? scatter_aos_kernel_t<2048, true>(nc) : scatter_aos_kernel_t<2048, false>(nc); smem = sa_smem_bytes<2048>(nc, bins); per_sm = sa_occ<2048>(nc); }
   else { k = plain ? scatter_aos_kernel_t<1024, true>(nc) : scatter_aos_kernel_t<1024, false>(nc); smem = sa_smem_bytes<1024>(nc, bins); per_sm = sa_occ<1024>(nc); }
   if (!k || smem > 227 * 1024) { set_error("internal: AoS scatter of %d columns into %d bins does not fit shared memory", nc, bins); return TQ_ERR_INVALID_ARG; }
   TQ_CUDA(cudaFuncSetAttribute(k, cudaFuncAttributeMaxDynamicSharedMemorySize, smem));
