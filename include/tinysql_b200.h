@@ -290,10 +290,38 @@ typedef struct tq_join tq_join;
 
 int32_t tq_join_create(const tq_join_desc *desc, tq_join **out);
 /* OtherConditions of the joiners (executor/joiner.go:155-167: baseJoiner.filter over the joined rows; an outer row whose
- * joined rows all fail is emitted once with a NULL inner side).  Each condition compares output column lhs_col (index
- * into lhs ++ rhs) with output column rhs_col, or with the constant when rhs_col < 0: BIGINT with BIGINT (any sign mix)
- * or DOUBLE with DOUBLE; all conditions are ANDed.  Call once, right after tq_join_create.  EXPERIMENTAL in round 1
- * (see DESIGN.md): general expressions stay with the shim, which filters the returned chunk with tq_vec_*. */
+ * joined rows all fail is emitted once with a NULL / defaultInner inner side).  Two forms, one per handle:
+ *
+ * tq_join_set_other_conditions: each condition compares output column lhs_col (index into lhs ++ rhs) with output column
+ * rhs_col, or with the constant when rhs_col < 0: BIGINT with BIGINT (any sign mix) or DOUBLE with DOUBLE; all conditions
+ * are ANDed, a NULL operand fails.  At most 8 conditions.  The library runs them as the program below (one CMP + FILTER
+ * item per condition).
+ *
+ * tq_join_set_other_program: the conditions as a tq_expr_op program over the joined row (left ++ right).  Input register
+ * k = output column input_cols[k], which must be an INT64 / UINT64 / FLOAT64 column.  ops: kinds TQ_X_CONST .. TQ_X_FILTER
+ * (no TQ_X_COMPACT), at least one TQ_X_FILTER, with the operand rules of tq_expr_eval.  A joined row passes iff every
+ * FILTER item selects it.
+ *
+ * Rules.  Call either setter once, right after tq_join_create; a handle that has conditions of one form answers a call
+ * for the other with TQ_ERR_STATE.  A malformed program (a bad register or operator, TQ_X_COMPACT, no FILTER, more than
+ * TQ_EXPR_MAX_INPUTS inputs or TQ_EXPR_MAX_OPS ops) is TQ_ERR_INVALID_ARG, an input column of type FLOAT or var-len
+ * TQ_ERR_UNSUPPORTED_TYPE; both before any device work.
+ *
+ * Semantics (joiner.go:155-167,225-340).
+ *  - Inner join: a joined row survives iff the conditions select it.
+ *  - Outer join: a probe row with key matches none of which passes is emitted once as its miss row, defaultInner on the
+ *    inner side, at the position of one of its failed joined rows.
+ *  - The conditions never run for probe rows without a key match, with a NULL key or with selected[i] == 0: the reference
+ *    returns before filter when inners.Len() == 0 (joiner.go:225-228,288-291).  Such rows raise no error and no warning.
+ *  - Errors: a joined row in the evaluation set (tq_expr_eval's narrowing: a row an earlier FILTER item dropped does not
+ *    raise) that overflows makes the call that would deliver its batch return TQ_ERR_OVERFLOW_BIGINT / _UNSIGNED /
+ *    _DOUBLE — tq_join_next, tq_join_next_device or tq_join_next_bytes, whichever takes up the batch.  After that the
+ *    handle only supports tq_join_destroy.  The reference reports the first error in its per-chunk order; here any in-set
+ *    row of the batch may be the one reported (DESIGN.md §3).
+ *  - Result order is unchanged: compaction is stable, so the one-table path (build side below 2^18 rows) still yields
+ *    (probe row ascending, build insertion ascending).
+ * tq_join_warnings: division-by-zero warnings raised so far by joined rows in the evaluation set (handleDivisionByZeroError,
+ * builtin_arithmetic_vec.go:369-375), counted as their batches are finished. */
 typedef struct tq_join_cond {
   int32_t op;         /* TQ_CMP_*                                   */
   int32_t lhs_col;    /* output column                              */
@@ -302,6 +330,8 @@ typedef struct tq_join_cond {
   uint64_t const_bits;
 } tq_join_cond;
 int32_t tq_join_set_other_conditions(tq_join *j, int32_t n_conds, const tq_join_cond *conds);
+int32_t tq_join_set_other_program(tq_join *j, int32_t n_inputs, const int32_t *input_cols, int32_t n_ops, const tq_expr_op *ops);
+int32_t tq_join_warnings(tq_join *j, int64_t *div_by_zero);
 int32_t tq_join_put_build(tq_join *j, const tq_column *cols, int32_t mem);
 int32_t tq_join_finalize_build(tq_join *j);
 /* selected: outerSideFilter result (join.go:328), n bytes of 0/1 in HOST memory, or NULL = all selected. */
@@ -487,10 +517,16 @@ typedef struct tq_mjoin_desc {
 } tq_mjoin_desc;
 typedef struct tq_mjoin tq_mjoin;
 int32_t tq_mjoin_create(const tq_mjoin_desc *desc, tq_mjoin **out);
-/* OtherConditions of the joiner (baseJoiner.filter, joiner.go:155-167; tryToMatchInners in merge_join.go:290-305): the same
- * tq_join_cond comparisons tq_join_set_other_conditions takes, over the joined row left ++ right; an outer row whose joined rows
- * all fail takes the miss path.  Call once, right after tq_mjoin_create. */
+/* OtherConditions of the joiner (baseJoiner.filter, joiner.go:155-167; tryToMatchInners in merge_join.go:290-305): the two forms
+ * of the hash join (tq_join_cond comparisons or a tq_expr_op program), over the joined row left ++ right, with the same rules
+ * and semantics; an outer row whose joined rows all fail takes the miss path, in its place in the output.  Set them right
+ * after tq_mjoin_create; the comparison list may be set again, the program once.  The result is computed by
+ * tq_mjoin_finish; an overflow of an in-set joined row is returned by every tq_mjoin_next / _next_device / _next_bytes
+ * call after it.  The output order stays exactly the reference's. */
 int32_t tq_mjoin_set_other_conditions(tq_mjoin *j, int32_t n_conds, const tq_join_cond *conds);
+int32_t tq_mjoin_set_other_program(tq_mjoin *j, int32_t n_inputs, const int32_t *input_cols, int32_t n_ops, const tq_expr_op *ops);
+/* division-by-zero warnings raised by joined rows in the evaluation set (handleDivisionByZeroError, builtin_arithmetic_vec.go:369-375) */
+int32_t tq_mjoin_warnings(tq_mjoin *j, int64_t *div_by_zero);
 /* host chunks (all layouts) or, for 8-byte column types, device chunks (TQ_MEM_DEVICE) — per child one or the other */
 int32_t tq_mjoin_put_inner(tq_mjoin *j, const tq_column *cols, int32_t mem);
 int32_t tq_mjoin_put_outer(tq_mjoin *j, const tq_column *cols, const uint8_t *selected, int32_t mem); /* selected: HOST Go []bool or NULL */

@@ -25,6 +25,7 @@ import (
 	"github.com/pingcap/tidb/expression"
 	"github.com/pingcap/tidb/parser/mysql"
 	plannercore "github.com/pingcap/tidb/planner/core"
+	"github.com/pingcap/tidb/sessionctx"
 	"github.com/pingcap/tidb/types"
 	"github.com/pingcap/tidb/util/chunk"
 )
@@ -52,7 +53,7 @@ type GPUHashJoinExec struct {
 	outerSideExec, innerSideExec Executor
 	outerSideFilter              expression.CNFExprs
 	outerKeys, innerKeys         []*expression.Column
-	otherConditions              expression.CNFExprs // comparisons go to tq_join_set_other_conditions; see Open / Next
+	otherConditions              expression.CNFExprs // run inside the library (setOtherConditions); what is left: see Next
 	defaultValues                []types.Datum       // PhysicalHashJoin.DefaultValues (builder.go:449)
 	joinType                     plannercore.JoinType
 	outerIsRight                 bool
@@ -69,6 +70,7 @@ type GPUHashJoinExec struct {
 	sizes     *C.int64_t
 	prepared  bool
 	outerDone bool
+	warned    int64 // division-by-zero warnings of the OtherConditions program already in the statement context
 }
 
 // cInt32s builds an int32 array in C memory (a tq_join_desc in C memory may only point at C memory).
@@ -113,19 +115,19 @@ func (e *GPUHashJoinExec) Open(ctx context.Context) error {
 	if st := C.tq_join_create(d, &e.h); st != C.TQ_OK {
 		return chunk.StatusError(int32(st))
 	}
-	// OtherConditions (joiner.go:155-167): conjunctions of column-vs-column / column-vs-constant comparisons run inside the
-	// library (also for outer joins: a probe row whose joined rows all fail becomes a miss row); any other expression of an
-	// INNER join is evaluated with the tq_vec_* builtins on the returned chunk in Next.  An OUTER join with a condition the
-	// library cannot take fails here — there is no Go-executor fallback.
-	if conds, rest, ok := asJoinConds(e.otherConditions, e.outerIsRight, np, nb); ok && len(conds) > 0 {
-		cc := (*C.tq_join_cond)(C.malloc(C.size_t(len(conds)) * C.size_t(unsafe.Sizeof(C.tq_join_cond{}))))
-		defer C.free(unsafe.Pointer(cc))
-		copy((*[1 << 10]C.tq_join_cond)(unsafe.Pointer(cc))[:len(conds)], conds)
-		if st := C.tq_join_set_other_conditions(e.h, C.int32_t(len(conds)), cc); st != C.TQ_OK {
-			return chunk.StatusError(int32(st))
-		}
-		e.otherConditions = rest
+	// OtherConditions (joiner.go:155-167) run inside the library, for outer joins too (a probe row whose joined rows all fail
+	// becomes a miss row): see setOtherConditions.  Only trees that do not lower (string operands, ...) are left; for an
+	// INNER join Next evaluates them with the tq_vec_* builtins on the returned chunk, an OUTER join fails here — there is no
+	// Go-executor fallback.
+	rest, err := setOtherConditions(e.otherConditions, e.outerIsRight, np, nb,
+		func(n C.int32_t, cc *C.tq_join_cond) C.int32_t { return C.tq_join_set_other_conditions(e.h, n, cc) },
+		func(nIn C.int32_t, in *C.int32_t, nOps C.int32_t, ops *C.tq_expr_op) C.int32_t {
+			return C.tq_join_set_other_program(e.h, nIn, in, nOps, ops)
+		})
+	if err != nil {
+		return err
 	}
+	e.otherConditions = rest
 	if len(e.otherConditions) > 0 && e.joinType != plannercore.InnerJoin {
 		return errors.New("tinysql_b200: this OtherCondition of an outer hash join is not supported on the device path")
 	}
@@ -142,7 +144,7 @@ func (e *GPUHashJoinExec) Open(ctx context.Context) error {
 	e.outViews = chunk.NewCViewSet(len(e.outTypes))
 	e.sizes = (*C.int64_t)(C.calloc(C.size_t(len(e.outTypes)), 8))
 	e.innerChk, e.outerChk = newFirstChunk(e.innerSideExec), newFirstChunk(e.outerSideExec)
-	e.prepared, e.outerDone = false, false
+	e.prepared, e.outerDone, e.warned = false, false, 0
 	return nil
 }
 
@@ -203,6 +205,9 @@ func (e *GPUHashJoinExec) Next(ctx context.Context, req *chunk.Chunk) error {
 		if st != C.TQ_OK {
 			return chunk.StatusError(int32(st))
 		}
+		var warned C.int64_t
+		C.tq_join_warnings(e.h, &warned)
+		appendDivByZeroWarnings(e.ctx, int64(warned), &e.warned)
 		if n > 0 || eof != 0 {
 			for i := range e.outTypes {
 				e.outViews.CopyBack(i, req.Column(i), int(n))
@@ -303,6 +308,48 @@ func datumBits(d *types.Datum, ft *types.FieldType) uint64 {
 		return math.Float64bits(d.GetFloat64())
 	}
 	return uint64(d.GetInt64())
+}
+
+// setOtherConditions hands a join's OtherConditions to the library and returns what it could not take.  A CNF made only of
+// comparisons asJoinConds recognises goes to the comparison setter.  Otherwise, if CompileProgram lowers every item, the WHOLE
+// CNF goes to the program setter (one form per handle).  Otherwise the comparisons go to the comparison setter and the rest is
+// returned.  Column.Index of an OtherCondition is already an index into the joined row lhs ++ rhs, the program's input space.
+func setOtherConditions(conds expression.CNFExprs, outerIsRight bool, nOuter, nInner int, setConds func(C.int32_t, *C.tq_join_cond) C.int32_t,
+	setProgram func(C.int32_t, *C.int32_t, C.int32_t, *C.tq_expr_op) C.int32_t) (expression.CNFExprs, error) {
+	if len(conds) == 0 {
+		return nil, nil
+	}
+	cmps, rest, _ := asJoinConds(conds, outerIsRight, nOuter, nInner)
+	if len(rest) > 0 {
+		if prog, lowered := expression.CompileProgram(conds, nil); lowered {
+			defer prog.Free()
+			inputs, ops, nOps := prog.JoinArgs()
+			in := cInt32s(len(inputs), func(i int) C.int32_t { return C.int32_t(inputs[i]) })
+			defer C.free(unsafe.Pointer(in))
+			if st := setProgram(C.int32_t(len(inputs)), in, C.int32_t(nOps), (*C.tq_expr_op)(ops)); st != C.TQ_OK {
+				return nil, chunk.StatusError(int32(st))
+			}
+			return nil, nil
+		}
+	}
+	if len(cmps) > 0 {
+		cc := (*C.tq_join_cond)(C.malloc(C.size_t(len(cmps)) * C.size_t(unsafe.Sizeof(C.tq_join_cond{}))))
+		defer C.free(unsafe.Pointer(cc))
+		copy((*[1 << 10]C.tq_join_cond)(unsafe.Pointer(cc))[:len(cmps)], cmps)
+		if st := setConds(C.int32_t(len(cmps)), cc); st != C.TQ_OK {
+			return nil, chunk.StatusError(int32(st))
+		}
+	}
+	return rest, nil
+}
+
+// appendDivByZeroWarnings adds the warnings a join's condition program raised since the last call to the statement context,
+// one expression.ErrDivisionByZero each, as handleDivisionByZeroError does in a SELECT (expression/errors.go:65-77).
+func appendDivByZeroWarnings(ctx sessionctx.Context, total int64, seen *int64) {
+	sc := ctx.GetSessionVars().StmtCtx
+	for ; *seen < total; *seen++ {
+		sc.AppendWarning(expression.ErrDivisionByZero)
+	}
 }
 
 // asJoinConds splits OtherConditions into the comparisons tq_join_set_other_conditions takes — `col op col` / `col op const`

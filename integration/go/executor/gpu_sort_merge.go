@@ -16,6 +16,7 @@ import "C"
 
 import (
 	"context"
+	"errors"
 	"unsafe"
 
 	"github.com/pingcap/tidb/expression"
@@ -164,7 +165,7 @@ type GPUMergeJoinExec struct {
 	outerKeys     []*expression.Column
 	innerKeys     []*expression.Column
 	outerFilter   expression.CNFExprs
-	otherConditions expression.CNFExprs
+	otherConditions expression.CNFExprs // run inside the library (setOtherConditions, gpu_join.go); what is left: see Next
 	defaultValues []types.Datum // PhysicalMergeJoin.DefaultValues -> defaultInner (joiner.go:139-143)
 
 	h        *C.tq_mjoin
@@ -173,12 +174,14 @@ type GPUMergeJoinExec struct {
 	chk      [2]*chunk.Chunk
 	selected []bool
 	selBytes []byte
+	filtered []bool
 	pump     resultPump
 }
 
-// Open implements Executor (merge_join.go:185-198).  OtherConditions that asJoinConds (gpu_join.go) can lower — comparisons of
-// fixed-width columns / constants — are handed to tq_mjoin_set_other_conditions; buildMergeJoin keeps the rest in a SelectionExec
-// above an inner join.
+// Open implements Executor (merge_join.go:185-198).  OtherConditions go to the library as the hash join hands them over
+// (setOtherConditions, gpu_join.go): comparisons to tq_mjoin_set_other_conditions, any CNF CompileProgram lowers to
+// tq_mjoin_set_other_program, for outer joins too.  Trees that do not lower stay with Next for an inner join; an outer join
+// with such a condition fails here.
 func (e *GPUMergeJoinExec) Open(ctx context.Context) error {
 	if err := e.baseExecutor.Open(ctx); err != nil {
 		return err
@@ -216,13 +219,17 @@ func (e *GPUMergeJoinExec) Open(ctx context.Context) error {
 	if st := C.tq_mjoin_create(d, &e.h); st != C.TQ_OK {
 		return chunk.StatusError(int32(st))
 	}
-	if conds, _, ok := asJoinConds(e.otherConditions, e.outerIdx == 1, len(oft), len(ift)); ok && len(conds) > 0 {
-		cc := (*[1 << 6]C.tq_join_cond)(C.calloc(C.size_t(len(conds)), C.sizeof_tq_join_cond))
-		defer C.free(unsafe.Pointer(cc))
-		copy(cc[:len(conds)], conds)
-		if st := C.tq_mjoin_set_other_conditions(e.h, C.int32_t(len(conds)), &cc[0]); st != C.TQ_OK {
-			return chunk.StatusError(int32(st))
-		}
+	rest, err := setOtherConditions(e.otherConditions, e.outerIdx == 1, len(oft), len(ift),
+		func(n C.int32_t, cc *C.tq_join_cond) C.int32_t { return C.tq_mjoin_set_other_conditions(e.h, n, cc) },
+		func(nIn C.int32_t, in *C.int32_t, nOps C.int32_t, ops *C.tq_expr_op) C.int32_t {
+			return C.tq_mjoin_set_other_program(e.h, nIn, in, nOps, ops)
+		})
+	if err != nil {
+		return err
+	}
+	e.otherConditions = rest
+	if len(e.otherConditions) > 0 && e.joinType != plannercore.InnerJoin {
+		return errors.New("tinysql_b200: this OtherCondition of an outer merge join is not supported on the device path")
 	}
 	e.prepared = false
 	e.chk = [2]*chunk.Chunk{newFirstChunk(inner), newFirstChunk(outer)}
@@ -283,10 +290,32 @@ func (e *GPUMergeJoinExec) Next(ctx context.Context, req *chunk.Chunk) error {
 			return chunk.StatusError(int32(st))
 		}
 		e.prepared = true
+		var warned C.int64_t
+		C.tq_mjoin_warnings(e.h, &warned)
+		var seen int64
+		appendDivByZeroWarnings(e.ctx, int64(warned), &seen)
 	}
-	return e.pump.fill(req,
-		func(want C.int64_t, sizes *C.int64_t) C.int32_t { return C.tq_mjoin_next_bytes(e.h, want, sizes) },
-		func(want C.int64_t, out *C.tq_column, n *C.int64_t, eof *C.int32_t) C.int32_t { return C.tq_mjoin_next(e.h, want, out, n, eof) })
+	for {
+		// an overflow of the OtherConditions program comes back from tq_mjoin_next_bytes / tq_mjoin_next
+		if err := e.pump.fill(req,
+			func(want C.int64_t, sizes *C.int64_t) C.int32_t { return C.tq_mjoin_next_bytes(e.h, want, sizes) },
+			func(want C.int64_t, out *C.tq_column, n *C.int64_t, eof *C.int32_t) C.int32_t { return C.tq_mjoin_next(e.h, want, out, n, eof) }); err != nil {
+			return err
+		}
+		if req.NumRows() == 0 || len(e.otherConditions) == 0 {
+			return nil
+		}
+		// inner joins only (Open rejected the outer case): baseJoiner.filter (joiner.go:155-167) on the returned chunk
+		var err error
+		if e.filtered, err = expression.VectorizedFilter(e.ctx, e.otherConditions, chunk.NewIterator4Chunk(req), e.filtered); err != nil {
+			return err
+		}
+		req.SetSel(selToIdx(e.filtered))
+		if req.NumRows() > 0 {
+			return nil
+		}
+		req.Reset()
+	}
 }
 
 // Close implements Executor (merge_join.go:178-182).

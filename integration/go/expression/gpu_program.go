@@ -274,6 +274,13 @@ func (p *GPUProgram) Run(input *chunk.Chunk, results []*chunk.Column, selected [
 	return selected, int64(warnings), nil // warnings: one handleDivisionByZeroError call each (builtin_arithmetic_vec.go:369-375)
 }
 
+// JoinArgs hands a filter-only program to tq_join_set_other_program / tq_mjoin_set_other_program: the column each input
+// register reads (an index into the joined row left ++ right when the filters are a join's OtherConditions) and the op
+// array in C memory (a *C.tq_expr_op of the caller's package; cgo types do not cross packages).
+func (p *GPUProgram) JoinArgs() (inputs []int, ops unsafe.Pointer, nOps int) {
+	return p.inputs, unsafe.Pointer(p.ops), p.nOps
+}
+
 // Free releases the C memory of the program.
 func (p *GPUProgram) Free() {
 	C.free(unsafe.Pointer(p.ops))

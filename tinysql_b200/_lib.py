@@ -101,6 +101,8 @@ SYMBOLS = {
     "tq_chunk_decode": (_I32, [_P, _I64, _I32, C.POINTER(_I32), _COL, C.POINTER(_I64)]),
     "tq_join_create": (_I32, [C.POINTER(TQJoinDesc), C.POINTER(_P)]),
     "tq_join_set_other_conditions": (_I32, [_P, _I32, C.POINTER(TQJoinCond)]),
+    "tq_join_set_other_program": (_I32, [_P, _I32, C.POINTER(_I32), _I32, C.POINTER(TQExprOp)]),
+    "tq_join_warnings": (_I32, [_P, C.POINTER(_I64)]),
     "tq_join_put_build": (_I32, [_P, _COL, _I32]), "tq_join_finalize_build": (_I32, [_P]),
     "tq_join_put_probe": (_I32, [_P, _COL, _P, _I32]), "tq_join_probe_eof": (_I32, [_P]),
     "tq_join_put_probe_segments": (_I32, [_P, _I32, _COL, C.POINTER(_P), _I64]),
@@ -131,6 +133,8 @@ SYMBOLS = {
     "tq_sort_destroy": (_I32, [_P]),
     "tq_mjoin_create": (_I32, [C.POINTER(TQMJoinDesc), C.POINTER(_P)]),
     "tq_mjoin_set_other_conditions": (_I32, [_P, _I32, C.POINTER(TQJoinCond)]),
+    "tq_mjoin_set_other_program": (_I32, [_P, _I32, C.POINTER(_I32), _I32, C.POINTER(TQExprOp)]),
+    "tq_mjoin_warnings": (_I32, [_P, C.POINTER(_I64)]),
     "tq_mjoin_put_inner": (_I32, [_P, _COL, _I32]),
     "tq_mjoin_put_outer": (_I32, [_P, _COL, _P, _I32]),
     "tq_mjoin_finish": (_I32, [_P]),

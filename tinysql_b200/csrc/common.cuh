@@ -18,6 +18,11 @@
 #ifndef TQ_LAUNCH
 #define TQ_LAUNCH(kernel, grid, block, smem, stream, ...) kernel<<<(grid), (block), (smem), (stream)>>>(__VA_ARGS__)
 #endif
+// A kernel parameter whose address is taken (sort.cu: k_mj_prog) is declared __grid_constant__ so that it stays in the
+// parameter space; the emulation build has no such qualifier and takes the parameter by value.
+#ifndef __grid_constant__
+#define __grid_constant__
+#endif
 
 namespace tq {
 

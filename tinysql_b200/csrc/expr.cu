@@ -2,12 +2,10 @@
 // and their C-ABI.  All kernels are HBM-streaming maps: 128-bit coalesced loads of the operand
 // columns, null-bitmap words assembled with warp REDUX, 128-bit stores of the result column.
 // No tensor cores: nothing here is a contraction.
-#include <cfloat>
-#include <cmath>
 #include <cstring>
 #include <cstdint>
 
-#include "common.cuh"
+#include "expr_prog.cuh"
 
 namespace tq {
 
@@ -15,8 +13,6 @@ static constexpr int MAP_THREADS = 256;
 static constexpr int MAP_UNROLL = 4;        // independent 64-row groups in flight per warp
 static constexpr int MAX_IN_LIST = 32;
 static constexpr int64_t SLAB_ROWS = 1 << 22;  // host-path slab: 4M rows = 32 MiB per column
-
-enum : unsigned { ERR_BIGINT = 1u, ERR_UBIGINT = 2u, ERR_DOUBLE = 4u };
 
 template <int NIN> struct InCols {
   const uint64_t *d[NIN];
@@ -99,184 +95,7 @@ __global__ void __launch_bounds__(MAP_THREADS) k_map(InCols<NIN> in, OutCols<NOU
   }
 }
 
-// ------------------------------------------------------------------ functors
-__device__ __forceinline__ int cmp_int_dev(bool ua, bool ub, int64_t x, int64_t y) {
-  // types.VecCompare{UU,II,UI,IU}  types/compare.go:44-100
-  if (ua && ub) { uint64_t a = (uint64_t)x, b = (uint64_t)y; return a < b ? -1 : (a == b ? 0 : 1); }
-  if (!ua && !ub) return x < y ? -1 : (x == y ? 0 : 1);
-  if (ua) { if (y < 0 || x < 0) return 1; return x < y ? -1 : (x == y ? 0 : 1); }   // x<0 <=> uint64(x) > MaxInt64
-  if (x < 0 || y < 0) return -1;
-  return x < y ? -1 : (x == y ? 0 : 1);
-}
-__device__ __forceinline__ uint64_t cmp_res_dev(int op, int c) {
-  // vecResOf{LT,LE,GT,GE,EQ,NE}  expression/builtin_compare_vec.go:214-279
-  switch (op) {
-    case TQ_CMP_LT: return c < 0;
-    case TQ_CMP_LE: return c <= 0;
-    case TQ_CMP_GT: return c > 0;
-    case TQ_CMP_GE: return c >= 0;
-    case TQ_CMP_EQ: return c == 0;
-    default: return c != 0;
-  }
-}
-
-struct FCompareInt {
-  int op; bool ua, ub;
-  __device__ __forceinline__ void operator()(const uint64_t (&v)[2], const bool (&nn)[2], uint64_t (&o)[1], bool (&onn)[1],
-                                             unsigned &, unsigned &, bool) const {
-    o[0] = cmp_res_dev(op, cmp_int_dev(ua, ub, (int64_t)v[0], (int64_t)v[1]));
-    onn[0] = nn[0] && nn[1];  // result.MergeNulls(buf0, buf1)
-  }
-};
-struct FCompareReal {
-  int op;
-  __device__ __forceinline__ void operator()(const uint64_t (&v)[2], const bool (&nn)[2], uint64_t (&o)[1], bool (&onn)[1],
-                                             unsigned &, unsigned &, bool) const {
-    onn[0] = nn[0] && nn[1];
-    const double x = __longlong_as_double((long long)v[0]), y = __longlong_as_double((long long)v[1]);
-    const int c = x < y ? -1 : (x == y ? 0 : 1);  // types.CompareFloat64
-    o[0] = onn[0] ? cmp_res_dev(op, c) : 0;
-  }
-};
-
-// signed overflow predicates written on unsigned words (no UB, no 64-bit division)
-__device__ __forceinline__ bool add_overflows_ss(int64_t a, int64_t b) {
-  // (lh > 0 && rh > MaxInt64-lh) || (lh < 0 && rh < MinInt64-lh)  builtin_arithmetic_vec.go:488
-  const int64_t s = (int64_t)((uint64_t)a + (uint64_t)b);
-  return ((a ^ s) & (b ^ s)) < 0;
-}
-__device__ __forceinline__ int64_t wneg(int64_t x) { return (int64_t)(0ull - (uint64_t)x); }  // Go's wrapping -x
-
-struct FArithInt {
-  int op; bool ua, ub;
-  __device__ __forceinline__ void operator()(const uint64_t (&v)[2], const bool (&nn)[2], uint64_t (&o)[1], bool (&onn)[1],
-                                             unsigned &err, unsigned &, bool) const {
-    onn[0] = nn[0] && nn[1];
-    o[0] = 0;
-    if (!onn[0]) return;  // `if result.IsNull(i) { continue }`
-    const int64_t lh = (int64_t)v[0], rh = (int64_t)v[1];
-    const uint64_t ul = v[0], ur = v[1];
-    if (op == TQ_ARITH_PLUS) {
-      if (ua && ub) { if (ul > ~0ull - ur) err |= ERR_UBIGINT; }                                        // plusUU :437
-      else if (ua && !ub) {                                                                              // plusUS :448-459 (verbatim, lh twice)
-        if (rh < 0 && (uint64_t)wneg(rh) > ul) err |= ERR_UBIGINT;
-        if (rh > 0 && ul > ~0ull - ul) err |= ERR_UBIGINT;
-      } else if (!ua && ub) {                                                                            // plusSU :464-476
-        if (lh < 0 && (uint64_t)wneg(lh) > ur) err |= ERR_UBIGINT;
-        if (lh > 0 && ur > ~0ull - ul) err |= ERR_UBIGINT;
-      } else if (add_overflows_ss(lh, rh)) err |= ERR_BIGINT;                                            // plusSS :488
-      o[0] = ul + ur;
-    } else if (op == TQ_ARITH_MINUS) {
-      if (ua && ub) { if (ul < ur) err |= ERR_UBIGINT; }                                                 // minusUU :208
-      else if (ua && !ub) {                                                                              // minusUS :224-229
-        if (rh >= 0 && ul < ur) err |= ERR_UBIGINT;
-        if (rh < 0 && ul > ~0ull - (uint64_t)wneg(rh)) err |= ERR_UBIGINT;
-      } else if (!ua && ub) {                                                                            // minusSU :245
-        if ((ul - 0x8000000000000000ull) < ur) err |= ERR_UBIGINT;
-      } else {                                                                                           // minusSS :260 (verbatim, with Go's wrapping -rh)
-        const int64_t nr = wneg(rh);
-        const int64_t max_minus = (int64_t)(0x7fffffffffffffffull - ul);
-        const int64_t min_minus = (int64_t)(0x8000000000000000ull - ul);
-        if ((lh > 0 && nr > max_minus) || (lh < 0 && nr < min_minus)) err |= ERR_BIGINT;
-      }
-      o[0] = ul - ur;
-    } else {
-      const uint64_t lo = ul * ur;
-      if (ua || ub) {                                                                                    // MultiplyIntUnsigned :521-529 (either side unsigned: builtin_arithmetic.go:344-348)
-        if (__umul64hi(ul, ur) != 0) err |= ERR_UBIGINT;
-      } else {                                                                                           // MultiplyInt :332-338
-        // `x != 0 && tmp/x != y` with Go's wrapping quotient: a true overflow is missed exactly when
-        // x == -1 and y == MinInt64 (tmp == MinInt64, MinInt64 / -1 wraps back to MinInt64 == y).
-        const int64_t hi = __mul64hi(lh, rh);
-        const bool true_ovf = hi != ((int64_t)lo >> 63);
-        if (true_ovf && !(lh == -1 && ur == 0x8000000000000000ull)) err |= ERR_BIGINT;
-      }
-      o[0] = lo;
-    }
-  }
-};
-
-struct FArithReal {
-  int op;
-  __device__ __forceinline__ void operator()(const uint64_t (&v)[2], const bool (&nn)[2], uint64_t (&o)[1], bool (&onn)[1],
-                                             unsigned &err, unsigned &cnt, bool) const {
-    onn[0] = nn[0] && nn[1];
-    o[0] = 0;
-    if (!onn[0]) return;
-    const double x = __longlong_as_double((long long)v[0]), y = __longlong_as_double((long long)v[1]);
-    double r = 0;
-    switch (op) {
-      case TQ_ARITH_PLUS:                                                                 // builtin_arithmetic_vec.go:302-305
-        if ((x > 0 && y > DBL_MAX - x) || (x < 0 && y < -DBL_MAX - x)) err |= ERR_DOUBLE;
-        r = x + y; break;
-      case TQ_ARITH_MINUS:                                                                // :80-83
-        if ((x > 0 && -y > DBL_MAX - x) || (x < 0 && -y < -DBL_MAX - x)) err |= ERR_DOUBLE;
-        r = x - y; break;
-      case TQ_ARITH_MUL:                                                                  // :49-52
-        r = x * y; if (isinf(r)) err |= ERR_DOUBLE; break;
-      default:                                                                            // :368-381
-        if (y == 0) { cnt++; onn[0] = false; r = 0; }
-        else { r = x / y; if (isinf(r)) err |= ERR_DOUBLE; }
-        break;
-    }
-    o[0] = (uint64_t)__double_as_longlong(r);
-  }
-};
-
-struct FLogic {
-  int op;
-  __device__ __forceinline__ void operator()(const uint64_t (&v)[2], const bool (&nn)[2], uint64_t (&o)[1], bool (&onn)[1],
-                                             unsigned &, unsigned &, bool) const {
-    const bool n0 = !nn[0], n1 = !nn[1];
-    if (op == TQ_LOGIC_AND) {                                      // builtin_op_vec.go:192-211
-      if ((!n0 && v[0] == 0) || (!n1 && v[1] == 0)) { o[0] = 0; onn[0] = true; }
-      else if (n0 || n1) { o[0] = 0; onn[0] = false; }
-      else { o[0] = 1; onn[0] = true; }
-    } else {                                                       // builtin_op_vec.go:46-66
-      if ((!n0 && v[0] != 0) || (!n1 && v[1] != 0)) { o[0] = 1; onn[0] = true; }
-      else if (n0 || n1) { o[0] = 0; onn[0] = false; }
-      else { o[0] = 0; onn[0] = true; }
-    }
-  }
-};
-
-struct FUnary {
-  int op; bool ua;
-  __device__ __forceinline__ void operator()(const uint64_t (&v)[1], const bool (&nn)[1], uint64_t (&o)[1], bool (&onn)[1],
-                                             unsigned &err, unsigned &, bool active) const {
-    onn[0] = nn[0];
-    o[0] = 0;
-    switch (op) {
-      case TQ_UNARY_NOT_INT: if (nn[0]) o[0] = (v[0] == 0); break;                                   // builtin_op_vec.go:255-265
-      case TQ_UNARY_NOT_REAL: if (nn[0]) o[0] = (__longlong_as_double((long long)v[0]) == 0.0); break; // :152-165
-      case TQ_UNARY_MINUS_INT:                                                                        // :221-243
-        if (nn[0]) {
-          if (ua) { if (v[0] > 0x8000000000000000ull) err |= ERR_BIGINT; }
-          else if (v[0] == 0x8000000000000000ull) err |= ERR_BIGINT;
-          o[0] = 0ull - v[0];
-        }
-        break;
-      case TQ_UNARY_MINUS_REAL: if (nn[0]) o[0] = v[0] ^ 0x8000000000000000ull; break;               // :74-86 (-x flips the sign bit)
-      default: o[0] = nn[0] ? 0 : 1; onn[0] = active; break;                                          // IsNull :98-106 — never NULL
-    }
-  }
-};
-
-struct FIf {
-  __device__ __forceinline__ void operator()(const uint64_t (&v)[3], const bool (&nn)[3], uint64_t (&o)[1], bool (&onn)[1],
-                                             unsigned &, unsigned &, bool) const {
-    const bool take_b = !nn[0] || v[0] == 0;                       // builtin_control_vec_generated.go:141-156
-    onn[0] = take_b ? nn[2] : nn[1];
-    o[0] = onn[0] ? (take_b ? v[2] : v[1]) : 0;
-  }
-};
-struct FIfNull {
-  __device__ __forceinline__ void operator()(const uint64_t (&v)[2], const bool (&nn)[2], uint64_t (&o)[1], bool (&onn)[1],
-                                             unsigned &, unsigned &, bool) const {
-    onn[0] = nn[0] || nn[1];                                       // builtin_control_vec_generated.go:38-45
-    o[0] = nn[0] ? v[0] : (nn[1] ? v[1] : 0);
-  }
-};
+// ------------------------------------------------------------------ functors (the builtins are in expr_prog.cuh)
 struct FLtPlus {  // config C2: (a < b, a + b) in one pass over a and b
   __device__ __forceinline__ void operator()(const uint64_t (&v)[2], const bool (&nn)[2], uint64_t (&o)[2], bool (&onn)[2],
                                              unsigned &err, unsigned &, bool) const {
@@ -355,18 +174,9 @@ __global__ void k_filter_int(const uint64_t *a, const uint32_t *abm, uint8_t *se
 // Selection + Projection in one pass over the chunk (executor/executor.go SelectionExec.Next :463-499 →
 // expression.VectorizedFilter chunk_executor.go:196-245, VecEvalBool expression.go:205-279; ProjectionExec →
 // evalOneVec chunk_executor.go).  The host lowers the expression trees to a straight-line register program over
-// the builtin functors above; every intermediate column the reference materialises (one chunk.Column per builtin,
+// the builtin functors, run per row by xp_run_row (expr_prog.cuh); every intermediate column the reference materialises (one chunk.Column per builtin,
 // globalColumnAllocator) stays in a per-row register file here, so the HBM traffic is the input columns once and
 // the output columns once.  Register k < n_in is input column k; register n_in + i is the result of op i.
-static constexpr int XP_MAX_IN = TQ_EXPR_MAX_INPUTS;
-static constexpr int XP_MAX_OPS = TQ_EXPR_MAX_OPS;
-static constexpr int XP_MAX_OUT = TQ_EXPR_MAX_OUTPUTS;
-static constexpr int XP_REGS = XP_MAX_IN + XP_MAX_OPS;
-
-struct XOp {
-  int8_t kind, op, a, b, c, flags;   // flags: 1 a_unsigned, 2 b_unsigned, 4 constant is NULL
-  uint64_t imm;
-};
 struct ExprProg {
   int n_in, n_ops, n_out;
   const uint64_t *in_d[XP_MAX_IN];
@@ -414,49 +224,8 @@ __global__ void __launch_bounds__(MAP_THREADS) k_expr_prog(const __grid_constant
         rv[k] = e ? iv[k].y : iv[k].x;
         if (active && ((iw[k] >> ((2 * lane + e) & 31)) & 1u)) nn |= 1ull << k;
       }
-      // alive: the row is still in VecEvalBool's sel slice (errors and warnings of later builtins count for it);
-      // sel: the row passes every filter seen so far.
-      bool alive = active, sel = active;
-      for (int i = 0; i < P.n_ops; i++) {
-        const XOp x = P.ops[i];
-        const uint64_t v2[2] = {rv[x.a], rv[x.b]};
-        const bool n2[2] = {(bool)((nn >> x.a) & 1), (bool)((nn >> x.b) & 1)};
-        uint64_t o1[1] = {0};
-        bool on[1] = {true};
-        unsigned e_ = 0, c_ = 0;
-        switch (x.kind) {
-          case TQ_X_CONST: o1[0] = x.imm; on[0] = !(x.flags & 4); break;
-          case TQ_X_CMP_INT: FCompareInt{x.op, (bool)(x.flags & 1), (bool)(x.flags & 2)}(v2, n2, o1, on, e_, c_, active); break;
-          case TQ_X_CMP_REAL: FCompareReal{x.op}(v2, n2, o1, on, e_, c_, active); break;
-          case TQ_X_ARITH_INT: FArithInt{x.op, (bool)(x.flags & 1), (bool)(x.flags & 2)}(v2, n2, o1, on, e_, c_, active); break;
-          case TQ_X_ARITH_REAL: FArithReal{x.op}(v2, n2, o1, on, e_, c_, active); break;
-          case TQ_X_LOGIC: FLogic{x.op}(v2, n2, o1, on, e_, c_, active); break;
-          case TQ_X_UNARY: {
-            const uint64_t v1[1] = {v2[0]};
-            const bool n1[1] = {n2[0]};
-            FUnary{x.op, (bool)(x.flags & 1)}(v1, n1, o1, on, e_, c_, active);
-            break;
-          }
-          case TQ_X_IF: {
-            const uint64_t v3[3] = {v2[0], v2[1], rv[x.c]};
-            const bool n3[3] = {n2[0], n2[1], (bool)((nn >> x.c) & 1)};
-            FIf{}(v3, n3, o1, on, e_, c_, active);
-            break;
-          }
-          case TQ_X_IFNULL: FIfNull{}(v2, n2, o1, on, e_, c_, active); break;
-          case TQ_X_FILTER: {                                          // VecEvalBool expression.go:231-268
-            const bool isnull = !n2[0];
-            const bool zero = x.op ? (fabs(__longlong_as_double((long long)v2[0])) < 0.5) : (v2[0] == 0);
-            if (isnull) { sel = false; if (x.op) alive = false; }       // ETInt NULL stays in sel, flagged in nulls[]
-            else if (zero) { sel = false; alive = false; }
-            break;
-          }
-          default: alive = sel; break;                                 // TQ_X_COMPACT: Selection hands only selected rows on
-        }
-        if (alive) { my_err |= e_; my_cnt += c_; }
-        rv[P.n_in + i] = o1[0];
-        nn = (nn & ~(1ull << (P.n_in + i))) | ((uint64_t)on[0] << (P.n_in + i));
-      }
+      bool alive, sel;
+      xp_run_row(P.ops, P.n_ops, P.n_in, rv, nn, active, alive, sel, my_err, my_cnt);
 #pragma unroll
       for (int q = 0; q < XP_MAX_OUT; q++) {
         if (q < P.n_out) {
@@ -636,13 +405,6 @@ static int32_t run_map(int64_t n, int32_t mem, int nin, const tq_column *const *
   return TQ_OK;
 }
 
-static int32_t err_to_status(unsigned e, const char *what) {
-  if (e & ERR_UBIGINT) { set_error("BIGINT UNSIGNED value is out of range in '%s'", what); return TQ_ERR_OVERFLOW_BIGINT_UNSIGNED; }
-  if (e & ERR_BIGINT) { set_error("BIGINT value is out of range in '%s'", what); return TQ_ERR_OVERFLOW_BIGINT; }
-  if (e & ERR_DOUBLE) { set_error("DOUBLE value is out of range in '%s'", what); return TQ_ERR_OVERFLOW_DOUBLE; }
-  return TQ_OK;
-}
-
 template <int NIN, int NOUT, typename F>
 static int32_t map_call(int64_t n, int32_t mem, const tq_column *const *ins, tq_column *const *outs, F f, bool want_counter, ErrOut *eo) {
   auto launch = [&](const uint64_t **id, const uint32_t **ib, uint64_t **od, uint32_t **ob, int64_t rows, unsigned *d_err,
@@ -814,33 +576,7 @@ int32_t tq_expr_eval(int64_t n, int32_t n_inputs, const tq_column *inputs, int32
   memset(&P, 0, sizeof(P));
   P.n_in = n_inputs; P.n_ops = n_ops; P.n_out = n_outputs;
   bool want_counter = false;
-  for (int i = 0; i < n_ops; i++) {
-    const tq_expr_op &s = ops[i];
-    const int avail = n_inputs + i;   // an op reads inputs and earlier results only
-    int arity = 2, lo = 0, hi = 0;
-    switch (s.kind) {
-      case TQ_X_CONST: arity = 0; break;
-      case TQ_X_CMP_INT: case TQ_X_CMP_REAL: lo = TQ_CMP_LT; hi = TQ_CMP_NE; break;
-      case TQ_X_ARITH_INT: lo = TQ_ARITH_PLUS; hi = TQ_ARITH_MUL; break;
-      case TQ_X_ARITH_REAL: lo = TQ_ARITH_PLUS; hi = TQ_ARITH_DIV; want_counter = true; break;
-      case TQ_X_LOGIC: lo = TQ_LOGIC_AND; hi = TQ_LOGIC_OR; break;
-      case TQ_X_UNARY: arity = 1; lo = TQ_UNARY_NOT_INT; hi = TQ_UNARY_ISNULL; break;
-      case TQ_X_IF: arity = 3; break;
-      case TQ_X_IFNULL: break;
-      case TQ_X_FILTER: arity = 1; lo = 0; hi = 1; break;
-      case TQ_X_COMPACT: arity = 0; break;
-      default: set_error("expression program: op %d has unknown kind %d", i, s.kind); return TQ_ERR_INVALID_ARG;
-    }
-    if (s.op < lo || s.op > hi) { set_error("expression program: op %d (kind %d) has bad operator %d", i, s.kind, s.op); return TQ_ERR_INVALID_ARG; }
-    const int regs[3] = {s.a, s.b, s.c};
-    for (int k = 0; k < arity; k++)
-      if (regs[k] < 0 || regs[k] >= avail) { set_error("expression program: op %d reads register %d before it is written", i, regs[k]); return TQ_ERR_INVALID_ARG; }
-    XOp &x = P.ops[i];
-    x.kind = (int8_t)s.kind; x.op = (int8_t)s.op;
-    x.a = (int8_t)(arity > 0 ? s.a : 0); x.b = (int8_t)(arity > 1 ? s.b : 0); x.c = (int8_t)(arity > 2 ? s.c : 0);
-    x.flags = (int8_t)((s.a_unsigned ? 1 : 0) | (s.b_unsigned ? 2 : 0) | (s.is_null ? 4 : 0));
-    x.imm = s.imm;
-  }
+  TQ_TRY(xp_decode(n_inputs, n_ops, ops, P.ops, &want_counter));
   const tq_column *ins[XP_MAX_IN]; tq_column *op[XP_MAX_OUT];
   for (int k = 0; k < n_inputs; k++) ins[k] = &inputs[k];
   for (int q = 0; q < n_outputs; q++) {

@@ -1452,6 +1452,7 @@ struct ResultBatch {
   std::vector<PinBuf> h_data, h_bm;
   std::vector<VarOut> var;   // gathered FLOAT / var-len output columns (indexed like cols)
   std::vector<DevColBuf> alt;  // OtherConditions: the filtered copy of cols (swapped in)
+  unsigned oc_err = 0;         // OtherConditions: ERR_* bits its rows raised; the call that delivers the batch reports them
   bool on_host = false;
   cudaEvent_t ev_ready = nullptr;
   ~ResultBatch() { if (ev_ready) cudaEventDestroy(ev_ready); }
@@ -1515,9 +1516,10 @@ struct tq_join {
   int out_side[2 * MAXC] = {};            // per result-batch column: 0 = plain, 1 = build-side store, 2 = probe-side store
   int out_col[2 * MAXC] = {};
   DevBuf lens_scratch, scan_scratch3;
-  // OtherConditions (experimental, othercond.cuh): applied to every finished result batch
+  // OtherConditions (othercond.cuh): applied to every finished result batch
   bool has_oc = false;
   OcPlan oc;
+  int64_t oc_warnings = 0;                // division-by-zero warnings of the condition program so far
   int p_hidden_rowid = -1;                // outer joins: hidden probe column carrying the row id within the batch
   DevBuf oc_rowid[2], oc_scratch, oc_scan;
   int64_t batch_rows = 1 << 22;
@@ -2396,10 +2398,11 @@ static int32_t apply_other_conditions(tq_join *j, ResultBatch *rb, int64_t n_pro
     oc_cols.out_data[c] = rb->alt[c].data.as<uint64_t>();
     oc_cols.out_bm[c] = rb->alt[c].bm.as<uint32_t>();
   }
-  int64_t kept = 0;
-  TQ_TRY(oc_filter(j->oc, oc_cols, rb->n, n_probe_rows, j->oc_scratch, j->oc_scan, &kept, rt().compute));
+  int64_t kept = 0, warnings = 0;
+  TQ_TRY(oc_filter(j->oc, oc_cols, rb->n, n_probe_rows, j->oc_scratch, j->oc_scan, &kept, &rb->oc_err, &warnings, rt().compute));
   std::swap(rb->cols, rb->alt);
   rb->n = kept;
+  j->oc_warnings += warnings;
   return TQ_OK;
 }
 
@@ -2432,6 +2435,7 @@ static int32_t finalize_pending(tq_join *j) {
     if (cudaEventElapsedTime(&ms, j->ev_a[pb.cursor_slot], j->ev_b[pb.cursor_slot]) == cudaSuccess) j->last_probe_ns = (int64_t)(ms * 1e6);
   }
   pb.rb->n = (int64_t)produced;
+  pb.rb->oc_err = 0;
   if (j->has_oc) TQ_TRY(apply_other_conditions(j, pb.rb.get(), pb.n));
   j->joined_rows_total += pb.rb->n;
   if (j->any_ind) TQ_TRY(materialize_indirect(j, pb.rb.get(), pb.cursor_slot));  // synchronises the compute stream
@@ -2721,37 +2725,33 @@ int32_t tq_join_create(const tq_join_desc *d, tq_join **out) {
   return TQ_OK;
 }
 
-int32_t tq_join_set_other_conditions(tq_join *j, int32_t n_conds, const tq_join_cond *conds) {
-  if (!j || n_conds < 0 || n_conds > OC_MAX_CONDS || (n_conds && !conds)) { set_error("OtherConditions: 0..%d conditions", OC_MAX_CONDS); return TQ_ERR_INVALID_ARG; }
+}  // extern "C"
+
+// user output column (lhs ++ rhs) -> (build side?, column of that side)
+static void join_user_col(const tq_join *j, int u, bool *is_build, int *col) {
+  const int first_user = j->outer_is_right ? j->nb_user : j->np_user;
+  const bool first = u < first_user;
+  *is_build = j->outer_is_right ? first : !first;
+  *col = first ? u : u - first_user;
+}
+static int join_user_type(const tq_join *j, int u) {
+  bool is_build; int col;
+  join_user_col(j, u, &is_build, &col);
+  return is_build ? j->build_types[col] : j->probe_types[col];
+}
+
+static int32_t join_oc_settable(const tq_join *j) {
   if (j->state != tq_join::BUILDING || j->n_build != 0 || j->has_oc) { set_error("OtherConditions must be set once, right after tq_join_create"); return TQ_ERR_STATE; }
-  if (n_conds == 0) return TQ_OK;
+  return TQ_OK;
+}
+
+// Installs the OtherConditions program of either setter.  prog's input registers name user output columns.  An outer join
+// gets the hidden probe row-id column (last on the probe side), which moves the result-batch layout.
+static int32_t join_set_oc(tq_join *j, const JoinProg &prog, bool cmp_list) {
   const bool outer = j->join_type != TQ_JOIN_INNER;
   if (outer && j->n_probe_cols + 1 > MAXC) { set_error("OtherConditions on an outer join need one spare probe column"); return TQ_ERR_INVALID_ARG; }
   const int n_user = j->nb_user + j->np_user;
-  // user output column (lhs ++ rhs) -> (side, column, type)
-  auto side_of = [&](int u, bool *is_build, int *col) {
-    const int first_user = j->outer_is_right ? j->nb_user : j->np_user;
-    const bool first = u < first_user;
-    *is_build = j->outer_is_right ? first : !first;
-    *col = first ? u : u - first_user;
-  };
-  int types[OC_MAX_CONDS][2], sides[OC_MAX_CONDS][2], ccols[OC_MAX_CONDS][2];
-  for (int k = 0; k < n_conds; k++) {
-    const tq_join_cond &q = conds[k];
-    if (q.op < TQ_CMP_LT || q.op > TQ_CMP_NE || q.lhs_col < 0 || q.lhs_col >= n_user || q.rhs_col >= n_user) { set_error("OtherConditions: bad condition %d", k); return TQ_ERR_INVALID_ARG; }
-    for (int o = 0; o < 2; o++) {
-      const int u = o == 0 ? q.lhs_col : q.rhs_col;
-      if (u < 0) { types[k][o] = q.const_type; sides[k][o] = -1; ccols[k][o] = -1; continue; }
-      bool is_build; int col;
-      side_of(u, &is_build, &col);
-      types[k][o] = is_build ? j->build_types[col] : j->probe_types[col];
-      sides[k][o] = is_build ? 1 : 0;
-      ccols[k][o] = col;
-    }
-    const bool fa = types[k][0] == TQ_TYPE_FLOAT64, fb = types[k][1] == TQ_TYPE_FLOAT64;
-    if (!type_ok(types[k][0]) || !type_ok(types[k][1]) || fa != fb) { set_error("OtherConditions compare BIGINT with BIGINT or DOUBLE with DOUBLE columns"); return TQ_ERR_UNSUPPORTED_TYPE; }
-  }
-  if (outer) {  // hidden probe row-id column, last on the probe side
+  if (outer) {
     j->p_hidden_rowid = j->n_probe_cols;
     j->probe_types[j->n_probe_cols] = TQ_TYPE_INT64;
     j->n_probe_cols++;
@@ -2766,7 +2766,9 @@ int32_t tq_join_set_other_conditions(tq_join *j, int32_t n_conds, const tq_join_
   }
   const int bbase = j->outer_is_right ? 0 : j->n_probe_cols, pbase = j->outer_is_right ? j->n_build_cols : 0;
   j->oc = OcPlan();
-  j->oc.n_conds = n_conds;
+  j->oc.prog = prog;
+  j->oc.cmp_list = cmp_list ? 1 : 0;
+  for (int k = 0; k < prog.n_in; k++) j->oc.prog.in_col[k] = j->out_map[prog.in_col[k]];
   j->oc.outer = outer ? 1 : 0;
   j->oc.build_key_col = bbase + j->build_key;
   j->oc.rowid_col = outer ? pbase + j->p_hidden_rowid : -1;
@@ -2774,16 +2776,40 @@ int32_t tq_join_set_other_conditions(tq_join *j, int32_t n_conds, const tq_join_
   j->oc.build_hi = bbase + j->n_build_cols;
   for (int c = 0; c < j->n_build_cols; c++) j->oc.def_val[c] = j->def_val[c];
   j->oc.def_mask = j->def_mask;
-  for (int k = 0; k < n_conds; k++) {
-    OcCond &d = j->oc.c[k];
-    d.op = conds[k].op;
-    d.lhs = (sides[k][0] ? bbase : pbase) + ccols[k][0];
-    d.rhs = sides[k][1] < 0 ? -1 : (sides[k][1] ? bbase : pbase) + ccols[k][1];
-    d.lhs_type = types[k][0];
-    d.rhs_type = types[k][1];
-    d.cbits = conds[k].const_bits;
-  }
   j->has_oc = true;
+  return TQ_OK;
+}
+
+extern "C" {
+
+int32_t tq_join_set_other_conditions(tq_join *j, int32_t n_conds, const tq_join_cond *conds) {
+  if (!j || n_conds < 0 || n_conds > JP_MAX_CONDS || (n_conds && !conds)) { set_error("OtherConditions: 0..%d conditions", JP_MAX_CONDS); return TQ_ERR_INVALID_ARG; }
+  TQ_TRY(join_oc_settable(j));
+  if (n_conds == 0) return TQ_OK;
+  const int n_user = j->nb_user + j->np_user;
+  for (int k = 0; k < n_conds; k++) {
+    const tq_join_cond &q = conds[k];
+    if (q.op < TQ_CMP_LT || q.op > TQ_CMP_NE || q.lhs_col < 0 || q.lhs_col >= n_user || q.rhs_col >= n_user) { set_error("OtherConditions: bad condition %d", k); return TQ_ERR_INVALID_ARG; }
+    const int ta = join_user_type(j, q.lhs_col), tb = q.rhs_col >= 0 ? join_user_type(j, q.rhs_col) : q.const_type;
+    const bool fa = ta == TQ_TYPE_FLOAT64, fb = tb == TQ_TYPE_FLOAT64;
+    if (!type_ok(ta) || !type_ok(tb) || fa != fb) { set_error("OtherConditions compare BIGINT with BIGINT or DOUBLE with DOUBLE columns"); return TQ_ERR_UNSUPPORTED_TYPE; }
+  }
+  JoinProg prog;
+  join_prog_from_conds(n_conds, conds, [&](int u) { return join_user_type(j, u); }, &prog);
+  return join_set_oc(j, prog, true);
+}
+
+int32_t tq_join_set_other_program(tq_join *j, int32_t n_inputs, const int32_t *input_cols, int32_t n_ops, const tq_expr_op *ops) {
+  if (!j) return TQ_ERR_INVALID_ARG;
+  TQ_TRY(join_oc_settable(j));
+  JoinProg prog;
+  TQ_TRY(join_prog_from_ops(n_inputs, input_cols, n_ops, ops, j->nb_user + j->np_user, [&](int u) { return join_user_type(j, u); }, &prog));
+  return join_set_oc(j, prog, false);
+}
+
+int32_t tq_join_warnings(tq_join *j, int64_t *div_by_zero) {
+  if (!j || !div_by_zero) return TQ_ERR_INVALID_ARG;
+  *div_by_zero = j->oc_warnings;
   return TQ_OK;
 }
 
@@ -3055,6 +3081,7 @@ static int32_t join_current_batch(tq_join *j, int64_t max_rows, int *have, int32
     j->host_cur = std::move(j->results.front());
     j->results.pop_front();
     j->host_cur_pos = 0;
+    if (j->host_cur->oc_err) return err_to_status(j->host_cur->oc_err, "other conditions");
     if (!j->host_cur->on_host) {
       // Large consumer buffers: copy straight from HBM into the caller's columns (no staging, no CPU memcpy).
       // (a queued batch is complete: finalize_pending waited for its kernels — no stream-wide sync here, so the copy
@@ -3174,6 +3201,7 @@ int32_t tq_join_next_device(tq_join *j, tq_column *out_cols, int64_t *n_rows, in
   }
   j->lent = std::move(j->results.front());
   j->results.pop_front();
+  if (j->lent->oc_err) return err_to_status(j->lent->oc_err, "other conditions");
   const int ncols = j->nb_user + j->np_user;
   for (int c = 0; c < ncols; c++) {
     out_cols[c].length = j->lent->n;

@@ -1,29 +1,21 @@
-// othercond.cuh — HashJoinExec OtherConditions on the device (EXPERIMENTAL: written in round 1 after the GPU budget was
-// spent; parity tests exist but are gated behind TQ_RUN_EXPERIMENTS until they have run on the GPU).
+// othercond.cuh — HashJoinExec OtherConditions on the device.
 //
 // Reference: joiner.tryToMatchInners builds the joined rows of one outer row, baseJoiner.filter keeps those for which every
-// condition is true, and an outer row none of whose joined rows survive is emitted once with a NULL inner side by
-// onMissMatch (executor/joiner.go:155-167,225-248,274-277,337-340).  Here the conditions are applied to a finished result
-// batch: evaluate per joined row, count survivors per probe row (outer joins carry a hidden probe-row-id column), turn one
-// failed row of every survivor-less probe row into its miss row, compact.
+// condition is true (expression.VectorizedFilter), and an outer row none of whose joined rows survive is emitted once with a
+// NULL / defaultInner inner side by onMissMatch (executor/joiner.go:155-167,225-248,274-277,337-340).  Here the conditions
+// are applied to a finished result batch: run the condition program (expr_prog.cuh) per joined row, count survivors per
+// probe row (outer joins carry a hidden probe-row-id column), turn one failed row of every survivor-less probe row into its
+// miss row, compact.
 #pragma once
-#include "common.cuh"
+#include "expr_prog.cuh"
 
 namespace tq {
 
-static constexpr int OC_MAX_CONDS = 8;
 static constexpr int OC_MAX_COLS = 34;
 
-struct OcCond {
-  int op;            // TQ_CMP_*
-  int lhs, rhs;      // result-batch column indices; rhs < 0: compare with the constant
-  int lhs_type, rhs_type;
-  uint64_t cbits;
-};
-
 struct OcPlan {
-  int n_conds = 0;
-  OcCond c[OC_MAX_CONDS];
+  JoinProg prog;           // input registers name result-batch columns
+  int cmp_list = 0;        // prog is a lowered tq_join_cond list: evaluated by oc_cmp_list_passes
   int outer = 0;           // left / right outer join
   int build_key_col = -1;  // result column of the build-side key: NOT NULL <=> the row is a key match
   int rowid_col = -1;      // outer joins: result column holding the probe row id within the batch
@@ -40,8 +32,9 @@ struct OcCols {
   uint32_t *out_bm[OC_MAX_COLS];
 };
 
-// Filters n joined rows into the out_* columns (caller-allocated for n rows, bitmaps zeroed here); *n_out = rows kept.
+// Filters n joined rows into the out_* columns (caller-allocated for n rows, bitmaps zeroed here); *n_out = rows kept,
+// *err = the ERR_* bits and *div_by_zero = the division-by-zero warnings the key-matched rows raised.
 int32_t oc_filter(const OcPlan &plan, const OcCols &cols, int64_t n, int64_t n_probe_rows, DevBuf &scratch, DevBuf &scan_scratch, int64_t *n_out,
-                  cudaStream_t s);
+                  unsigned *err, int64_t *div_by_zero, cudaStream_t s);
 
 }  // namespace tq

@@ -27,6 +27,7 @@
 #include <vector>
 
 #include "common.cuh"
+#include "expr_prog.cuh"
 #include "varlen.cuh"
 
 using namespace tq;
@@ -283,53 +284,40 @@ __global__ void __launch_bounds__(256) k_mj_expand(const uint32_t *__restrict__ 
   }
 }
 
-// OtherConditions of the joiner (baseJoiner.filter, executor/joiner.go:155-167) over the joined pairs: comparisons of two 8-byte
-// columns of the joined row, or of a column with a constant; a NULL operand fails the condition (VectorizedFilter drops it)
-constexpr int MJ_MAX_CONDS = 8;
-struct MJOperand {
-  int side;               // 0 inner row, 1 outer row, 2 constant
-  int type;               // TQ_TYPE_INT64 / UINT64 / FLOAT64
-  const uint64_t *data;
-  const uint32_t *bm;
-  uint64_t cbits;
+// OtherConditions of the joiner (baseJoiner.filter, executor/joiner.go:155-167) over the expanded pairs: the condition program
+// (expr_prog.cuh) with input register k gathered by row id from the inner or the outer row store.  flags[t] = 1 iff pair t
+// joins an inner row and the program selects it.  A ROW_MISS pair (no key match, a NULL key, an outer row the outer filter
+// dropped) never runs the program, so it raises no error and no warning (joiner.go:225-228,288-291 return before filter).
+struct MJProg {
+  int n_in = 0, n_ops = 0;
+  const uint64_t *data[JP_MAX_IN] = {};
+  const uint32_t *bm[JP_MAX_IN] = {};
+  int inner[JP_MAX_IN] = {};   // 1: register k comes from the inner row, 0: from the outer row
+  XOp ops[XP_MAX_OPS] = {};
 };
-struct MJCond { int op; MJOperand a, b; };
-struct MJConds { int n; MJCond c[MJ_MAX_CONDS]; };
-
-__device__ __forceinline__ bool mj_operand(const MJOperand &x, uint32_t inner_row, uint32_t outer_row, uint64_t *v) {
-  if (x.side == 2) { *v = x.cbits; return true; }
-  const uint32_t r = x.side == 0 ? inner_row : outer_row;
-  if (!tqd::bm_not_null(x.bm, r)) return false;
-  *v = x.data[r];
-  return true;
-}
-// types.CompareInt with the operands' unsigned flags (expression/builtin_compare.go:541-560), CompareFloat64
-__device__ __forceinline__ int mj_cmp_values(int ta, uint64_t a, int tb, uint64_t b) {
-  if (ta == TQ_TYPE_FLOAT64) { const double x = __longlong_as_double((long long)a), y = __longlong_as_double((long long)b); return x < y ? -1 : (x == y ? 0 : 1); }
-  const bool ua = ta == TQ_TYPE_UINT64, ub = tb == TQ_TYPE_UINT64;
-  if (ua && ub) return a < b ? -1 : (a == b ? 0 : 1);
-  const int64_t x = (int64_t)a, y = (int64_t)b;
-  if (!ua && !ub) return x < y ? -1 : (x == y ? 0 : 1);
-  if (ua && !ub) { if (y < 0 || a > 0x7FFFFFFFFFFFFFFFull) return 1; return x < y ? -1 : (x == y ? 0 : 1); }
-  if (x < 0 || b > 0x7FFFFFFFFFFFFFFFull) return -1;
-  return x < y ? -1 : (x == y ? 0 : 1);
-}
-// flags[t] = 1 iff pair t joins an inner row and passes every condition
-__global__ void __launch_bounds__(256) k_mj_cond(const MJConds C, const uint32_t *__restrict__ out_outer, const uint32_t *__restrict__ out_inner, int64_t m,
-                                                 uint32_t *__restrict__ flags) {
+// err_warn[0] |= ERR_* bits, err_warn[1] += division-by-zero warnings of the evaluated pairs
+__global__ void __launch_bounds__(256) k_mj_prog(const __grid_constant__ MJProg P, const uint32_t *__restrict__ out_outer, const uint32_t *__restrict__ out_inner,
+                                                 int64_t m, uint32_t *__restrict__ flags, unsigned long long *err_warn) {
   const int64_t stride = (int64_t)gridDim.x * blockDim.x;
+  unsigned my_err = 0, my_cnt = 0;
   for (int64_t t = (int64_t)blockIdx.x * blockDim.x + threadIdx.x; t < m; t += stride) {
     const uint32_t ir = out_inner[t], orow = out_outer[t];
-    bool ok = ir != ROW_MISS;
-    for (int k = 0; ok && k < C.n; k++) {
-      uint64_t a, b;
-      if (!mj_operand(C.c[k].a, ir, orow, &a) || !mj_operand(C.c[k].b, ir, orow, &b)) { ok = false; break; }
-      const int c = mj_cmp_values(C.c[k].a.type, a, C.c[k].b.type, b);
-      const int op = C.c[k].op;
-      ok = op == TQ_CMP_LT ? c < 0 : op == TQ_CMP_LE ? c <= 0 : op == TQ_CMP_GT ? c > 0 : op == TQ_CMP_GE ? c >= 0 : op == TQ_CMP_EQ ? c == 0 : c != 0;
+    bool pass = false;
+    if (ir != ROW_MISS) {
+      uint64_t rv[JP_REGS];
+      uint64_t nn = 0;
+      for (int k = 0; k < P.n_in; k++) {
+        const uint32_t r = P.inner[k] ? ir : orow;
+        rv[k] = P.data[k][r];
+        if (tqd::bm_not_null(P.bm[k], r)) nn |= 1ull << k;
+      }
+      bool alive;
+      xp_run_row(P.ops, P.n_ops, P.n_in, rv, nn, true, alive, pass, my_err, my_cnt);
     }
-    flags[t] = ok ? 1u : 0u;
+    flags[t] = pass ? 1u : 0u;
   }
+  if (my_err) atomicOr(&err_warn[0], (unsigned long long)my_err);
+  if (my_cnt) atomicAdd(&err_warn[1], (unsigned long long)my_cnt);
 }
 // rows each outer row emits once its pairs are filtered: the survivors, or the miss row of an outer join when none survived
 __global__ void __launch_bounds__(256) k_mj_survivors(const uint32_t *__restrict__ emit_off, const uint32_t *__restrict__ fscan, int64_t n_outer, int64_t m, uint32_t n_pass,
@@ -779,7 +767,10 @@ struct tq_mjoin {
   bool has_selected = false;
   std::vector<uint64_t> dflt_bits;
   std::vector<uint8_t> dflt_nn;
-  std::vector<tq_join_cond> conds;   // OtherConditions (tq_mjoin_set_other_conditions)
+  int oc_form = 0;                   // OtherConditions: 0 none, 1 tq_mjoin_set_other_conditions, 2 tq_mjoin_set_other_program
+  JoinProg oc;                       // input registers name output columns (left ++ right)
+  unsigned oc_err = 0;               // ERR_* bits the program raised: the calls that deliver the result report them
+  int64_t oc_warnings = 0;
   bool finished = false;
   ResultHost res;
   bool host_ready = false;
@@ -975,29 +966,59 @@ int32_t tq_mjoin_create(const tq_mjoin_desc *d, tq_mjoin **out) {
   return TQ_OK;
 }
 
+}  // extern "C"
+
+// output column c of left ++ right
+static const StoreCol &mjoin_col(const tq_mjoin *h, int c) {
+  const int n_first = (int)(h->outer_is_right ? h->inner.cols.size() : h->outer.cols.size());
+  const bool in_first = c < n_first;
+  const RowStore &st = (in_first == (h->outer_is_right != 0)) ? h->inner : h->outer;
+  return st.cols[(size_t)(in_first ? c : c - n_first)];
+}
+// the comparison list may be set again (the last call counts); the program once, and never both forms on one handle
+static int32_t mjoin_oc_settable(const tq_mjoin *h, int form) {
+  if (h->finished || h->inner.n || h->outer.n) { set_error("other conditions must be set right after tq_mjoin_create"); return TQ_ERR_STATE; }
+  if (h->oc_form && (h->oc_form != form || form == 2)) { set_error("the handle has other conditions already"); return TQ_ERR_STATE; }
+  return TQ_OK;
+}
+
+extern "C" {
+
 // OtherConditions: comparisons over the joined row (left ++ right), as tq_join_set_other_conditions takes them
 int32_t tq_mjoin_set_other_conditions(tq_mjoin *h, int32_t n_conds, const tq_join_cond *conds) {
-  if (!h || n_conds < 0 || n_conds > MJ_MAX_CONDS || (n_conds && !conds)) { set_error("at most %d other conditions", MJ_MAX_CONDS); return TQ_ERR_INVALID_ARG; }
-  if (h->finished || h->inner.n || h->outer.n) { set_error("other conditions must be set right after tq_mjoin_create"); return TQ_ERR_STATE; }
-  const int n_first = (int)(h->outer_is_right ? h->inner.cols.size() : h->outer.cols.size());
+  if (!h || n_conds < 0 || n_conds > JP_MAX_CONDS || (n_conds && !conds)) { set_error("at most %d other conditions", JP_MAX_CONDS); return TQ_ERR_INVALID_ARG; }
+  TQ_TRY(mjoin_oc_settable(h, 1));
   const int n_all = (int)(h->inner.cols.size() + h->outer.cols.size());
-  auto col_of = [&](int c) -> const StoreCol & {   // output column c of left ++ right
-    const bool in_first = c < n_first;
-    const RowStore &st = (in_first == (h->outer_is_right != 0)) ? h->inner : h->outer;
-    return st.cols[(size_t)(in_first ? c : c - n_first)];
-  };
   for (int k = 0; k < n_conds; k++) {
     const tq_join_cond &c = conds[k];
     if (c.op < TQ_CMP_LT || c.op > TQ_CMP_NE || c.lhs_col < 0 || c.lhs_col >= n_all || c.rhs_col >= n_all) { set_error("bad other condition %d", k); return TQ_ERR_INVALID_ARG; }
-    const StoreCol &a = col_of(c.lhs_col);
-    const int tb = c.rhs_col >= 0 ? col_of(c.rhs_col).type : (c.const_type & 0xFF);
-    const bool b_fixed8 = c.rhs_col >= 0 ? col_of(c.rhs_col).kind == 0 : (tb >= TQ_TYPE_INT64 && tb <= TQ_TYPE_FLOAT64);
+    const StoreCol &a = mjoin_col(h, c.lhs_col);
+    const int tb = c.rhs_col >= 0 ? mjoin_col(h, c.rhs_col).type : (c.const_type & 0xFF);
+    const bool b_fixed8 = c.rhs_col >= 0 ? mjoin_col(h, c.rhs_col).kind == 0 : (tb >= TQ_TYPE_INT64 && tb <= TQ_TYPE_FLOAT64);
     if (a.kind != 0 || !b_fixed8 || ((a.type == TQ_TYPE_FLOAT64) != (tb == TQ_TYPE_FLOAT64))) {
       set_error("other condition %d: BIGINT with BIGINT (any sign mix) or DOUBLE with DOUBLE", k);
       return TQ_ERR_UNSUPPORTED_TYPE;
     }
   }
-  h->conds.assign(conds, conds + n_conds);
+  h->oc_form = 0;
+  if (n_conds == 0) return TQ_OK;
+  join_prog_from_conds(n_conds, conds, [&](int c) { return mjoin_col(h, c).type; }, &h->oc);
+  h->oc_form = 1;
+  return TQ_OK;
+}
+
+int32_t tq_mjoin_set_other_program(tq_mjoin *h, int32_t n_inputs, const int32_t *input_cols, int32_t n_ops, const tq_expr_op *ops) {
+  if (!h) return TQ_ERR_INVALID_ARG;
+  TQ_TRY(mjoin_oc_settable(h, 2));
+  const int n_all = (int)(h->inner.cols.size() + h->outer.cols.size());
+  TQ_TRY(join_prog_from_ops(n_inputs, input_cols, n_ops, ops, n_all, [&](int c) { return mjoin_col(h, c).type; }, &h->oc));
+  h->oc_form = 2;
+  return TQ_OK;
+}
+
+int32_t tq_mjoin_warnings(tq_mjoin *h, int64_t *div_by_zero) {
+  if (!h || !div_by_zero) return TQ_ERR_INVALID_ARG;
+  *div_by_zero = h->oc_warnings;
   return TQ_OK;
 }
 
@@ -1161,40 +1182,40 @@ int32_t tq_mjoin_finish(tq_mjoin *h) {
   const uint32_t *rows_o = out_o.as<uint32_t>(), *rows_i = out_i.as<uint32_t>();
   int64_t m_out = m;
   DevBuf flags, fscan, emit2, new_o, new_i;
-  if (!h->conds.empty()) {
+  if (h->oc_form) {
     // tryToMatchInners filters the joined rows of an outer row with the OtherConditions; when none survives the outer row
     // takes the miss path (merge_join.go:290-305, joiner.go:225-248,288-311,351-378)
-    MJConds C{};
-    C.n = (int)h->conds.size();
+    MJProg P;
+    P.n_in = h->oc.n_in;
+    P.n_ops = h->oc.n_ops;
+    for (int i = 0; i < P.n_ops; i++) P.ops[i] = h->oc.ops[i];
     const int n_first = (int)first->cols.size();
-    auto operand = [&](int c, int const_type, uint64_t cbits) {
-      MJOperand x{};
-      if (c < 0) { x.side = 2; x.type = const_type & 0xFF; x.cbits = cbits; return x; }
+    for (int k = 0; k < P.n_in; k++) {
+      const int c = h->oc.in_col[k];
       const bool in_first = c < n_first;
       const RowStore *st = in_first ? first : second;
       const StoreCol &sc = st->cols[(size_t)(in_first ? c : c - n_first)];
-      x.side = st == &h->inner ? 0 : 1;
-      x.type = sc.type;
-      x.data = sc.d_data.as<uint64_t>();
-      x.bm = sc.bm();
-      return x;
-    };
-    for (int k = 0; k < C.n; k++) {
-      C.c[k].op = h->conds[(size_t)k].op;
-      C.c[k].a = operand(h->conds[(size_t)k].lhs_col, 0, 0);
-      C.c[k].b = operand(h->conds[(size_t)k].rhs_col, h->conds[(size_t)k].const_type, h->conds[(size_t)k].const_bits);
+      P.inner[k] = st == &h->inner ? 1 : 0;
+      P.data[k] = sc.d_data.as<uint64_t>();
+      P.bm[k] = sc.bm();
     }
     TQ_TRY(flags.reserve((size_t)(m ? m : 1) * 4));
     TQ_TRY(fscan.reserve((size_t)(m ? m : 1) * 4));
     TQ_TRY(emit2.reserve((size_t)no * 4));
     uint64_t n_pass = 0;
     if (m > 0) {
-      TQ_LAUNCH(k_mj_cond, grid_for(m), 256, 0, s, C, out_o.as<uint32_t>(), out_i.as<uint32_t>(), m, flags.as<uint32_t>());
+      // meta[5] / meta[6]: the program's error bits and warnings, read back with n_pass (meta[3])
+      TQ_LAUNCH(k_mj_prog, grid_for(m), 256, 0, s, P, out_o.as<uint32_t>(), out_i.as<uint32_t>(), m, flags.as<uint32_t>(),
+                reinterpret_cast<unsigned long long *>(meta.as<uint64_t>() + 5));
       count_launch();
-      TQ_TRY(check_launch("k_mj_cond"));
+      TQ_TRY(check_launch("k_mj_prog"));
       TQ_TRY(exclusive_scan_u32(flags.as<uint32_t>(), 1, fscan.as<uint32_t>(), 1, m, meta.as<uint64_t>() + 3, scan, s));
-      TQ_CUDA(cudaMemcpyAsync(&n_pass, meta.as<uint64_t>() + 3, 8, cudaMemcpyDeviceToHost, s));
+      uint64_t back[4] = {0, 0, 0, 0};   // n_pass, (meta[4]), error bits, warnings
+      TQ_CUDA(cudaMemcpyAsync(back, meta.as<uint64_t>() + 3, 32, cudaMemcpyDeviceToHost, s));
       TQ_CUDA(cudaStreamSynchronize(s));
+      n_pass = back[0];
+      h->oc_err = (unsigned)back[2];
+      h->oc_warnings += (int64_t)back[3];
     }
     TQ_LAUNCH(k_mj_survivors, grid_for(no), 256, 0, s, emit.as<uint32_t>(), fscan.as<uint32_t>(), no, m, (uint32_t)n_pass, outer_join ? 1 : 0, emit2.as<uint32_t>());
     count_launch();
@@ -1273,6 +1294,7 @@ extern "C" {
 int32_t tq_mjoin_next_bytes(tq_mjoin *h, int64_t max_rows, int64_t *bytes_per_col) {
   if (!h || !bytes_per_col || max_rows <= 0) return TQ_ERR_INVALID_ARG;
   if (!h->finished) { set_error("next before finish"); return TQ_ERR_STATE; }
+  if (h->oc_err) return err_to_status(h->oc_err, "other conditions");
   TQ_TRY(mjoin_host_result(h));
   return result_next_bytes(h->res, max_rows, bytes_per_col);
 }
@@ -1280,6 +1302,7 @@ int32_t tq_mjoin_next_bytes(tq_mjoin *h, int64_t max_rows, int64_t *bytes_per_co
 int32_t tq_mjoin_next(tq_mjoin *h, int64_t max_rows, tq_column *out_cols, int64_t *n_rows, int32_t *eof) {
   if (!h || !out_cols || !n_rows || !eof || max_rows <= 0) return TQ_ERR_INVALID_ARG;
   if (!h->finished) { set_error("next before finish"); return TQ_ERR_STATE; }
+  if (h->oc_err) return err_to_status(h->oc_err, "other conditions");
   TQ_TRY(mjoin_host_result(h));
   return result_next(h->res, max_rows, out_cols, n_rows, eof);
 }
@@ -1288,6 +1311,7 @@ int32_t tq_mjoin_next(tq_mjoin *h, int64_t max_rows, tq_column *out_cols, int64_
 int32_t tq_mjoin_next_device(tq_mjoin *h, tq_column *out_cols, int64_t *n_rows, int32_t *eof) {
   if (!h || !out_cols || !n_rows || !eof) return TQ_ERR_INVALID_ARG;
   if (!h->finished) { set_error("next before finish"); return TQ_ERR_STATE; }
+  if (h->oc_err) return err_to_status(h->oc_err, "other conditions");
   TQ_TRY(ensure_init());
   Runtime &r = rt();
   std::lock_guard<std::recursive_mutex> lk(r.mu);

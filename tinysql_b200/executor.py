@@ -11,6 +11,7 @@ import numpy as np
 
 from . import _lib as L
 from .chunk import (BYTES, FLOAT64, INT64, MAX_CHUNK_SIZE, UINT64, Chunk, Column, DeviceColumn, VarColumn, device_to_host, tq_array)
+from .expression import JoinProgram
 
 INNER_JOIN, LEFT_OUTER_JOIN, RIGHT_OUTER_JOIN = 0, 1, 2  # planner/core/logical_plans.go:52-57
 AGG_COUNT, AGG_SUM, AGG_AVG, AGG_MAX, AGG_MIN, AGG_FIRSTROW = range(6)
@@ -46,16 +47,20 @@ class HashJoinExec:
     """executor/join.go:31-146.  inner = build side, outer = probe side; output = left ++ right."""
 
     def __init__(self, outer_exec, inner_exec, outer_keys, inner_keys, join_type=INNER_JOIN, outer_is_right=False,
-                 outer_filter=None, probe_batch_rows=0, max_chunk_size=MAX_CHUNK_SIZE, stable_input=False, other_conditions=(), default_inner=None):
+                 outer_filter=None, probe_batch_rows=0, max_chunk_size=MAX_CHUNK_SIZE, stable_input=False, other_conditions=(), default_inner=None,
+                 other_program=()):
         self.outer, self.inner = outer_exec, inner_exec
         self.outer_keys, self.inner_keys = list(outer_keys), list(inner_keys)
         self.join_type, self.outer_is_right = join_type, outer_is_right
         self.outer_filter = outer_filter  # callable(chunk) -> selected bytes (expression.VectorizedFilter result)
         self.probe_batch_rows = probe_batch_rows
         self.stable_input = stable_input  # TQ_JOIN_STABLE_INPUT: the children keep every chunk alive and unmodified until Close
-        # OtherConditions (joiner.go:155-167) as (op, lhs_col, rhs_col) or (op, lhs_col, None, const_type, const_value) over
-        # the output row lhs ++ rhs — EXPERIMENTAL device path (tq_join_set_other_conditions)
+        # OtherConditions (joiner.go:155-167) over the output row lhs ++ rhs, in one of two forms: other_conditions as
+        # (op, lhs_col, rhs_col) or (op, lhs_col, None, const_type, const_value) comparisons (tq_join_set_other_conditions),
+        # or other_program as a CNF list of expression.Expr filters, Col(i) = output column i (tq_join_set_other_program)
         self.other_conditions = list(other_conditions)
+        self.other_program = list(other_program)
+        self.warnings = 0   # division-by-zero warnings of other_program (tq_join_warnings), current after each Next
         # PhysicalHashJoin.DefaultValues (builder.go:449-465): per inner column the value a miss row of an outer join carries (None = NULL)
         self.default_inner = default_inner
         self.max_chunk_size = max_chunk_size
@@ -91,6 +96,9 @@ class HashJoinExec:
                 else:
                     arr[i] = L.TQJoinCond(c[0], c[1], c[2], 0, 0)
             L.check(lib.tq_join_set_other_conditions(h, len(self.other_conditions), arr))
+        if self.other_program:
+            JoinProgram(self.other_program).set_on(lib.tq_join_set_other_program, h)
+        self.warnings = 0
         self.prepared = False
         self.outer_done = False
 
@@ -137,6 +145,9 @@ class HashJoinExec:
                 sel = np.ascontiguousarray(self.outer_filter(chk), dtype=np.uint8)
             L.check(lib.tq_join_put_probe(self.handle, tq_array(chk.cols), sel.ctypes.data if sel is not None else None, L.TQ_MEM_HOST))
         k = n.value
+        w = C.c_int64(0)
+        L.check(lib.tq_join_warnings(self.handle, C.byref(w)))
+        self.warnings = w.value
         return Chunk([c.head(k) if t == BYTES else Column(t, c.values[:k], c.not_null()[:k]) for t, c in zip(self.types, out)])
 
     def Close(self):
@@ -322,9 +333,12 @@ class MergeJoinExec:
     """executor/merge_join.go:31-373.  Both children sorted ascending by their keys; output = left ++ right in outer order."""
 
     def __init__(self, outer_exec, inner_exec, outer_keys, inner_keys, join_type=INNER_JOIN, outer_is_right=False, outer_filter=None,
-                 max_chunk_size=MAX_CHUNK_SIZE, default_inner=None, other_conditions=()):
-        # other_conditions: (op, lhs_col, rhs_col) or (op, lhs_col, None, const_type, const_value) over the output row left ++ right
+                 max_chunk_size=MAX_CHUNK_SIZE, default_inner=None, other_conditions=(), other_program=()):
+        # OtherConditions over the output row left ++ right, as in HashJoinExec: other_conditions = (op, lhs_col, rhs_col) or
+        # (op, lhs_col, None, const_type, const_value) comparisons, other_program = a CNF list of expression.Expr filters
         self.other_conditions = list(other_conditions)
+        self.other_program = list(other_program)
+        self.warnings = 0   # division-by-zero warnings of other_program (tq_mjoin_warnings), current after each Next
         self.outer, self.inner = outer_exec, inner_exec
         self.outer_keys, self.inner_keys = list(outer_keys), list(inner_keys)
         self.join_type, self.outer_is_right, self.outer_filter = join_type, outer_is_right, outer_filter
@@ -357,6 +371,9 @@ class MergeJoinExec:
                 else:
                     arr[i] = L.TQJoinCond(c[0], c[1], c[2], 0, 0)
             L.check(lib.tq_mjoin_set_other_conditions(h, len(self.other_conditions), arr))
+        if self.other_program:
+            JoinProgram(self.other_program).set_on(lib.tq_mjoin_set_other_program, h)
+        self.warnings = 0
 
     def Next(self, required_rows=None):
         lib = L.load()
@@ -376,6 +393,9 @@ class MergeJoinExec:
                 L.check(lib.tq_mjoin_put_outer(self.handle, tq_array(chk.cols), sel.ctypes.data if sel is not None else None, L.TQ_MEM_HOST))
             L.check(lib.tq_mjoin_finish(self.handle))
             self.prepared = True
+            w = C.c_int64(0)
+            L.check(lib.tq_mjoin_warnings(self.handle, C.byref(w)))
+            self.warnings = w.value
         return _drain_result(lib, self.types, required_rows or self.max_chunk_size, lib.tq_mjoin_next_bytes, lib.tq_mjoin_next, self.handle)
 
     def Close(self):

@@ -329,3 +329,30 @@ class ExprProgram:
         L.check(L.load().tq_expr_eval(n, len(cols), tq_array(cols), len(self.ops), ops, len(outs), regs, tq_array(outs),
                                       sel.ctypes.data if sel is not None else None, C.byref(dz), L.TQ_MEM_HOST))
         return outs, (sel[:n] if sel is not None else None), dz.value
+
+
+class JoinProgram:
+    """OtherConditions of a join as the program of tq_join_set_other_program / tq_mjoin_set_other_program: filters is a CNF
+    list of Expr trees over the joined row (Col(i) = output column i of left ++ right).  The referenced output columns become
+    the input registers in order of first use; the trees are lowered by ExprProgram."""
+
+    def __init__(self, filters):
+        self.input_cols = []
+
+        def remap(e):
+            if isinstance(e, Col):
+                if e.idx not in self.input_cols:
+                    self.input_cols.append(e.idx)
+                return Col(self.input_cols.index(e.idx), e.tp)
+            if isinstance(e, Const):
+                return e
+            return Func(e.name, *[remap(a) for a in e.args])
+
+        filters = [remap(f) for f in filters]
+        self.program = ExprProgram(len(self.input_cols), filters)
+
+    def set_on(self, setter, handle):
+        """calls setter(handle, n_inputs, input_cols, n_ops, ops) and checks its status"""
+        cols = (C.c_int32 * max(len(self.input_cols), 1))(*self.input_cols)
+        ops = (L.TQExprOp * max(len(self.program.ops), 1))(*self.program.ops)
+        L.check(setter(handle, len(self.input_cols), cols, len(self.program.ops), ops))
