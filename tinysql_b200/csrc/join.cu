@@ -11,7 +11,7 @@
 //       row-major in key order; duplicates keep build insertion order (rowHashMap.Get, hash_table.go:259-272).
 //       Build: insert+count, exclusive scan, fill, sort duplicate segments, gather rows.
 //   Large NOT NULL build sides that fit an entry first try the streaming build (try_stream_build, gated by stream_build_ok):
-//       k_scatter_aos into AoS slabs, then k_build_cluster builds each partition's tables in cluster shared memory.
+//       k_scatter_aos into one AoS slab per sub-table, then k_build_cluster builds each sub-table in cluster shared memory.
 // Probe.  Small build (one table): k_probe, ordered output (probe row asc, build insertion asc) via
 //   ticketed tiles + decoupled look-back.
 //   Large build, PK-FK shape (stream_probe_ok, no probe NULL bitmap): the streaming positional path of join_stream.cuh
@@ -53,7 +53,7 @@ enum { KEYMODE_RAW = 0, KEYMODE_NO_SIGNBIT = 1, KEYMODE_NEVER = 2 };
 
 struct JoinTable {
   uint64_t *words;  // entry e = words[e << shift ...]
-  uint64_t mask;    // entries per partition table - 1
+  uint32_t cap;     // entries per partition table (even; partition table t starts at entry t * cap)
   int pbits;        // log2(#partition tables); 0 = one table
   int shift;        // log2(words per entry): 1 or 2
   int row_mode;
@@ -68,7 +68,17 @@ __device__ __forceinline__ bool key_valid(uint64_t key, bool not_null, int key_m
   return false;
 }
 
-__device__ __forceinline__ uint32_t home_loc(uint64_t h, uint64_t mask, int shift) { return (uint32_t)((shift == 1) ? ((h & mask) & ~1ull) : (h & mask)); }
+// The slot arithmetic of every partition table (builders and probers alike).  A table of `cap` entries need not be a power
+// of two: the home slot scales the low 32 hash bits onto [0, cap) (the partition comes from the top bits), and probing wraps
+// inside the table.  16-byte entries (shift == 1) start on an even slot, so a 32-byte sector holds a whole entry PAIR.
+__device__ __forceinline__ uint32_t home_slot(uint64_t h, uint32_t cap, int shift) {
+  const uint32_t s = __umulhi((uint32_t)h, cap);
+  return shift == 1 ? (s & ~1u) : s;
+}
+__device__ __forceinline__ uint32_t next_slot(uint32_t loc, uint32_t step, uint32_t cap) {
+  loc += step;
+  return loc >= cap ? loc - cap : loc;
+}
 
 // (word0, word1) of an entry with one 128-bit load
 __device__ __forceinline__ ulonglong2 ld_entry(const uint64_t *words, uint64_t e, int shift) {
@@ -94,7 +104,7 @@ struct InsertParams {
   int write_rows;
   int64_t n;
   uint64_t *words;
-  uint64_t mask;
+  uint32_t cap;           // entries per partition table
   int pbits, shift;
   uint32_t sent_entry;
   uint32_t *row_slot;
@@ -124,8 +134,8 @@ __global__ void __launch_bounds__(256) k_build_insert(const InsertParams b) {
       continue;
     }
     const uint64_t h = tqd::hash_key(key);
-    const uint64_t base = part_of_hash(h, b.pbits) * (b.mask + 1);
-    uint64_t loc = (b.shift == 1) ? ((h & b.mask) & ~1ull) : (h & b.mask);  // 16-byte entries: start on a 32-byte sector boundary (probes read entry PAIRS)
+    const uint64_t base = part_of_hash(h, b.pbits) * b.cap;
+    uint32_t loc = home_slot(h, b.cap, b.shift);
     my_valid++;
     for (;;) {
       const uint64_t e = base + loc;
@@ -136,7 +146,7 @@ __global__ void __launch_bounds__(256) k_build_insert(const InsertParams b) {
         if (b.write_rows) write_row_words(b, b.words + (e << b.shift), i, false);
       }
       if (prev == EMPTY_KEY || prev == key) { b.row_slot[i] = (uint32_t)e; break; }
-      loc = (loc + 1) & b.mask;
+      loc = next_slot(loc, 1, b.cap);
     }
   }
   my_valid = __reduce_add_sync(0xffffffffu, my_valid);
@@ -361,7 +371,7 @@ template <bool SMEM>
 __device__ __forceinline__ uint2 resolve(const JoinTable &t, const uint64_t *tbl /*partition base (global or smem)*/, uint64_t ebase, uint64_t key,
                                          uint32_t loc, ulonglong2 &cur /* in: home entry; out: matched entry (word0, word1) */) {
   while (cur.x != key && cur.x != EMPTY_KEY) {  // linear probing; short at load factor <= 0.5
-    loc = (loc + 1) & (uint32_t)t.mask;
+    loc = next_slot(loc, 1, t.cap);
     cur = ld_entry(tbl, loc, t.shift);
   }
   if (cur.x != key) return make_uint2(OFF_MISS, 0);
@@ -553,8 +563,8 @@ __global__ void __launch_bounds__(PROBE_THREADS) k_probe(const ProbeParams p, co
         valid[k] = sel && key_valid(key[k], tqd::bm_not_null(kbm, r), p.key_mode);
       }
       const uint64_t h = tqd::hash_key(key[k]);
-      ebase[k] = part_of_hash(h, t.pbits) * (t.mask + 1);
-      loc[k] = home_loc(h, t.mask, t.shift);
+      ebase[k] = part_of_hash(h, t.pbits) * t.cap;
+      loc[k] = home_slot(h, t.cap, t.shift);
     }
 #pragma unroll
     for (int k = 0; k < PROBE_ROWS_PER_THREAD; k++) {  // the 4 random entry loads are issued back to back
@@ -983,7 +993,7 @@ __device__ __forceinline__ bool part_prologue(const ProbeParams &p, const JoinTa
   c.t_hi = p_tiles * (sub + 1) / p.split;
   if (c.t_lo >= c.t_hi) return false;
   c.has_table = c.part < n_parts;  // partition n_parts: rows that cannot match (outer joins only)
-  const uint64_t cap = t.mask + 1;
+  const uint64_t cap = t.cap;
   c.ebase = (uint64_t)(c.has_table ? c.part : 0) * cap;
   c.tbl = t.words + (c.ebase << t.shift);
   // Small partition tables are copied into shared memory by TMA; larger ones are probed in place — consecutive
@@ -1042,7 +1052,7 @@ __global__ void __launch_bounds__(PROBE_THREADS) k_probe_part_uniq(const ProbePa
     ulonglong2 first[R];
 #pragma unroll
     for (int k = 0; k < R; k++) {  // independent entry loads issued back to back
-      loc[k] = home_loc(tqd::hash_key(key[k]), t.mask, t.shift);
+      loc[k] = home_slot(tqd::hash_key(key[k]), t.cap, t.shift);
       first[k] = make_ulonglong2(EMPTY_KEY, 0);
       if (inb[k] && cx.has_table && key[k] != EMPTY_KEY) first[k] = ld_entry(cx.tbl, loc[k], t.shift);
     }
@@ -1130,7 +1140,7 @@ __global__ void __launch_bounds__(PROBE_THREADS, 4) k_probe_part_fast(const Prob
 #pragma unroll
   for (int c = 1; c < NP; c++) if (c == kc) keys = pin[c];
   const unsigned lt_mask = (1u << lane) - 1;
-  const uint32_t mask = (uint32_t)t.mask;
+  const uint32_t cap = t.cap;
   const int shift = t.shift;
   const bool smem = cx.use_smem;
   unsigned matched_acc = 0;
@@ -1159,7 +1169,7 @@ __global__ void __launch_bounds__(PROBE_THREADS, 4) k_probe_part_fast(const Prob
       EntryPair pr[R];
 #pragma unroll
       for (int k = 0; k < R; k++) {  // R independent sector loads in flight
-        loc[k] = home_loc(tqd::hash_key(key[k]), mask, 1);
+        loc[k] = home_slot(tqd::hash_key(key[k]), cap, 1);
         pr[k].a = make_ulonglong2(EMPTY_KEY, 0);
         pr[k].b = pr[k].a;
         if (key[k] != EMPTY_KEY) pr[k] = ld_pair(cx.tbl, loc[k], smem);
@@ -1179,7 +1189,7 @@ __global__ void __launch_bounds__(PROBE_THREADS, 4) k_probe_part_fast(const Prob
             if (pr[k].a.x == EMPTY_KEY) break;
             if (pr[k].b.x == key[k]) { ent[k] = pr[k].b; loc[k] += 1; hit = true; break; }
             if (pr[k].b.x == EMPTY_KEY) break;
-            loc[k] = (loc[k] + 2) & mask;
+            loc[k] = next_slot(loc[k], 2, cap);
             pr[k] = ld_pair(cx.tbl, loc[k], smem);
           }
         } else if ((wbase + k * 32) < cx.p_hi && t.sent_cnt) {  // a probe key equal to the empty marker: its row is the side entry
@@ -1193,7 +1203,7 @@ __global__ void __launch_bounds__(PROBE_THREADS, 4) k_probe_part_fast(const Prob
     } else {
 #pragma unroll
       for (int k = 0; k < R; k++) {
-        loc[k] = home_loc(tqd::hash_key(key[k]), mask, shift);
+        loc[k] = home_slot(tqd::hash_key(key[k]), cap, shift);
         ent[k] = make_ulonglong2(EMPTY_KEY, 0);
         if (key[k] != EMPTY_KEY) ent[k] = ld_entry(cx.tbl, loc[k], shift);
       }
@@ -1207,7 +1217,7 @@ __global__ void __launch_bounds__(PROBE_THREADS, 4) k_probe_part_fast(const Prob
         bool hit = false;
         if (key[k] != EMPTY_KEY) {
           while (ent[k].x != key[k] && ent[k].x != EMPTY_KEY) {
-            loc[k] = (loc[k] + 1) & mask;
+            loc[k] = next_slot(loc[k], 1, cap);
             ent[k] = ld_entry(cx.tbl, loc[k], shift);
           }
           hit = ent[k].x == key[k];
@@ -1312,7 +1322,7 @@ __global__ void __launch_bounds__(PROBE_THREADS) k_probe_part(const ProbeParams 
 #pragma unroll
     for (int k = 0; k < PROBE_ROWS_PER_THREAD; k++) {
       const int64_t r = tile_base + k * PROBE_THREADS + tid;
-      loc[k] = home_loc(tqd::hash_key(key[k]), t.mask, t.shift);
+      loc[k] = home_slot(tqd::hash_key(key[k]), t.cap, t.shift);
       first[k] = make_ulonglong2(EMPTY_KEY, 0);
       if (r < cx.p_hi && cx.has_table && key[k] != EMPTY_KEY) first[k] = ld_entry(cx.tbl, loc[k], t.shift);
     }
@@ -1669,8 +1679,8 @@ static bool stream_probe_ok(const tq_join *j) {
          j->n_probe_cols <= 4 && j->n_build_cols <= 4 && !j->has_oc && !g_no_fast_kernel;
 }
 
-// Partition-local build (join_stream.cuh): scatter the build rows into AoS partition slabs, then one thread-block cluster
-// per partition builds its sub-tables in distributed shared memory (k_build_cluster).  The table has 2^(pbits + sbits)
+// Partition-local build (join_stream.cuh): scatter the build rows into one AoS slab per sub-table, then one thread-block
+// cluster per slab builds its sub-table in distributed shared memory (k_build_cluster).  The table has 2^(pbits + sbits)
 // sub-tables; the probe side keeps the 2^pbits coarse partitions.  Covers the PK-FK shape — NOT NULL build columns that fit
 // a table entry, unique keys; anything else (*done == false) takes the general build below.
 static int32_t try_stream_build(tq_join *j, bool *done) {
@@ -1683,24 +1693,29 @@ static int32_t try_stream_build(tq_join *j, bool *done) {
   if (pbits > SA_MAX_PBITS) pbits = SA_MAX_PBITS;
   if (pbits < 1) return TQ_OK;
   const int P = 1 << pbits;
-  const uint64_t slab = slab_rows(n, P, true);
-  if (slab * P > 0xFFFFFFF0ull) return TQ_OK;
   // Table capacity from the row count alone (no host round trip for the partition histogram): hash partitions of m rows hold
   // m +- a few sqrt(m); a sub-table that turns out fuller than the load limit allows is flagged by the build kernel and the
   // general path takes over.  sbits: the fewest sub-tables per partition for which one fits the shared memory of a cluster.
+  // cap is that estimate at the load limit, rounded up to 16 entries so that every CTA's slice holds whole 32-byte sectors.
   const int shift = NB > 2 ? 2 : 1;
   int sbits = 0;
-  uint64_t cap = 64;
+  uint64_t cap = 0;
   for (;; sbits++) {
     if (pbits + sbits > PART_MAX_BITS) return TQ_OK;  // (the general probe path scatters into one bin per sub-table)
     const double mean = (double)n / (double)((uint64_t)P << sbits);
     const uint64_t est_max = (uint64_t)(mean + 8.0 * sqrt(mean) + 64.0);
-    cap = 64;
-    while (cap * (uint64_t)g_max_load_pct < est_max * 100) cap <<= 1;
+    cap = (est_max * 100 / (uint64_t)g_max_load_pct + 15) & ~15ull;
     if (((cap << shift) * 8) / BC_CLUSTER <= (uint64_t)BC_MAX_SLICE_BYTES) break;
   }
   const uint64_t n_slots = ((uint64_t)P << sbits) * cap;
   if (n_slots > (uint64_t)n * 12 + 4096 || n_slots > 0xFFFFFFF0ull) return TQ_OK;
+  // The build rows are scattered straight into one slab per sub-table when the scatter has that many bins; beyond
+  // SA_MAX_PBITS bits each slab holds 2^(pbits + sbits - bbits) sub-tables, which its cluster builds one after another.
+  const int tbits = pbits + sbits;
+  const int bbits = tbits < SA_MAX_PBITS ? tbits : SA_MAX_PBITS;
+  const int n_bins = 1 << bbits;
+  const uint64_t bin_slab = slab_rows(n, n_bins, true);
+  if (bin_slab * n_bins > 0xFFFFFFF0ull) return TQ_OK;
   const BuildClusterKernel kb = build_cluster_kernel(NB);
   const int slice_bytes = (int)(((cap << shift) * 8) / BC_CLUSTER);
   cudaLaunchConfig_t cfg{};
@@ -1709,7 +1724,7 @@ static int32_t try_stream_build(tq_join *j, bool *done) {
   cl[0].val.clusterDim.x = BC_CLUSTER;
   cl[0].val.clusterDim.y = 1;
   cl[0].val.clusterDim.z = 1;
-  cfg.gridDim = dim3((unsigned)(P * BC_CLUSTER));
+  cfg.gridDim = dim3((unsigned)(n_bins * BC_CLUSTER));
   cfg.blockDim = dim3(BC_THREADS);
   cfg.stream = s;
   cfg.attrs = cl;
@@ -1735,7 +1750,7 @@ static int32_t try_stream_build(tq_join *j, bool *done) {
   for (int c = 0; c < NB; c++) q.sp.in[c] = j->b_view[c];
   q.sp.key_col = j->build_key;
   q.sp.key_mode = j->key_mode;   // rows whose key can never match are dropped here (hash_table.go:161-163 skips NULL keys; none here)
-  q.sp.pbits = pbits;
+  q.sp.pbits = bbits;
   q.sp.n = n;
   q.sp.overflow = cur + 2;
   TQ_TRY(scatter_aos(q, j->b_aos, off, hi, lim, s));
@@ -1749,8 +1764,8 @@ static int32_t try_stream_build(tq_join *j, bool *done) {
   bp.words = words;
   bp.cap = (uint32_t)cap;
   bp.max_rows = (uint32_t)(cap * (uint64_t)g_max_load_pct / 100);
-  bp.pbits = pbits;
-  bp.sbits = sbits;
+  bp.tbits = tbits;
+  bp.lbits = tbits - bbits;
   bp.key_col = j->build_key;
   {
     int w = 1;
@@ -1764,15 +1779,15 @@ static int32_t try_stream_build(tq_join *j, bool *done) {
   TQ_CUDA(cudaLaunchKernelEx(&cfg, kb, bp));
   count_launch();
   TQ_TRY(check_launch("k_build_cluster"));
-  std::vector<uint32_t> h_hi((size_t)P);
+  std::vector<uint32_t> h_hi((size_t)n_bins);
   unsigned long long h_cur[4] = {0, 0, 0, 0};
-  TQ_CUDA(cudaMemcpyAsync(h_hi.data(), hi.p, (size_t)P * 4, cudaMemcpyDeviceToHost, s));
+  TQ_CUDA(cudaMemcpyAsync(h_hi.data(), hi.p, (size_t)n_bins * 4, cudaMemcpyDeviceToHost, s));
   TQ_CUDA(cudaMemcpyAsync(h_cur, cur, 32, cudaMemcpyDeviceToHost, s));
   TQ_CUDA(cudaStreamSynchronize(s));
   if (h_cur[2]) return TQ_OK;  // a slab overflowed: skewed hash partitions
   if (h_cur[3]) return TQ_OK;  // duplicate keys, the empty-marker key, or a partition over the load limit: the general build handles them
   uint64_t n_valid = 0;
-  for (int q2 = 0; q2 < P; q2++) n_valid += h_hi[q2] - (uint64_t)q2 * slab;
+  for (int q2 = 0; q2 < n_bins; q2++) n_valid += h_hi[q2] - (uint64_t)q2 * bin_slab;
   j->shift = shift;
   j->pbits = pbits;
   j->n_slots = n_slots;
@@ -1781,8 +1796,8 @@ static int32_t try_stream_build(tq_join *j, bool *done) {
   j->build_unique = true;
   j->row_mode = true;
   j->table.words = words;
-  j->table.mask = cap - 1;
-  j->table.pbits = pbits + sbits;
+  j->table.cap = (uint32_t)cap;
+  j->table.pbits = tbits;
   j->table.shift = shift;
   j->table.row_mode = 1;
   j->table.sent_off = (uint32_t)n_slots;
@@ -1875,7 +1890,7 @@ static int32_t join_build(tq_join *j) {
   ip.write_rows = row_candidate ? 1 : 0;
   ip.n = n;
   ip.words = words;
-  ip.mask = cap - 1;
+  ip.cap = (uint32_t)cap;
   ip.pbits = pbits;
   ip.shift = shift;
   ip.sent_entry = (uint32_t)n_slots;
@@ -1895,7 +1910,7 @@ static int32_t join_build(tq_join *j) {
   j->n_distinct = distinct_regular + (sent_cnt ? 1 : 0);
   j->build_unique = (j->n_distinct == j->n_valid);
   j->table.words = words;
-  j->table.mask = cap - 1;
+  j->table.cap = (uint32_t)cap;
   j->table.pbits = pbits;
   j->table.shift = shift;
   j->row_mode = j->build_unique && row_candidate;
@@ -2327,7 +2342,7 @@ static int32_t launch_probe(tq_join *j, const std::vector<DCol> &probe, const ui
     if (split64 * work_parts > (1ll << 30)) split64 = (1ll << 30) / work_parts;
     int split = (int)split64;
     p.split = split;
-    const size_t image_bytes = (size_t)((j->table.mask + 1) << j->shift) * 8;
+    const size_t image_bytes = ((size_t)j->table.cap << j->shift) * 8;
     const bool in_smem = image_bytes <= PART_MAX_SMEM_BYTES;
     p.table_in_smem = in_smem ? 1 : 0;
     const size_t table_bytes = in_smem ? image_bytes : 0;

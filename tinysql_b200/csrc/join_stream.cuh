@@ -14,8 +14,8 @@
 //                       slots are real.  The holes (misses, and the padding of each partition to a multiple of 32) are
 //                       filled afterwards from the tail of the result (k_hole_*): for a foreign-key join that is a few
 //                       thousand rows.  The contract is the result MULTISET (SURVEY Appendix B); order is not.
-//   k_build_cluster<NB> build of the partition tables from build-side AoS slabs: one 8-CTA cluster per partition builds
-//                       its sub-tables one after another in distributed shared memory and writes each out once.
+//   k_build_cluster<NB> build of the partition tables from build-side AoS slabs (one per sub-table): one 8-CTA cluster per
+//                       slab builds its sub-table in distributed shared memory and writes it out once.
 #pragma once
 
 #include <cooperative_groups.h>
@@ -354,28 +354,35 @@ struct ProbePosParams {
 };
 
 // Find `key` in its partition table starting at its home entry.  SHIFT == 1: 16-byte entries fetched as 32-byte aligned
-// PAIRS (one sector tests two slots); SHIFT == 2: 32-byte entries.  loc is the entry index in the whole table: the table's
-// first entry (a multiple of mask + 1) OR the index inside it, so a wrap keeps the high bits.  Returns hit; (w0, w1) = words
-// 0 / 1 of the matched entry, loc = its index.  The common case — the key sits in its home pair — is straight-line code.
+// PAIRS (one sector tests two slots); SHIFT == 2: 32-byte entries.  loc is the entry index in the whole table (the home
+// entry, already loaded into a / b); past it the walk wraps inside the key's table of `cap` entries (table index = its top
+// `pbits` hash bits).  Returns hit; w1 = word 1 of the matched entry, loc = its index.  The common case — the key sits in
+// its home pair — is straight-line code.
 template <int SHIFT>
-__device__ __forceinline__ bool probe_find(const uint64_t *words, uint32_t mask, uint64_t key, uint32_t &loc, uint64_t &w1, ulonglong2 a, ulonglong2 b) {
-  if constexpr (SHIFT == 1) {
-    for (;;) {
-      if (a.x == key) { w1 = a.y; return true; }
-      if (b.x == key) { w1 = b.y; loc += 1; return true; }
-      if (a.x == EMPTY_KEY || b.x == EMPTY_KEY) return false;
-      loc = (loc & ~mask) | ((loc + 2) & mask);
+__device__ __forceinline__ bool probe_find(const uint64_t *words, uint32_t cap, int pbits, uint64_t key, uint32_t &loc, uint64_t &w1, ulonglong2 a, ulonglong2 b) {
+  // 1: hit at loc (+ 1 for the pair's second entry), 0: miss, -1: the walk goes on
+  auto test = [&](ulonglong2 x, ulonglong2 y) -> int {
+    if (x.x == key) { w1 = x.y; return 1; }
+    if constexpr (SHIFT == 1) {
+      if (y.x == key) { w1 = y.y; loc += 1; return 1; }
+      if (y.x == EMPTY_KEY) return 0;
+    }
+    return x.x == EMPTY_KEY ? 0 : -1;
+  };
+  int r = test(a, b);
+  if (r >= 0) return r != 0;
+  const uint32_t base = (uint32_t)part_of_hash(tqd::hash_key(key), pbits) * cap;
+  uint32_t i = loc - base;
+  for (;;) {
+    i = next_slot(i, SHIFT == 1 ? 2 : 1, cap);
+    loc = base + i;
+    if constexpr (SHIFT == 1) {
       const EntryPair pr = ld_pair(words, loc, false);
-      a = pr.a;
-      b = pr.b;
+      r = test(pr.a, pr.b);
+    } else {
+      r = test(ld_entry(words, loc, SHIFT), b);
     }
-  } else {
-    for (;;) {
-      if (a.x == key) { w1 = a.y; return true; }
-      if (a.x == EMPTY_KEY) return false;
-      loc = (loc & ~mask) | ((loc + 1) & mask);
-      a = ld_entry(words, loc, SHIFT);
-    }
+    if (r >= 0) return r != 0;
   }
 }
 
@@ -437,8 +444,7 @@ __global__ void __launch_bounds__((CW + 1) * 32, OCC) k_probe_pos(const ProbePos
   }
   // ---- consumers: warp w owns rows [w * 32 * R, (w + 1) * 32 * R) of every tile.  The table may be split finer than the
   // probe partitions (k_build_cluster's sub-tables), so a row's table comes from its own hash.
-  const uint32_t cap = (uint32_t)(t.mask + 1);
-  const uint32_t mask = (uint32_t)t.mask;
+  const uint32_t cap = t.cap;
   const int kc = p.key_col;
   const int woff = warp * (32 * R) + lane;                      // this lane's first row inside a tile
   const uint64_t obase = (uint64_t)p.out_base[part] + woff;     // ... and its output slot inside the partition's range
@@ -494,7 +500,7 @@ __global__ void __launch_bounds__((CW + 1) * 32, OCC) k_probe_pos(const ProbePos
       for (int c = 1; c < NP; c++) if (c == kc) key[k] = v[k][c];
       inb[k] = (t0 + woff + k * 32) < p_rows;
       const uint64_t h = tqd::hash_key(key[k]);
-      loc[k] = (uint32_t)part_of_hash(h, t.pbits) * cap | home_loc(h, mask, SHIFT);
+      loc[k] = (uint32_t)part_of_hash(h, t.pbits) * cap + home_slot(h, cap, SHIFT);
       ea[k] = make_ulonglong2(EMPTY_KEY, 0);
       eb[k] = ea[k];
       if (inb[k] && key[k] != EMPTY_KEY) {
@@ -508,7 +514,7 @@ __global__ void __launch_bounds__((CW + 1) * 32, OCC) k_probe_pos(const ProbePos
       uint64_t w1 = 0;
       bool hit = false;
       if (inb[k]) {
-        if (key[k] != EMPTY_KEY) hit = probe_find<SHIFT>(t.words, mask, key[k], loc[k], w1, ea[k], eb[k]);
+        if (key[k] != EMPTY_KEY) hit = probe_find<SHIFT>(t.words, cap, t.pbits, key[k], loc[k], w1, ea[k], eb[k]);
         else if (t.sent_cnt) {  // a probe key equal to the empty marker: its row is the table's side entry
           loc[k] = t.sent_off;
           w1 = t.words[((uint64_t)t.sent_off << SHIFT) + 1];
@@ -619,15 +625,16 @@ __global__ void __launch_bounds__(256) k_hole_move(const HoleMoveParams h) {
 }
 
 // ------------------------------------------------------------------------------------------------ cluster build
-// One cluster of BC_CLUSTER CTAs builds the tables of one coarse partition in distributed shared memory.  The partition's
-// table is split into 2^sbits sub-tables (the next sbits hash bits below the partition bits); each is small enough to live
-// in the cluster's shared memory, CTA r holding entries [r * slice, (r + 1) * slice).  Per sub-table: initialise the slices,
-// insert the partition's rows of that sub-table with atomicCAS on the owning CTA's shared memory (re-reads of the slab after
-// the first hit L2), then stream every slice to its place in the table with coalesced 16-byte stores.  Each table line is
-// written to DRAM once, with no initialisation pass and no L2 atomics.
+// One cluster of BC_CLUSTER CTAs builds the sub-tables of one scatter bin in distributed shared memory.  A partition's table
+// is split into 2^sbits sub-tables (the next sbits hash bits below the partition bits), each small enough to live in the
+// cluster's shared memory, CTA r holding entries [r * slice, (r + 1) * slice).  The build side is scattered into one slab per
+// sub-table (2^lbits sub-tables per slab only past SA_MAX_PBITS scatter bits).  Per sub-table: initialise the slices, insert
+// the slab's rows of that sub-table with atomicCAS on the owning CTA's shared memory, then stream every slice to its place in
+// the table with coalesced 16-byte stores.  Each table line is written to DRAM once, with no initialisation pass and no L2
+// atomics.  With one sub-table per slab the write-back follows the last cluster barrier, so no CTA waits for it.
 static constexpr int BC_CLUSTER = 8;
-static constexpr int BC_THREADS = 1024;
-static constexpr int BC_MAX_SLICE_BYTES = 128 << 10;  // one CTA's share of a sub-table (capacities are powers of two: 1 MB per cluster)
+static constexpr int BC_THREADS = 512;
+static constexpr int BC_MAX_SLICE_BYTES = 112 << 10;  // one CTA's share of a sub-table: two CTAs fit an SM's 228 KB
 // shared::cluster addresses: the same shared-memory offset in the CTA of the given rank, and accesses through them
 __device__ __forceinline__ uint32_t dsmem_map(uint32_t local, uint32_t rank) {
   uint32_t a;
@@ -643,17 +650,17 @@ __device__ __forceinline__ void dsmem_st_u64(uint32_t a, uint64_t v) { asm volat
 __device__ __forceinline__ void dsmem_add_u32(uint32_t a, uint32_t v) { asm volatile("red.shared::cluster.add.u32 [%0], %1;" ::"r"(a), "r"(v) : "memory"); }
 
 struct BuildClusterParams {
-  const uint64_t *slab;              // AoS build rows (NB words each)
+  const uint64_t *slab;              // AoS build rows (NB words each), one slab per scatter bin
   const uint32_t *lo, *hi, *lim;     // a slab that overflowed (hi > lim) holds lim - lo rows; the caller discards the build anyway
-  uint64_t *words;                   // the table: sub-table t = (coarse partition << sbits) | sub starts at entry t * cap
-  uint32_t cap;                      // entries per sub-table (a power of two, >= 64: every slice holds whole entry pairs)
+  uint64_t *words;                   // the table: sub-table t (top tbits hash bits) starts at entry t * cap
+  uint32_t cap;                      // entries per sub-table (a multiple of 16: every slice holds whole entry pairs)
   uint32_t max_rows;                 // rows a sub-table may hold at the configured load factor
-  int pbits, sbits, key_col;
+  int tbits, lbits, key_col;         // 2^tbits sub-tables in all, 2^lbits of them per scatter bin
   int word_of_col[4];
   unsigned *flags;                   // |= 1: duplicate key, |= 2: the empty-marker key appeared, |= 4: a sub-table is over the load limit  -> the caller rebuilds on the general path
 };
 template <int NB>
-__global__ void __launch_bounds__(BC_THREADS, 1) k_build_cluster(const BuildClusterParams b) {
+__global__ void __launch_bounds__(BC_THREADS, 2) k_build_cluster(const BuildClusterParams b) {
   namespace cg = cooperative_groups;
   constexpr int SHIFT = NB > 2 ? 2 : 1;  // words per entry = 1 << SHIFT (the probers read the table the same way)
   constexpr int BC_UNROLL = 4;  // slab rows loaded ahead of their inserts, per thread
@@ -662,16 +669,16 @@ __global__ void __launch_bounds__(BC_THREADS, 1) k_build_cluster(const BuildClus
   cg::cluster_group cluster = cg::this_cluster();
   const int tid = threadIdx.x;
   const uint32_t rank = cluster.block_rank();
-  const uint32_t part = blockIdx.x / BC_CLUSTER;
-  const uint32_t slice = b.cap / BC_CLUSTER, slice_bits = __ffs(slice) - 1, mask = b.cap - 1;
+  const uint32_t bin = blockIdx.x / BC_CLUSTER;
+  const uint32_t cap = b.cap, slice = cap / BC_CLUSTER;
   const uint32_t n_vec = (slice << SHIFT) / 2;        // 16-byte pieces of a slice
-  const int64_t p_lo = b.lo[part];
-  int64_t p_hi = b.hi[part];
-  if (p_hi > (int64_t)b.lim[part]) p_hi = b.lim[part];
+  const int64_t p_lo = b.lo[bin];
+  int64_t p_hi = b.hi[bin];
+  if (p_hi > (int64_t)b.lim[bin]) p_hi = b.lim[bin];
   const uint32_t s_base = smem_u32(s_tbl), rows0 = dsmem_map(smem_u32(&s_rows), 0);
   ulonglong2 *s_vec = reinterpret_cast<ulonglong2 *>(s_tbl);
-  const int n_sub = 1 << b.sbits;
-  for (int sub = 0; sub < n_sub; sub++) {
+  const uint32_t n_sub = 1u << b.lbits;
+  for (uint32_t sub = 0; sub < n_sub; sub++) {
     for (uint32_t i = tid; i < n_vec; i += BC_THREADS)
       s_vec[i] = (SHIFT == 1 || (i & 1) == 0) ? make_ulonglong2(EMPTY_KEY, 0) : make_ulonglong2(0, 0);
     if (rank == 0 && tid == 0) s_rows = 0;
@@ -704,12 +711,14 @@ __global__ void __launch_bounds__(BC_THREADS, 1) k_build_cluster(const BuildClus
         for (int c = 0; c < NB; c++) key |= w[u][c] & (c == b.key_col ? ~0ull : 0ull);
         if (key == EMPTY_KEY) { if (sub == 0) atomicOr(b.flags, 2u); continue; }
         const uint64_t h = tqd::hash_key(key);
-        if (((uint32_t)part_of_hash(h, b.pbits + b.sbits) & (uint32_t)(n_sub - 1)) != (uint32_t)sub) continue;
+        // (n_sub == 1, every slab a single sub-table: the mask is 0 and every row passes)
+        if (((uint32_t)part_of_hash(h, b.tbits) & (n_sub - 1)) != sub) continue;
         mine++;
-        uint32_t loc = home_loc(h, mask, SHIFT);
+        uint32_t loc = home_slot(h, cap, SHIFT);
         for (uint32_t probes = 0;; probes++) {
-          if (probes > mask) { atomicOr(b.flags, 4u); break; }  // the sub-table is full (far over the load limit)
-          const uint32_t ent = dsmem_map(s_base + ((loc & (slice - 1)) << (SHIFT + 3)), loc >> slice_bits);
+          if (probes >= cap) { atomicOr(b.flags, 4u); break; }  // the sub-table is full (far over the load limit)
+          const uint32_t owner = loc / slice;
+          const uint32_t ent = dsmem_map(s_base + ((loc - owner * slice) << (SHIFT + 3)), owner);
           const uint64_t prev = dsmem_cas_u64(ent, EMPTY_KEY, key);
           if (prev == EMPTY_KEY) {
 #pragma unroll
@@ -717,7 +726,7 @@ __global__ void __launch_bounds__(BC_THREADS, 1) k_build_cluster(const BuildClus
             break;
           }
           if (prev == key) { atomicOr(b.flags, 1u); break; }
-          loc = (loc + 1) & mask;
+          loc = next_slot(loc, 1, cap);
         }
       }
     }
@@ -727,9 +736,9 @@ __global__ void __launch_bounds__(BC_THREADS, 1) k_build_cluster(const BuildClus
     // this iteration, so after the last sub-table it is the barrier that lets every CTA exit.
     cluster.sync();
     if (rank == 0 && tid == 0 && s_rows > b.max_rows) atomicOr(b.flags, 4u);
-    uint64_t *dst = b.words + (((((uint64_t)part << b.sbits) | (uint64_t)sub) * b.cap + (uint64_t)rank * slice) << SHIFT);
+    uint64_t *dst = b.words + (((((uint64_t)bin << b.lbits) | (uint64_t)sub) * cap + (uint64_t)rank * slice) << SHIFT);
     for (uint32_t i = tid; i < n_vec; i += BC_THREADS) tqd::st_stream_u64x2(dst + 2 * (uint64_t)i, s_vec[i]);
-    __syncthreads();  // the slice is re-initialised for the next sub-table
+    if (sub + 1 < n_sub) __syncthreads();  // the slice is re-initialised for the next sub-table
   }
 }
 typedef void (*BuildClusterKernel)(const BuildClusterParams);
