@@ -341,7 +341,12 @@ int32_t tq_join_probe_eof(tq_join *j);
  * peers' tq_partition_push_regions kernels).  cols[g * n_probe_cols + c] = column c of region g (NOT NULL 8-byte columns,
  * `length` ignored); *seg_counts[g] = the rows region g holds — a DEVICE value, read by the kernels, never by the host, so no
  * host synchronisation sits between the exchange and the join; seg_cap = rows a region can hold.  Inner PK-FK joins on the
- * streaming path only (TQ_ERR_UNSUPPORTED_TYPE otherwise: read the counts and use tq_join_put_probe per region). */
+ * streaming path only (TQ_ERR_UNSUPPORTED_TYPE otherwise: read the counts and use tq_join_put_probe per region).
+ * The call only enqueues the batch: the regions and their counts must stay unchanged until the batch is finalised, i.e.
+ * until the next tq_join_put_probe / _put_probe_segments, tq_join_probe_eof, or the tq_join_next* call that returns its
+ * rows.  Skewed probe keys that overflow a partition slab are still joined: the batch is then re-run on the exact
+ * (histogram) path, which costs one host read of the counts, a device copy of every region's rows into one buffer, and a
+ * second probe pass.  Later segmented batches on the handle start on the streaming path again. */
 int32_t tq_join_put_probe_segments(tq_join *j, int32_t n_segs, const tq_column *cols, const uint64_t *const *seg_counts, int64_t seg_cap);
 /* Fills at most max_rows joined rows into out_cols (n_build_cols + n_probe_cols caller-
  * allocated columns, host memory).  *n_rows == 0 with *eof == 0 means "feed more probe

@@ -206,6 +206,11 @@ extern "C" int32_t tq_last_error(char *buf, int32_t buf_len) {
   return TQ_OK;
 }
 
+// The library's placement hashes themselves (common.cuh), for tests/test_hash_targets.py: the key-aiming edge tests restate
+// them in Python, and this is what keeps the restatement honest.  Test-only exports, not part of the product ABI.
+extern "C" uint64_t tq_emu_hash_key(uint64_t k) { return tqd::hash_key(k); }
+extern "C" uint64_t tq_emu_mix64(uint64_t k) { return tqd::mix64(k); }
+
 // "device" memory is host memory here
 extern "C" int32_t tq_init(int32_t) { return TQ_OK; }
 extern "C" int32_t tq_memcpy_d2h(void *dst, const void *src, size_t bytes) { if (bytes) memcpy(dst, src, bytes); return TQ_OK; }

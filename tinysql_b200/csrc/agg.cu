@@ -563,8 +563,9 @@ struct tq_agg {
   MultiKeyEncoder mk;       // several GROUP BY columns: exact fold of the key tuple into one 64-bit word (dict.cuh)
   DevBuf mk_comb;
   // shared-memory pre-aggregation of large batches (k_agg_preagg)
-  bool pre_disabled = false;
+  bool pre_disabled = false;     // TQ_AGG_NO_PREAGG=1, or a batch gave up on the pre-aggregation: the general path from now on
   bool pre_partitioned = true;   // TQ_AGG_PREAGG_PART=0: do not pre-aggregate when the groups need radix partitioning
+  bool pre_force_part = false;   // TQ_AGG_PREAGG_PART=1: also in the middle range where the general path wins
   int64_t known_groups = 0;  // groups in the table after the last batch
   std::vector<DevBuf> pre_slabs, pre_out;
   DevBuf pre_aos;
@@ -681,8 +682,7 @@ static int32_t agg_update_device(tq_agg *a, const DCol *cols, int n_in_cols, int
 // Try the shared-memory pre-aggregation path for one raw batch; *done tells whether the batch was consumed.
 static int32_t agg_try_preagg(tq_agg *a, const DCol *cols, int64_t n, bool *done) {
   *done = false;
-  static const bool disabled_by_env = [] { const char *e = getenv("TQ_AGG_NO_PREAGG"); return e && e[0] == '1'; }();
-  if (disabled_by_env || a->pre_disabled || a->any_kind || a->n_group_by != 1 || n < (1 << 20) || n > 0xFFFFFFF0ll) return TQ_OK;
+  if (a->pre_disabled || a->any_kind || a->n_group_by != 1 || n < (1 << 20) || n > 0xFFFFFFF0ll) return TQ_OK;
   const int kc = a->key_col;
   if (a->types[kc] == TQ_TYPE_FLOAT64 || cols[kc].bm != nullptr) return TQ_OK;  // integer key without NULLs
   const int64_t g_est = a->known_groups > a->est_groups ? a->known_groups : a->est_groups;
@@ -724,8 +724,7 @@ static int32_t agg_try_preagg(tq_agg *a, const DCol *cols, int64_t n, bool *done
   if (pbits > 0 && !a->pre_partitioned) return TQ_OK;
   // Partitioned vs general path (scripts/agg_pre_probe.py, H100): in the middle range (4 to 128 partitions, up to 307,200
   // groups) the general table is still cache-friendly and the scatter is pure overhead, so it stays on the general path.
-  static const bool force_part = [] { const char *e = getenv("TQ_AGG_PREAGG_PART"); return e && e[0] == '1'; }();
-  if (pbits >= 2 && pbits <= 7 && !force_part) return TQ_OK;
+  if (pbits >= 2 && pbits <= 7 && !a->pre_force_part) return TQ_OK;
   Runtime &r = rt();
   cudaStream_t s = r.compute;
   const int P = 1 << pbits;
@@ -1103,7 +1102,9 @@ int32_t tq_agg_create(const tq_agg_desc *d, tq_agg **out) {
   a->n_group_by = d->n_group_by;
   a->n_funcs = d->n_funcs;
   a->est_groups = d->est_groups;
-  { const char *e = getenv("TQ_AGG_PREAGG_PART"); a->pre_partitioned = !(e && e[0] == '0'); }  // on by default since the AoS scatter + native 32-bit counts (2.88 vs 3.18 ms at 1e6 groups); =0 turns it off
+  // the pre-aggregation switches are read per handle, so a handle's path never depends on which handle came first
+  { const char *e = getenv("TQ_AGG_PREAGG_PART"); a->pre_partitioned = !(e && e[0] == '0'); a->pre_force_part = e && e[0] == '1'; }  // on by default since the AoS scatter + native 32-bit counts (2.88 vs 3.18 ms at 1e6 groups); =0 turns it off
+  { const char *e = getenv("TQ_AGG_NO_PREAGG"); a->pre_disabled = e && e[0] == '1'; }
   for (int c = 0; c < a->n_cols; c++) {
     const int t = d->input_types[c] & 0xFF;
     a->in_kind[c] = t == TQ_TYPE_FLOAT32 ? 1 : (t == TQ_TYPE_BYTES ? 2 : 0);

@@ -40,7 +40,7 @@ static constexpr int64_t PART_MIN_BUILD_ROWS = 1 << 18;  // below this the whole
 static constexpr int PART_MAX_BITS = 12;
 static constexpr uint64_t PART_MAX_SMEM_BYTES = 128 << 10;  // a partition table image that still fits in shared memory
 static const int64_t g_tiles_per_cta = 8;
-static int64_t g_part_target_rows = 150000;              // build rows per partition: a partition table ~ 4-8 MB, a few live ones fit in L2
+static constexpr int64_t PART_TARGET_ROWS = 150000;      // build rows per partition: a partition table ~ 4-8 MB, a few live ones fit in L2
 static const int64_t g_max_load_pct = 50;                // partition-table load-factor bound (pair probing keeps chains short)
 static bool g_no_fast_kernel = false;                    // TQ_JOIN_NO_FAST=1: use the generic kernels (tests)
 
@@ -1476,6 +1476,10 @@ struct ProbeInputSet {  // device copy of one host probe batch
   ~ProbeInputSet() { if (ev_h2d) cudaEventDestroy(ev_h2d); }
 };
 
+// A segmented probe batch (tq_join_put_probe_segments): n device regions of `cap` rows each; region g holds *cnt[g] rows,
+// column c of it starts at col[g][c].  n == 0: an ordinary batch.
+struct SegSpec { int n = 0; int64_t cap = 0; const uint64_t *col[SA_MAX_SEGS][4]; const unsigned long long *cnt[SA_MAX_SEGS]; };
+
 struct PendingBatch {  // a launched probe batch whose row count has not been read back yet
   bool active = false;
   std::unique_ptr<ResultBatch> rb;
@@ -1484,7 +1488,7 @@ struct PendingBatch {  // a launched probe batch whose row count has not been re
   const uint8_t *d_selected = nullptr;
   int64_t n = 0;
   bool want_host = false;
-  bool segmented = false;
+  SegSpec seg;                  // the regions of a segmented batch (re-read by the re-run after a slab overflow)
   int cursor_slot = 0;
   cudaEvent_t ev_k = nullptr;
 };
@@ -1563,6 +1567,7 @@ struct tq_join {
   int64_t n_valid = 0, n_distinct = 0;
   bool build_unique = true;
   int64_t build_ns = 0;
+  int64_t part_rows = PART_TARGET_ROWS;   // build rows per partition table (TQ_JOIN_PART_ROWS at tq_join_create, tests)
 
   // ---- probe side
   std::vector<HostAccum> p_host;
@@ -1580,7 +1585,8 @@ struct tq_join {
   DevBuf part_aos[2], pos_base[2], pos_valid[2], hole_pos[2], hole_src[2], hole_scan;
   DevBuf b_aos;                           // build-side AoS slabs (released after the build)
   // segmented probe batch (tq_join_put_probe_segments): consumed by the next launch_probe_stream
-  struct SegSpec { int n = 0; int64_t cap = 0; const uint64_t *col[SA_MAX_SEGS][4]; const unsigned long long *cnt[SA_MAX_SEGS]; } seg;
+  SegSpec seg;
+  DevBuf seg_gather[4];                   // a segmented batch whose slab overflowed, gathered into one range per column
   DevBuf scan_scratch2;
   PinBuf cursors_host;
   PendingBatch pending;
@@ -1672,10 +1678,11 @@ static bool stream_build_ok(const tq_join *j) {
 }
 
 // Whether probe batches may take the streaming positional path (launch_probe_stream) as far as the operator and its table
-// decide: a partitioned ROW-mode table with unique NOT NULL build rows, an inner join without OtherConditions, at most 4
-// columns per side, and optimistic slabs (no slab has overflowed yet).  The callers add what depends on the batch.
+// decide: a partitioned ROW-mode table with unique NOT NULL build rows, an inner join without OtherConditions, and at most 4
+// columns per side.  The callers add what depends on the batch: launch_probe requires optimistic slabs (no slab has
+// overflowed yet) for ordinary batches; a segmented batch always starts on this path (only k_scatter_aos reads regions).
 static bool stream_probe_ok(const tq_join *j) {
-  return j->pbits > 0 && j->pbits <= SA_MAX_PBITS && j->row_mode && j->join_type == TQ_JOIN_INNER && !j->build_has_nulls && j->optimistic_scatter &&
+  return j->pbits > 0 && j->pbits <= SA_MAX_PBITS && j->row_mode && j->join_type == TQ_JOIN_INNER && !j->build_has_nulls &&
          j->n_probe_cols <= 4 && j->n_build_cols <= 4 && !j->has_oc && !g_no_fast_kernel;
 }
 
@@ -1689,7 +1696,7 @@ static int32_t try_stream_build(tq_join *j, bool *done) {
   const int64_t n = j->n_build;
   const int NB = j->n_build_cols;
   int pbits = 0;
-  while (((uint64_t)g_part_target_rows << pbits) < (uint64_t)n) pbits++;
+  while (((uint64_t)j->part_rows << pbits) < (uint64_t)n) pbits++;
   if (pbits > SA_MAX_PBITS) pbits = SA_MAX_PBITS;
   if (pbits < 1) return TQ_OK;
   const int P = 1 << pbits;
@@ -1837,12 +1844,12 @@ static int32_t join_build(tq_join *j) {
   const bool row_candidate = row_words <= 4;
   const int shift = (row_candidate && row_words > 2) ? 2 : 1;
   j->shift = shift;
-  // Partitioning: ~g_part_target_rows build rows per partition table; small build sides keep ONE table.
+  // Partitioning: ~j->part_rows build rows per partition table; small build sides keep ONE table.
   uint64_t n_slots = 64, cap = 0;
   int pbits = 0;
   if (n >= PART_MIN_BUILD_ROWS) {
     uint64_t P = 1;
-    while (P * (uint64_t)g_part_target_rows < (uint64_t)n) P <<= 1;
+    while (P * (uint64_t)j->part_rows < (uint64_t)n) P <<= 1;
     while ((1ull << pbits) < P) pbits++;
     if (pbits > PART_MAX_BITS) pbits = PART_MAX_BITS;
     P = 1ull << pbits;
@@ -2200,7 +2207,7 @@ static int32_t launch_probe(tq_join *j, const std::vector<DCol> &probe, const ui
   // result is positional: room for the padding of every partition to 32 rows.
   bool any_in_bm = false;
   for (int c = 0; c < j->n_probe_cols; c++) any_in_bm |= (probe[c].bm != nullptr);
-  const bool pos_path = stream_probe_ok(j) && !any_in_bm;
+  const bool pos_path = stream_probe_ok(j) && !any_in_bm && (j->optimistic_scatter || j->seg.n);
   const uint64_t alloc_rows = capacity + (pos_path ? 32ull * ((1ull << j->pbits) + 2) : 0);
   for (int c = 0; c < ncols; c++) {
     TQ_TRY(rb->cols[c].data.reserve((size_t)(alloc_rows ? alloc_rows : 1) * 8));
@@ -2421,6 +2428,37 @@ static int32_t apply_other_conditions(tq_join *j, ResultBatch *rb, int64_t n_pro
   return TQ_OK;
 }
 
+// A segmented batch whose optimistic slab overflowed: the exact histogram path reads one contiguous range, so the regions'
+// rows are copied into one buffer per column.  The batch's kernels are complete, so the counts are read on the host here
+// (a region whose count exceeds its capacity reads as empty, as in k_scatter_aos).  pb then describes the gathered batch.
+static int32_t gather_segments(tq_join *j, PendingBatch &pb) {
+  cudaStream_t s = rt().compute;
+  const SegSpec &g = pb.seg;
+  const int T = scatter_aos_tile(j->n_probe_cols, (1 << j->pbits) + 2);
+  const uint64_t seg_rows = (uint64_t)((g.cap + T - 1) / T * T);
+  unsigned long long cnt[SA_MAX_SEGS];
+  for (int r = 0; r < g.n; r++) TQ_CUDA(cudaMemcpyAsync(&cnt[r], g.cnt[r], 8, cudaMemcpyDeviceToHost, s));
+  TQ_CUDA(cudaStreamSynchronize(s));
+  uint64_t total = 0;
+  for (int r = 0; r < g.n; r++) {
+    if (cnt[r] > seg_rows) cnt[r] = 0;
+    total += cnt[r];
+  }
+  for (int c = 0; c < j->n_probe_cols; c++) {
+    TQ_TRY(j->seg_gather[c].reserve((size_t)(total ? total : 1) * 8));
+    uint64_t at = 0;
+    for (int r = 0; r < g.n; r++) {
+      if (cnt[r]) TQ_CUDA(cudaMemcpyAsync(j->seg_gather[c].as<uint64_t>() + at, g.col[r][c], (size_t)cnt[r] * 8, cudaMemcpyDeviceToDevice, s));
+      at += cnt[r];
+    }
+    pb.probe[c].data = j->seg_gather[c].as<uint64_t>();
+    pb.probe[c].bm = nullptr;
+  }
+  pb.n = (int64_t)total;
+  pb.seg.n = 0;
+  return TQ_OK;
+}
+
 // Wait for the pending batch, re-run it if the output did not fit, queue its result.
 static int32_t finalize_pending(tq_join *j) {
   PendingBatch &pb = j->pending;
@@ -2432,10 +2470,11 @@ static int32_t finalize_pending(tq_join *j) {
   float ms = 0;
   if (cudaEventElapsedTime(&ms, j->ev_a[pb.cursor_slot], j->ev_b[pb.cursor_slot]) == cudaSuccess) j->last_probe_ns = (int64_t)(ms * 1e6);
   else cudaGetLastError();
-  if (hc[2] && pb.segmented) { set_error("segmented probe batch: a partition slab overflowed (heavily skewed keys)"); return TQ_ERR_INVALID_ARG; }
   if (hc[2]) {
     // a partition slab of the optimistic (histogram-free) scatter was too small — skewed keys: exact offsets from now on
+    // (for ordinary batches; a segmented batch always tries the slabs first, and is gathered for its re-run)
     j->optimistic_scatter = false;
+    if (pb.seg.n) TQ_TRY(gather_segments(j, pb));
     TQ_TRY(launch_probe(j, pb.probe, pb.d_selected, pb.n, pb.rb.get(), pb.rb->capacity, pb.cursor_slot));
     TQ_CUDA(cudaStreamSynchronize(r.compute));
     produced = hc[0];
@@ -2506,6 +2545,8 @@ static int32_t start_batch(tq_join *j, const std::vector<DCol> &probe, const uin
   const uint64_t capacity = (uint64_t)n;
   std::unique_ptr<ResultBatch> rb = get_result_batch(j);
   TQ_TRY(launch_probe(j, *pin, d_selected, n, rb.get(), capacity, slot));
+  const SegSpec seg = j->seg;
+  j->seg.n = 0;  // consumed by this launch: a re-run of the previous batch in finalize_pending must not read these regions
   cudaEvent_t ev = nullptr;
   TQ_CUDA(cudaEventCreateWithFlags(&ev, cudaEventDisableTiming));
   TQ_CUDA(cudaEventRecord(ev, r.compute));
@@ -2519,8 +2560,7 @@ static int32_t start_batch(tq_join *j, const std::vector<DCol> &probe, const uin
   pb.d_selected = d_selected;
   pb.n = n;
   pb.want_host = want_host;
-  pb.segmented = j->seg.n != 0;
-  j->seg.n = 0;
+  pb.seg = seg;
   pb.cursor_slot = slot;
   j->probe_rows_total += n;
   return TQ_OK;
@@ -2645,9 +2685,10 @@ int32_t tq_join_create(const tq_join_desc *d, tq_join **out) {
   if (d->join_type == TQ_JOIN_LEFT_OUTER && d->outer_is_right) { set_error("left outer join needs outer_is_right == 0"); return TQ_ERR_INVALID_ARG; }
   if (d->join_type == TQ_JOIN_RIGHT_OUTER && !d->outer_is_right) { set_error("right outer join needs outer_is_right == 1"); return TQ_ERR_INVALID_ARG; }
   { const char *e = getenv("TQ_JOIN_NO_FAST"); g_no_fast_kernel = e && e[0] == '1'; }
-  { const char *e = getenv("TQ_JOIN_PART_ROWS"); if (e && atoll(e) > 0) g_part_target_rows = atoll(e); }
   tq_join *j = new (std::nothrow) tq_join();
   if (!j) return TQ_ERR_OOM;
+  // per handle: unset or not a positive number means the default, whatever an earlier handle was created with
+  { const char *e = getenv("TQ_JOIN_PART_ROWS"); if (e && atoll(e) > 0) j->part_rows = atoll(e); }
   j->join_type = d->join_type;
   j->outer_is_right = d->outer_is_right ? 1 : 0;
   j->nb_user = d->n_build_cols;
