@@ -223,8 +223,9 @@ int32_t tq_vec_filter_string(int64_t n, const tq_column *a, uint8_t *selected, i
  *                        row in the set (nulls[] quirk, expression.go:249-259) but it is not selected.
  *   TQ_X_COMPACT       : the Selection → Projection boundary: only selected rows remain in the set.
  * Outputs are dense (all n rows; values of unselected rows are unspecified); selected (n bytes, may be
- * NULL when no FILTER op is present) is Go's []bool.  Errors are the first of the reference's overflow
- * errors any in-set row raises (same codes as tq_vec_arith_*). */
+ * NULL when no FILTER op is present) is Go's []bool.  The error is the error of the first op, in program
+ * order, that raises on an in-set row (same codes as tq_vec_arith_*): the reference evaluates children
+ * before parents, CNF items and projections in order, and returns at the first op that raises. */
 enum { TQ_X_CONST = 0, TQ_X_CMP_INT, TQ_X_CMP_REAL, TQ_X_ARITH_INT, TQ_X_ARITH_REAL, TQ_X_LOGIC, TQ_X_UNARY,
        TQ_X_IF, TQ_X_IFNULL, TQ_X_FILTER, TQ_X_COMPACT };
 #define TQ_EXPR_MAX_INPUTS 8

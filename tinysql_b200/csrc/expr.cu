@@ -596,7 +596,7 @@ int32_t tq_expr_eval(int64_t n, int32_t n_inputs, const tq_column *inputs, int32
   ErrOut eo;
   TQ_TRY(run_map(n, mem, n_inputs, ins, n_outputs, op, launch, &eo, &rs));
   if (div_by_zero_warnings) *div_by_zero_warnings = (int64_t)eo.counter;
-  return err_to_status(eo.err, "expression program");
+  return xp_err_to_status(eo.err, P.ops, "expression program");
 }
 
 }  // extern "C"

@@ -24,12 +24,23 @@ struct XOp {
   uint64_t imm;
 };
 
-// The first overflow error of the bits an evaluation raised, in the order the reference's checks would name them.
+// The status of the ERR_* bits a single builtin raised (a builtin raises one kind only).
 static inline int32_t err_to_status(unsigned e, const char *what) {
   if (e & ERR_UBIGINT) { set_error("BIGINT UNSIGNED value is out of range in '%s'", what); return TQ_ERR_OVERFLOW_BIGINT_UNSIGNED; }
   if (e & ERR_BIGINT) { set_error("BIGINT value is out of range in '%s'", what); return TQ_ERR_OVERFLOW_BIGINT; }
   if (e & ERR_DOUBLE) { set_error("DOUBLE value is out of range in '%s'", what); return TQ_ERR_OVERFLOW_DOUBLE; }
   return TQ_OK;
+}
+
+// The status of a program run; bit i of `raised`: op i raised on a row of its evaluation set.  The reference evaluates
+// vectorized, children before parents, CNF items and projections in order, and returns at the first op that raises, so the
+// lowest such op decides, and its kind follows from the op: integer arithmetic with an unsigned operand raises BIGINT
+// UNSIGNED, signed integer arithmetic and unary minus BIGINT, real arithmetic DOUBLE.
+static inline int32_t xp_err_to_status(unsigned raised, const XOp *ops, const char *what) {
+  if (!raised) return TQ_OK;
+  const XOp &x = ops[__builtin_ctz(raised)];
+  if (x.kind == TQ_X_ARITH_REAL) return err_to_status(ERR_DOUBLE, what);
+  return err_to_status(x.kind == TQ_X_ARITH_INT && (x.flags & 3) ? ERR_UBIGINT : ERR_BIGINT, what);
 }
 
 // Checks a tq_expr_op program over n_inputs input registers and decodes it into out[0, n_ops).  *want_counter: the program
@@ -274,7 +285,9 @@ struct FIfNull {
 //   alive — the row is still in the evaluation set (sel slice): errors and warnings of later ops count for it;
 //   sel   — the row passes every FILTER item seen so far.
 // Both start as `active`.  An ETInt NULL item leaves the row alive but not selected (the nulls[] quirk); TQ_X_COMPACT (the
-// Selection -> Projection boundary) keeps only selected rows alive.  err collects ERR_* bits, cnt division-by-zero warnings.
+// Selection -> Projection boundary) keeps only selected rows alive.  err collects bit i when op i raises for the row while it is
+// alive (XP_MAX_OPS <= 32: one word, see xp_err_to_status), cnt division-by-zero warnings.
+static_assert(XP_MAX_OPS <= 32, "the raise mask of a program is one 32-bit word");
 template <int NREGS>
 __device__ __forceinline__ void xp_run_row(const XOp *ops, int n_ops, int n_in, uint64_t (&rv)[NREGS], uint64_t &nn, bool active, bool &alive,
                                            bool &sel, unsigned &err, unsigned &cnt) {
@@ -316,7 +329,7 @@ __device__ __forceinline__ void xp_run_row(const XOp *ops, int n_ops, int n_in, 
       }
       default: alive = sel; break;                                 // TQ_X_COMPACT: Selection hands only selected rows on
     }
-    if (alive) { err |= e_; cnt += c_; }
+    if (alive) { err |= e_ ? 1u << i : 0u; cnt += c_; }
     rv[n_in + i] = o1[0];
     nn = (nn & ~(1ull << (n_in + i))) | ((uint64_t)on[0] << (n_in + i));
   }

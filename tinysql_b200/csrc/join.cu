@@ -1462,7 +1462,7 @@ struct ResultBatch {
   std::vector<PinBuf> h_data, h_bm;
   std::vector<VarOut> var;   // gathered FLOAT / var-len output columns (indexed like cols)
   std::vector<DevColBuf> alt;  // OtherConditions: the filtered copy of cols (swapped in)
-  unsigned oc_err = 0;         // OtherConditions: ERR_* bits its rows raised; the call that delivers the batch reports them
+  unsigned oc_err = 0;         // OtherConditions: ops that raised on its rows (bit i: op i); the call that delivers the batch reports the first
   bool on_host = false;
   cudaEvent_t ev_ready = nullptr;
   ~ResultBatch() { if (ev_ready) cudaEventDestroy(ev_ready); }
@@ -3137,7 +3137,7 @@ static int32_t join_current_batch(tq_join *j, int64_t max_rows, int *have, int32
     j->host_cur = std::move(j->results.front());
     j->results.pop_front();
     j->host_cur_pos = 0;
-    if (j->host_cur->oc_err) return err_to_status(j->host_cur->oc_err, "other conditions");
+    if (j->host_cur->oc_err) return xp_err_to_status(j->host_cur->oc_err, j->oc.prog.ops, "other conditions");
     if (!j->host_cur->on_host) {
       // Large consumer buffers: copy straight from HBM into the caller's columns (no staging, no CPU memcpy).
       // (a queued batch is complete: finalize_pending waited for its kernels — no stream-wide sync here, so the copy
@@ -3257,7 +3257,7 @@ int32_t tq_join_next_device(tq_join *j, tq_column *out_cols, int64_t *n_rows, in
   }
   j->lent = std::move(j->results.front());
   j->results.pop_front();
-  if (j->lent->oc_err) return err_to_status(j->lent->oc_err, "other conditions");
+  if (j->lent->oc_err) return xp_err_to_status(j->lent->oc_err, j->oc.prog.ops, "other conditions");
   const int ncols = j->nb_user + j->np_user;
   for (int c = 0; c < ncols; c++) {
     out_cols[c].length = j->lent->n;

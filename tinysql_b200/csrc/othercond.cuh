@@ -33,7 +33,7 @@ struct OcCols {
 };
 
 // Filters n joined rows into the out_* columns (caller-allocated for n rows, bitmaps zeroed here); *n_out = rows kept,
-// *err = the ERR_* bits and *div_by_zero = the division-by-zero warnings the key-matched rows raised.
+// *err = the ops that raised on key-matched rows (bit i: op i), *div_by_zero = the division-by-zero warnings they raised.
 int32_t oc_filter(const OcPlan &plan, const OcCols &cols, int64_t n, int64_t n_probe_rows, DevBuf &scratch, DevBuf &scan_scratch, int64_t *n_out,
                   unsigned *err, int64_t *div_by_zero, cudaStream_t s);
 

@@ -295,7 +295,7 @@ struct MJProg {
   int inner[JP_MAX_IN] = {};   // 1: register k comes from the inner row, 0: from the outer row
   XOp ops[XP_MAX_OPS] = {};
 };
-// err_warn[0] |= ERR_* bits, err_warn[1] += division-by-zero warnings of the evaluated pairs
+// err_warn[0] |= bit i for each op i that raised, err_warn[1] += division-by-zero warnings of the evaluated pairs
 __global__ void __launch_bounds__(256) k_mj_prog(const __grid_constant__ MJProg P, const uint32_t *__restrict__ out_outer, const uint32_t *__restrict__ out_inner,
                                                  int64_t m, uint32_t *__restrict__ flags, unsigned long long *err_warn) {
   const int64_t stride = (int64_t)gridDim.x * blockDim.x;
@@ -769,7 +769,7 @@ struct tq_mjoin {
   std::vector<uint8_t> dflt_nn;
   int oc_form = 0;                   // OtherConditions: 0 none, 1 tq_mjoin_set_other_conditions, 2 tq_mjoin_set_other_program
   JoinProg oc;                       // input registers name output columns (left ++ right)
-  unsigned oc_err = 0;               // ERR_* bits the program raised: the calls that deliver the result report them
+  unsigned oc_err = 0;               // ops that raised (bit i: op i): the calls that deliver the result report the first
   int64_t oc_warnings = 0;
   bool finished = false;
   ResultHost res;
@@ -1294,7 +1294,7 @@ extern "C" {
 int32_t tq_mjoin_next_bytes(tq_mjoin *h, int64_t max_rows, int64_t *bytes_per_col) {
   if (!h || !bytes_per_col || max_rows <= 0) return TQ_ERR_INVALID_ARG;
   if (!h->finished) { set_error("next before finish"); return TQ_ERR_STATE; }
-  if (h->oc_err) return err_to_status(h->oc_err, "other conditions");
+  if (h->oc_err) return xp_err_to_status(h->oc_err, h->oc.ops, "other conditions");
   TQ_TRY(mjoin_host_result(h));
   return result_next_bytes(h->res, max_rows, bytes_per_col);
 }
@@ -1302,7 +1302,7 @@ int32_t tq_mjoin_next_bytes(tq_mjoin *h, int64_t max_rows, int64_t *bytes_per_co
 int32_t tq_mjoin_next(tq_mjoin *h, int64_t max_rows, tq_column *out_cols, int64_t *n_rows, int32_t *eof) {
   if (!h || !out_cols || !n_rows || !eof || max_rows <= 0) return TQ_ERR_INVALID_ARG;
   if (!h->finished) { set_error("next before finish"); return TQ_ERR_STATE; }
-  if (h->oc_err) return err_to_status(h->oc_err, "other conditions");
+  if (h->oc_err) return xp_err_to_status(h->oc_err, h->oc.ops, "other conditions");
   TQ_TRY(mjoin_host_result(h));
   return result_next(h->res, max_rows, out_cols, n_rows, eof);
 }
@@ -1311,7 +1311,7 @@ int32_t tq_mjoin_next(tq_mjoin *h, int64_t max_rows, tq_column *out_cols, int64_
 int32_t tq_mjoin_next_device(tq_mjoin *h, tq_column *out_cols, int64_t *n_rows, int32_t *eof) {
   if (!h || !out_cols || !n_rows || !eof) return TQ_ERR_INVALID_ARG;
   if (!h->finished) { set_error("next before finish"); return TQ_ERR_STATE; }
-  if (h->oc_err) return err_to_status(h->oc_err, "other conditions");
+  if (h->oc_err) return xp_err_to_status(h->oc_err, h->oc.ops, "other conditions");
   TQ_TRY(ensure_init());
   Runtime &r = rt();
   std::lock_guard<std::recursive_mutex> lk(r.mu);
