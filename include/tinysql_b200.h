@@ -49,7 +49,8 @@ enum {
                         *   group item / argument it counts as float64(f) (util/codec/codec.go:226-229).  Host memory only. */
   TQ_TYPE_BYTES = 5,   /* var-len (VARCHAR, BLOB, ...): offsets = length+1 int64 (Go's Column.offsets), data = the cells' bytes.
                         *   HashJoin key or payload, HashAgg GROUP BY item or COUNT / MAX / MIN / FIRSTROW argument; compared
-                        *   byte-wise (compactBytesFlag, codec.go:230-233).  Host memory only.                              */
+                        *   byte-wise (compactBytesFlag, codec.go:230-233).  Host or device memory (TQ_MEM_DEVICE rules at
+                        *   tq_column below).                                                                               */
   /* OR-ed into a tq_agg_desc.input_types entry: the column's FieldType carries mysql.NotNullFlag.  Lets HashAgg
    * drop the per-group "saw a non-NULL input" word of SUM / MAX / MIN (16-byte instead of 32-byte group records
    * for SUM + COUNT); any null bitmap passed for such a column is ignored. */
@@ -69,7 +70,17 @@ enum {
  * For outputs the caller provides both buffers (capacity >= the rows it asks for).
  * TQ_MEM_DEVICE columns (not Go memory) have stricter rules, checked by the vectorized-builtin calls: data
  * 16-byte aligned; null_bitmap 8-byte aligned and allocated as ((length + 63) / 64) * 8 bytes — the kernels move
- * whole 64-row bitmap groups. */
+ * whole 64-row bitmap groups.
+ * A var-len TQ_MEM_DEVICE column given to tq_join_put_build / _put_probe, tq_agg_put, tq_sort_put or tq_mjoin_put_*:
+ * offsets = length + 1 int64 in device memory, 8-byte aligned, non-decreasing; offsets[0] may be non-zero (a sliced column,
+ * a cell range of a lent result) and cell i is data[offsets[i], offsets[i + 1]); data has any alignment (may be NULL when
+ * every cell is empty); null_bitmap as for the other device columns.  The offsets are never read on the host: a put reads
+ * back offsets[0], offsets[length] and the longest cell once, and refuses offsets that go backwards (TQ_ERR_INVALID_ARG).
+ * Every such put copies (join, sort, merge join) or encodes (aggregation) the cells before it returns, so the caller may
+ * reuse offsets and data right away; the null_bitmap follows the rule of the operator's 8-byte device columns (sort, merge
+ * join, aggregation: copied too; join build: borrowed until tq_join_finalize_build; join probe: borrowed until the batch is
+ * finished — the next tq_join_put_probe, tq_join_probe_eof or the tq_join_next* call that returns its rows).
+ * FLOAT columns (TQ_TYPE_FLOAT32) come from host memory only: a TQ_MEM_DEVICE put refuses them (TQ_ERR_UNSUPPORTED_TYPE). */
 typedef struct tq_column {
   int64_t length;
   uint8_t *null_bitmap;
@@ -379,8 +390,9 @@ int32_t tq_chunk_decode(const uint8_t *buffer, int64_t len, int32_t n_cols, cons
  * (util/chunk/codec.go:92-143,246-353; distsql/select_result.go:102-141 is where the reference decodes on the CPU).
  * out[c] receives DEVICE pointers — data (8-byte slots; 4-byte slots for FLOAT; the cells' bytes for var-len columns),
  * offsets (var-len only) and null_bitmap (NULL when the column has no NULLs; otherwise 8-byte aligned words, tail bits 0) —
- * which the TQ_MEM_DEVICE entry points accept as they are (tq_join_put_build / put_probe, tq_agg_put, tq_vec_*, tq_expr_eval:
- * 8-byte column types).  *chunk == NULL creates a handle; passing the same handle again reuses its device memory (the
+ * which the TQ_MEM_DEVICE entry points accept as they are (tq_join_put_build / put_probe, tq_agg_put, tq_sort_put,
+ * tq_mjoin_put_*: 8-byte and var-len columns, FLOAT columns are refused; tq_vec_*, tq_expr_eval: their operand types).
+ * *chunk == NULL creates a handle; passing the same handle again reuses its device memory (the
  * previous columns become invalid).  The call returns after the bytes have left `buffer` and the columns are complete. */
 typedef struct tq_chunk_device tq_chunk_device;
 int32_t tq_chunk_decode_device(const uint8_t *buffer, int64_t len, int32_t n_cols, const int32_t *types, tq_chunk_device **chunk,
@@ -487,8 +499,8 @@ typedef struct tq_sort_desc {
 } tq_sort_desc;
 typedef struct tq_sort tq_sort;
 int32_t tq_sort_create(const tq_sort_desc *desc, tq_sort **out);
-/* Chunks come from host memory (all chunk layouts) or, for 8-byte column types, from HBM (TQ_MEM_DEVICE: e.g. the rows
- * tq_join_next_device lends) — one or the other per handle.  With device chunks the rows never leave the GPU: tq_sort_next_device
+/* Chunks come from host memory (all chunk layouts) or, for 8-byte and var-len column types, from HBM (TQ_MEM_DEVICE: e.g. the
+ * rows tq_join_next_device lends; FLOAT columns come from host memory only) — one or the other per handle.  With device chunks the rows never leave the GPU: tq_sort_next_device
  * lends the result (the TopN window) as device columns, and tq_sort_next copies it to the host only if it is called. */
 int32_t tq_sort_put(tq_sort *s, const tq_column *cols, int32_t mem);
 int32_t tq_sort_eof(tq_sort *s);
@@ -533,7 +545,7 @@ int32_t tq_mjoin_set_other_conditions(tq_mjoin *j, int32_t n_conds, const tq_joi
 int32_t tq_mjoin_set_other_program(tq_mjoin *j, int32_t n_inputs, const int32_t *input_cols, int32_t n_ops, const tq_expr_op *ops);
 /* division-by-zero warnings raised by joined rows in the evaluation set (handleDivisionByZeroError, builtin_arithmetic_vec.go:369-375) */
 int32_t tq_mjoin_warnings(tq_mjoin *j, int64_t *div_by_zero);
-/* host chunks (all layouts) or, for 8-byte column types, device chunks (TQ_MEM_DEVICE) — per child one or the other */
+/* host chunks (all layouts) or, for 8-byte and var-len column types, device chunks (TQ_MEM_DEVICE) — per child one or the other */
 int32_t tq_mjoin_put_inner(tq_mjoin *j, const tq_column *cols, int32_t mem);
 int32_t tq_mjoin_put_outer(tq_mjoin *j, const tq_column *cols, const uint8_t *selected, int32_t mem); /* selected: HOST Go []bool or NULL */
 int32_t tq_mjoin_finish(tq_mjoin *j);   /* both children exhausted */

@@ -183,7 +183,8 @@ class DeviceColumn:
     def __init__(self, tp, n, with_bitmap=True):
         lib = L.load()
         if tp in (FLOAT32, BYTES):
-            raise ValueError("DeviceColumn holds 8-byte slots (INT64 / UINT64 / FLOAT64); FLOAT32 and var-len columns enter through host chunks")
+            raise ValueError("DeviceColumn holds 8-byte slots (INT64 / UINT64 / FLOAT64); DeviceColumn.from_host puts a var-len column "
+                             "into a DeviceVarColumn; FLOAT32 columns enter through host chunks")
         self.tp, self.length = tp, int(n)
         self._data = C.c_void_p()
         L.check(lib.tq_device_alloc(max(self.length, 1) * 8, C.byref(self._data)))
@@ -195,6 +196,9 @@ class DeviceColumn:
 
     @classmethod
     def from_host(cls, col):
+        """the column in HBM: a DeviceColumn, or a DeviceVarColumn for a var-len (BYTES) column"""
+        if col.tp == BYTES:
+            return DeviceVarColumn.from_host(col)
         d = cls(col.tp, col.length, with_bitmap=col.bitmap is not None)
         lib = L.load()
         if col.length:
@@ -223,6 +227,79 @@ class DeviceColumn:
         if self._bm:
             lib.tq_device_free(self._bm)
             self._bm = C.c_void_p()
+
+
+class DeviceVarColumn:
+    """A var-len column in HBM (the TQ_MEM_DEVICE form of VarColumn): int64 offsets[length + 1] (8-byte aligned), the cells'
+    bytes and the padded NOT-NULL bitmap of DeviceColumn.  `lead` puts that many filler bytes before the first cell, so
+    offsets[0] == lead — the shape of a sliced column or of a cell range inside a larger buffer."""
+
+    def __init__(self):
+        self.tp, self.length, self.lead = BYTES, 0, 0
+        self.off_bytes = self.data_bytes = 0
+        self._off, self._data, self._bm = C.c_void_p(), C.c_void_p(), C.c_void_p()
+
+    @classmethod
+    def from_host(cls, col, lead=0):
+        assert col.tp == BYTES
+        lib = L.load()
+        d = cls()
+        d.length, d.lead = col.length, int(lead)
+        offs = (np.asarray(col.offsets, dtype=np.int64) - int(col.offsets[0]) + d.lead) if col.length else np.full(1, d.lead, dtype=np.int64)
+        nbytes = int(offs[-1])
+        data = np.empty(max(nbytes, 1), dtype=np.uint8)
+        data[: d.lead] = 0xEE
+        data[d.lead: nbytes] = col.data[int(col.offsets[0]): int(col.offsets[0]) + nbytes - d.lead]
+        d.off_bytes, d.data_bytes = offs.nbytes, data.nbytes
+        L.check(lib.tq_device_alloc(offs.nbytes, C.byref(d._off)))
+        L.check(lib.tq_memcpy_h2d(d._off, offs.ctypes.data, offs.nbytes))
+        L.check(lib.tq_device_alloc(data.nbytes, C.byref(d._data)))
+        L.check(lib.tq_memcpy_h2d(d._data, data.ctypes.data, data.nbytes))
+        if col.bitmap is not None:
+            bm_bytes = (((d.length + 63) >> 6) << 3) + 8
+            L.check(lib.tq_device_alloc(bm_bytes, C.byref(d._bm)))
+            L.check(lib.tq_memset_device(d._bm, 0, bm_bytes))
+            if d.length:
+                L.check(lib.tq_memcpy_h2d(d._bm, col.bitmap.ctypes.data, bitmap_bytes(d.length)))
+        return d
+
+    def tq(self, length=None):
+        t = L.TQColumn()
+        t.length = self.length if length is None else length
+        t.data = self._data.value
+        t.null_bitmap = self._bm.value
+        t.offsets = self._off.value
+        return t
+
+    def to_host(self):
+        return device_var_to_host(self._data.value, self._off.value, self._bm.value, self.length)
+
+    def free(self):
+        lib = L.load()
+        for name in ("_off", "_data", "_bm"):
+            p = getattr(self, name)
+            if p:
+                lib.tq_device_free(p)
+                setattr(self, name, C.c_void_p())
+
+
+def device_var_to_host(data_ptr, off_ptr, bm_ptr, n):
+    """a var-len column in device memory (offsets[0] may be non-zero) copied into a VarColumn"""
+    lib = L.load()
+    offs = np.zeros(n + 1, dtype=np.int64)
+    L.check(lib.tq_memcpy_d2h(offs.ctypes.data, off_ptr, offs.nbytes))
+    nbytes = int(offs[n] - offs[0])
+    data = np.zeros(max(nbytes, 1), dtype=np.uint8)
+    if nbytes:
+        L.check(lib.tq_memcpy_d2h(data.ctypes.data, data_ptr + int(offs[0]), nbytes))
+    nn = None
+    if bm_ptr and n:
+        bm = np.zeros(bitmap_bytes(n), dtype=np.uint8)
+        L.check(lib.tq_memcpy_d2h(bm.ctypes.data, bm_ptr, bm.nbytes))
+        nn = unpack_not_null(bm, n)
+    rel = offs - offs[0]
+    cells = [data[rel[i]: rel[i + 1]].tobytes() for i in range(n)]
+    return VarColumn(BYTES, [c if (nn is None or nn[i]) else None for i, c in enumerate(cells)], nn)
 
 
 def device_to_host(tp, data_ptr, bm_ptr, n):

@@ -555,6 +555,7 @@ struct tq_agg {
   int in_kind[AGG_MAXC] = {};  // 0 = 8-byte slots as declared, 1 = FLOAT (4-byte slots, widened on the device), 2 = var-len (dictionary-encoded on the device)
   bool any_kind = false;
   StringDict sd[AGG_MAXC];  // one dictionary per var-len input column: GROUP BY items and string arguments work on ids (strdict.cuh)
+  std::vector<DevBuf> dev_ids;  // var-len columns of device chunks: their dictionary ids (indexed like the input columns)
   int out_kind[AGG_MAXF] = {};  // result column i: 0 = 8-byte, 1 = FLOAT (narrowed back), 2 = var-len (gathered from sd[out_src[i]])
   int out_src[AGG_MAXF] = {};
   DevBuf lens_scratch, scan_scratch;
@@ -956,8 +957,10 @@ static int32_t agg_put_common(tq_agg *a, const tq_column *cols, int32_t mem, boo
     const int kind = col_kind(a, merge, c);
     if (kind != 2 && cols[c].offsets) { set_error("unsupport column type for encode (var-len data in fixed-width column %d)", c); return TQ_ERR_UNSUPPORTED_TYPE; }
     if (kind == 2 && !cols[c].offsets) { set_error("var-len column %d needs offsets", c); return TQ_ERR_INVALID_ARG; }
-    if (rows && !cols[c].data && !(kind == 2 && cols[c].offsets[rows] == cols[c].offsets[0])) return TQ_ERR_INVALID_ARG;
-    if (kind != 0 && mem != TQ_MEM_HOST) { set_error("FLOAT / var-len columns are accepted from host memory only"); return TQ_ERR_UNSUPPORTED_TYPE; }
+    // (the offsets of a device column are not read on the host: device_cell_span reads the two it needs)
+    if (mem == TQ_MEM_HOST && rows && !cols[c].data && !(kind == 2 && cols[c].offsets[rows] == cols[c].offsets[0])) return TQ_ERR_INVALID_ARG;
+    if (mem != TQ_MEM_HOST && rows && !cols[c].data && kind != 2) return TQ_ERR_INVALID_ARG;
+    if (kind == 1 && mem != TQ_MEM_HOST) { set_error("FLOAT columns are accepted from host memory only"); return TQ_ERR_UNSUPPORTED_TYPE; }
   }
   if (rows == 0) return TQ_OK;
   Runtime &r = rt();
@@ -967,6 +970,22 @@ static int32_t agg_put_common(tq_agg *a, const tq_column *cols, int32_t mem, boo
     TQ_TRY(agg_flush_stage(a, merge, n_in_cols));
     std::vector<DCol> view(n_in_cols);
     for (int c = 0; c < n_in_cols; c++) { view[c].data = (const uint64_t *)cols[c].data; view[c].bm = (const uint32_t *)cols[c].null_bitmap; }
+    if (a->dev_ids.size() < (size_t)n_in_cols) a->dev_ids.resize(n_in_cols);
+    for (int c = 0; c < n_in_cols; c++) {
+      if (col_kind(a, merge, c) != 2) continue;
+      // var-len: dictionary ids straight from the caller's cells (the dictionary keeps its own copy of every distinct string;
+      // insert mode: an id is valid iff the cell is NOT NULL, so the column's own bitmap stays the ids' bitmap)
+      int64_t b0 = 0, b1 = 0;
+      TQ_TRY(device_cell_span(cols[c].offsets, rows, &b0, &b1, r.compute));
+      if (b1 > b0 && !cols[c].data) { set_error("var-len device column %d with %lld bytes of cells but no data", c, (long long)(b1 - b0)); return TQ_ERR_INVALID_ARG; }
+      StrView v;
+      v.off = cols[c].offsets;
+      v.base = b0;
+      v.bytes = cols[c].data ? cols[c].data + b0 : nullptr;
+      TQ_TRY(a->dev_ids[c].reserve((size_t)rows * 8));
+      TQ_TRY(a->sd[c].encode(v, view[c].bm, rows, b1 - b0, /*insert=*/true, a->dev_ids[c].as<uint64_t>(), nullptr, r.compute));
+      view[c].data = a->dev_ids[c].as<uint64_t>();
+    }
     return agg_update_device(a, view.data(), n_in_cols, rows, merge);
   }
   // host chunks accumulate in pinned staging until a device batch is full

@@ -1530,6 +1530,7 @@ struct tq_join {
   int out_side[2 * MAXC] = {};            // per result-batch column: 0 = plain, 1 = build-side store, 2 = probe-side store
   int out_col[2 * MAXC] = {};
   DevBuf lens_scratch, scan_scratch3;
+  DevBuf var_meta;                        // read-back record of append_cells_device (var-len columns of device chunks)
   // OtherConditions (othercond.cuh): applied to every finished result batch
   bool has_oc = false;
   OcPlan oc;
@@ -2882,8 +2883,10 @@ int32_t tq_join_put_build(tq_join *j, const tq_column *cols, int32_t mem) {
     if (cols[c].length != rows) { set_error("ragged build chunk"); return TQ_ERR_INVALID_ARG; }
     if (!var && cols[c].offsets) { set_error("unsupport column type for encode (var-len data in fixed-width column %d)", c); return TQ_ERR_UNSUPPORTED_TYPE; }
     if (var && !cols[c].offsets) { set_error("var-len column %d needs offsets", c); return TQ_ERR_INVALID_ARG; }
-    if (rows && !cols[c].data && !(var && cols[c].offsets[rows] == cols[c].offsets[0])) return TQ_ERR_INVALID_ARG;
-    if (j->b_ind[c] && mem != TQ_MEM_HOST) { set_error("FLOAT / var-len columns are accepted from host memory only"); return TQ_ERR_UNSUPPORTED_TYPE; }
+    // (the offsets of a device column are not read here: append_cells_device checks them on the device)
+    if (mem == TQ_MEM_HOST && rows && !cols[c].data && !(var && cols[c].offsets[rows] == cols[c].offsets[0])) return TQ_ERR_INVALID_ARG;
+    if (mem != TQ_MEM_HOST && rows && !cols[c].data && !var) return TQ_ERR_INVALID_ARG;
+    if (j->b_ind[c] && !var && mem != TQ_MEM_HOST) { set_error("FLOAT columns are accepted from host memory only"); return TQ_ERR_UNSUPPORTED_TYPE; }
   }
   if (rows == 0) return TQ_OK;
   if (mem == TQ_MEM_HOST) {
@@ -2921,6 +2924,23 @@ int32_t tq_join_put_build(tq_join *j, const tq_column *cols, int32_t mem) {
       }
     }
   } else {
+    // var-len cells are copied into the build store now (the caller may reuse those buffers on return); the 8-byte columns
+    // and every NULL bitmap are borrowed until tq_join_finalize_build
+    Runtime &r = rt();
+    std::lock_guard<std::recursive_mutex> lk(r.mu);
+    int64_t before[MAXC][2];
+    for (int c = 0; c < j->nb_user; c++) {
+      if (!j->b_ind[c]) continue;
+      before[c][0] = j->b_store[c].n;
+      before[c][1] = j->b_store[c].nbytes;
+      int64_t longest = 0;
+      const int32_t st = append_cells_device(j->b_store[c], cols[c].offsets, cols[c].data, rows, &longest, j->var_meta, r.compute);
+      if (st != TQ_OK) {   // a refused chunk leaves the stores as they were
+        for (int d = 0; d < c; d++)
+          if (j->b_ind[d]) { j->b_store[d].n = before[d][0]; j->b_store[d].nbytes = before[d][1]; }
+        return st;
+      }
+    }
     j->b_dev_chunks.emplace_back(cols, cols + j->nb_user);
   }
   j->n_build += rows;
@@ -2934,16 +2954,31 @@ int32_t tq_join_finalize_build(tq_join *j) {
   Runtime &r = rt();
   std::lock_guard<std::recursive_mutex> lk(r.mu);
   j->b_view.assign(j->n_build_cols, DCol());
+  if (j->build_mem == TQ_MEM_DEVICE) {
+    // var-len columns: the cells are in b_store (put_build); the kernels see row ids, exactly as on the host path
+    j->b_cols.resize(j->nb_user);
+    for (int c = 0; c < j->nb_user; c++) {
+      if (!j->b_ind[c]) continue;
+      if (j->b_elem[c] == 4) {   // FLOAT is refused from device memory: the side is empty
+        j->b_store[c].elem = 4;
+        TQ_TRY(j->b_store[c].bytes.reserve(16));
+      } else {
+        int64_t unused = 0;
+        TQ_TRY(append_cells_device(j->b_store[c], nullptr, nullptr, 0, &unused, j->var_meta, r.compute));   // offsets[0] of an empty side
+      }
+      TQ_TRY(j->b_cols[c].data.reserve((size_t)(j->n_build ? j->n_build : 1) * 8));
+      TQ_TRY(iota_u64(j->b_cols[c].data.as<uint64_t>(), j->n_build, r.compute));
+    }
+  }
   if (j->build_mem == TQ_MEM_DEVICE && j->b_dev_chunks.size() == 1) {
     for (int c = 0; c < j->nb_user; c++) {
-      j->b_view[c].data = (const uint64_t *)j->b_dev_chunks[0][c].data;
+      j->b_view[c].data = j->b_ind[c] ? j->b_cols[c].data.as<uint64_t>() : (const uint64_t *)j->b_dev_chunks[0][c].data;
       j->b_view[c].bm = (const uint32_t *)j->b_dev_chunks[0][c].null_bitmap;
     }
   } else if (j->build_mem == TQ_MEM_DEVICE) {
     // several device chunks: concatenate (data D2D; bitmaps need 8-row alignment at chunk boundaries)
-    j->b_cols.resize(j->nb_user);
     for (int c = 0; c < j->nb_user; c++) {
-      TQ_TRY(j->b_cols[c].data.reserve((size_t)j->n_build * 8));
+      if (!j->b_ind[c]) TQ_TRY(j->b_cols[c].data.reserve((size_t)j->n_build * 8));
       TQ_TRY(j->b_cols[c].bm.reserve(bitmap_alloc_bytes(j->n_build)));
       int64_t off = 0;
       bool any_bm = false;
@@ -2951,7 +2986,8 @@ int32_t tq_join_finalize_build(tq_join *j) {
       if (any_bm) TQ_CUDA(cudaMemsetAsync(j->b_cols[c].bm.p, 0xFF, bitmap_alloc_bytes(j->n_build), r.compute));
       for (auto &ch : j->b_dev_chunks) {
         const int64_t rows = ch[c].length;
-        TQ_CUDA(cudaMemcpyAsync(j->b_cols[c].data.as<uint8_t>() + off * 8, ch[c].data, (size_t)rows * 8, cudaMemcpyDeviceToDevice, r.compute));
+        if (!j->b_ind[c])
+          TQ_CUDA(cudaMemcpyAsync(j->b_cols[c].data.as<uint8_t>() + off * 8, ch[c].data, (size_t)rows * 8, cudaMemcpyDeviceToDevice, r.compute));
         if (ch[c].null_bitmap) {
           if (off & 7) { set_error("device build chunks with NULL bitmaps must have row counts that are multiples of 8"); return TQ_ERR_INVALID_ARG; }
           TQ_CUDA(cudaMemcpyAsync(j->b_cols[c].bm.as<uint8_t>() + (off >> 3), ch[c].null_bitmap, bitmap_bytes(rows), cudaMemcpyDeviceToDevice, r.compute));
@@ -3023,8 +3059,10 @@ int32_t tq_join_put_probe(tq_join *j, const tq_column *cols, const uint8_t *sele
     if (cols[c].length != rows) { set_error("ragged probe chunk"); return TQ_ERR_INVALID_ARG; }
     if (!var && cols[c].offsets) { set_error("unsupport column type for encode (var-len data in fixed-width column %d)", c); return TQ_ERR_UNSUPPORTED_TYPE; }
     if (var && !cols[c].offsets) { set_error("var-len column %d needs offsets", c); return TQ_ERR_INVALID_ARG; }
-    if (rows && !cols[c].data && !(var && cols[c].offsets[rows] == cols[c].offsets[0])) return TQ_ERR_INVALID_ARG;
-    if (j->p_ind[c] && mem != TQ_MEM_HOST) { set_error("FLOAT / var-len columns are accepted from host memory only"); return TQ_ERR_UNSUPPORTED_TYPE; }
+    // (the offsets of a device column are not read here: append_cells_device checks them on the device)
+    if (mem == TQ_MEM_HOST && rows && !cols[c].data && !(var && cols[c].offsets[rows] == cols[c].offsets[0])) return TQ_ERR_INVALID_ARG;
+    if (mem != TQ_MEM_HOST && rows && !cols[c].data && !var) return TQ_ERR_INVALID_ARG;
+    if (j->p_ind[c] && !var && mem != TQ_MEM_HOST) { set_error("FLOAT columns are accepted from host memory only"); return TQ_ERR_UNSUPPORTED_TYPE; }
   }
   if (rows == 0) return TQ_OK;
   Runtime &r = rt();
@@ -3037,6 +3075,23 @@ int32_t tq_join_put_probe(tq_join *j, const tq_column *cols, const uint8_t *sele
       view[c].bm = (const uint32_t *)cols[c].null_bitmap;
     }
     const int slot = j->pending.active ? 1 - j->pending.cursor_slot : 0;
+    if (j->any_ind) {
+      // var-len cells are copied into this batch's side store (no batch reads this input set any more: the one in flight
+      // uses the other slot); the join sees row ids 0..rows-1 + the column's NULL bitmap, as for a host piece
+      ProbeInputSet &in = j->in_set[slot];
+      in.store.resize(j->np_user);
+      in.cols.resize(j->n_probe_cols);
+      for (int c = 0; c < j->np_user; c++) {
+        if (!j->p_ind[c]) continue;
+        SideStore &st = in.store[c];
+        st.n = st.nbytes = 0;
+        int64_t longest = 0;
+        TQ_TRY(append_cells_device(st, cols[c].offsets, cols[c].data, rows, &longest, j->var_meta, r.compute));
+        TQ_TRY(in.cols[c].data.reserve((size_t)rows * 8));
+        TQ_TRY(iota_u64(in.cols[c].data.as<uint64_t>(), rows, r.compute));
+        view[c].data = in.cols[c].data.as<uint64_t>();
+      }
+    }
     const uint8_t *d_sel = nullptr;
     if (selected) {  // `selected` is host memory by contract
       ProbeInputSet &in = j->in_set[slot];

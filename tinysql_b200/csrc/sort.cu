@@ -32,6 +32,120 @@
 
 using namespace tq;
 
+// ------------------------------------------------------------------------------------------------ var-len cells from device memory
+// append_cells_device / device_cell_span (varlen.cuh): the one way a var-len column in device memory (TQ_MEM_DEVICE puts of the
+// sort, merge join, hash join and aggregation) enters the library.  The host path stages cells in a HostVarAccum and uploads them
+// once (upload_store); a device column never visits the host: one kernel writes its offsets rebased onto the store (and finds the
+// longest cell, which the sort needs for the number of 8-byte key words of a string ByItem), one D2D copy moves its bytes.  The
+// only host read is one small record per call: the column's first and last offset and the longest cell.  They live here, launched
+// through TQ_LAUNCH, because sort.cu is the source tests/emu compiles (varlen.cu is replaced by stand-ins there).
+namespace tq {
+
+namespace vl_append {   // (named: an anonymous namespace inside tq next to sort.cu's own would confuse nvcc's stubs)
+
+// meta[0] = off[0], meta[1] = off[rows], meta[2] = max over cells of (u64)(off[i + 1] - off[i]) (a decreasing offset shows up
+// as a huge length, which the host check rejects)
+__global__ void __launch_bounds__(256) k_var_append_offsets(const int64_t *__restrict__ off, int64_t rows, int64_t n0, int64_t total0,
+                                                            int64_t *__restrict__ out_off, unsigned long long *meta) {
+  const int64_t o0 = off[0];
+  const int64_t first = (int64_t)blockIdx.x * blockDim.x + threadIdx.x;
+  const int64_t stride = (int64_t)gridDim.x * blockDim.x;
+  if (first == 0) {
+    out_off[n0] = total0;
+    meta[0] = (unsigned long long)o0;
+    meta[1] = (unsigned long long)off[rows];
+  }
+  unsigned long long mx = 0;
+  for (int64_t i = first; i < rows; i += stride) {
+    const int64_t lo = off[i], hi = off[i + 1];
+    out_off[n0 + i + 1] = total0 + (hi - o0);
+    const unsigned long long len = (unsigned long long)(hi - lo);
+    mx = len > mx ? len : mx;
+  }
+#pragma unroll
+  for (int d = 16; d > 0; d >>= 1) {
+    const unsigned long long o = __shfl_xor_sync(0xffffffffu, mx, d);
+    mx = o > mx ? o : mx;
+  }
+  if ((threadIdx.x & 31) == 0 && mx) atomicMax(meta + 2, mx);
+}
+
+int append_grid(int64_t n) {
+  const int64_t blocks = (n + 255) / 256;
+  const int64_t cap = (int64_t)rt().sm_count * 8;
+  return (int)(blocks < cap ? (blocks < 1 ? 1 : blocks) : cap);
+}
+
+// grow b to at least `want` bytes (at least doubling), keeping its first `keep` bytes
+int32_t grow_keep(DevBuf &b, size_t keep, size_t want, cudaStream_t s) {
+  if (want <= b.cap && b.p) return TQ_OK;
+  DevBuf nb;
+  TQ_TRY(nb.reserve(std::max(want, b.cap * 2)));
+  if (keep) TQ_CUDA(cudaMemcpyAsync(nb.p, b.p, keep, cudaMemcpyDeviceToDevice, s));
+  TQ_CUDA(cudaStreamSynchronize(s));   // the old block goes back to the allocator: nothing may still read it
+  b = std::move(nb);
+  return TQ_OK;
+}
+
+}  // namespace vl_append
+
+int32_t append_cells_device(SideStore &st, const int64_t *offsets, const uint8_t *data, int64_t rows, int64_t *max_len, DevBuf &meta,
+                            cudaStream_t s) {
+  *max_len = 0;
+  const int64_t n0 = st.n, total0 = st.nbytes;
+  using namespace vl_append;
+  TQ_TRY(grow_keep(st.offsets, n0 ? (size_t)(n0 + 1) * 8 : 0, (size_t)(n0 + rows + 1) * 8, s));
+  if (rows <= 0) {
+    if (n0 == 0) TQ_CUDA(cudaMemsetAsync(st.offsets.p, 0, 8, s));
+    TQ_TRY(grow_keep(st.bytes, (size_t)total0, (size_t)total0 + 16, s));
+    TQ_CUDA(cudaStreamSynchronize(s));
+    st.elem = 0;
+    st.base = 0;
+    return TQ_OK;
+  }
+  if (!offsets) { set_error("var-len device column without offsets"); return TQ_ERR_INVALID_ARG; }
+  TQ_TRY(meta.reserve(32));
+  TQ_CUDA(cudaMemsetAsync(meta.p, 0, 24, s));
+  TQ_LAUNCH(k_var_append_offsets, append_grid(rows), 256, 0, s, offsets, rows, n0, total0, st.offsets.as<int64_t>(), meta.as<unsigned long long>());
+  count_launch();
+  TQ_TRY(check_launch("k_var_append_offsets"));
+  unsigned long long h[3] = {0, 0, 0};
+  TQ_CUDA(cudaMemcpyAsync(h, meta.p, sizeof(h), cudaMemcpyDeviceToHost, s));
+  TQ_CUDA(cudaStreamSynchronize(s));
+  const int64_t b0 = (int64_t)h[0], b1 = (int64_t)h[1], span = b1 - b0;
+  if (b0 < 0 || span < 0 || h[2] > (unsigned long long)span) {
+    set_error("var-len device column: offsets must be non-negative and non-decreasing (offsets[0] = %lld, offsets[%lld] = %lld)", (long long)b0,
+              (long long)rows, (long long)b1);
+    return TQ_ERR_INVALID_ARG;
+  }
+  if (span > 0 && !data) { set_error("var-len device column with %lld bytes of cells but no data", (long long)span); return TQ_ERR_INVALID_ARG; }
+  TQ_TRY(grow_keep(st.bytes, (size_t)total0, (size_t)(total0 + span) + 16, s));
+  if (span > 0) TQ_CUDA(cudaMemcpyAsync(st.bytes.as<uint8_t>() + total0, data + b0, (size_t)span, cudaMemcpyDeviceToDevice, s));
+  TQ_CUDA(cudaStreamSynchronize(s));   // the caller may reuse its buffers on return
+  st.elem = 0;
+  st.base = 0;
+  st.n = n0 + rows;
+  st.nbytes = total0 + span;
+  *max_len = (int64_t)h[2];
+  return TQ_OK;
+}
+
+int32_t device_cell_span(const int64_t *offsets, int64_t rows, int64_t *first, int64_t *last, cudaStream_t s) {
+  int64_t h[2] = {0, 0};
+  TQ_CUDA(cudaMemcpyAsync(&h[0], offsets, 8, cudaMemcpyDeviceToHost, s));
+  TQ_CUDA(cudaMemcpyAsync(&h[1], offsets + rows, 8, cudaMemcpyDeviceToHost, s));
+  TQ_CUDA(cudaStreamSynchronize(s));
+  if (h[0] < 0 || h[1] < h[0]) {
+    set_error("var-len device column: offsets[0] = %lld, offsets[%lld] = %lld", (long long)h[0], (long long)rows, (long long)h[1]);
+    return TQ_ERR_INVALID_ARG;
+  }
+  *first = h[0];
+  *last = h[1];
+  return TQ_OK;
+}
+
+}  // namespace tq
+
 namespace {
 
 constexpr uint32_t ROW_MISS = 0xFFFFFFFFu;
@@ -375,6 +489,7 @@ struct RowStore {
   bool uploaded = false;
   bool host_mode = false, device_mode = false;   // a handle takes host chunks or device chunks, not both
   int64_t dev_cap = 0;                           // device mode: rows the columns' device arrays can hold
+  DevBuf var_meta;                               // device mode: read-back record of append_cells_device
 
   int32_t init(int n_cols, const int32_t *types) {
     cols.resize((size_t)n_cols);
@@ -431,26 +546,47 @@ struct RowStore {
     }
   }
 
-  // One chunk whose columns live in HBM (TQ_MEM_DEVICE: e.g. rows lent by tq_join_next_device).  8-byte columns only; the data
-  // never leaves the device: it is appended to the column's device array (grown by doubling), only the NOT-NULL bitmap — one
-  // bit per row — is read back so that chunks can be concatenated at any bit offset.  The call returns after the copies, so
-  // the caller may recycle its buffers.
+  // One chunk whose columns live in HBM (TQ_MEM_DEVICE: e.g. rows lent by tq_join_next_device).  8-byte and var-len columns
+  // (FLOAT comes as host chunks); the data never leaves the device: 8-byte slots are appended to the column's device array
+  // (grown by doubling), var-len cells to its device store (append_cells_device), and only the NOT-NULL bitmap — one bit per
+  // row — is read back so that chunks can be concatenated at any bit offset.  The call returns after the copies, so the
+  // caller may recycle its buffers.
   int32_t append_device(const tq_column *in, cudaStream_t s) {
     if (cols.empty()) return TQ_OK;
     if (host_mode) { set_error("one handle takes either host chunks or device chunks"); return TQ_ERR_STATE; }
     const int64_t rows = in[0].length;
     if (rows < 0) return TQ_ERR_INVALID_ARG;
     for (size_t c = 0; c < cols.size(); c++) {
-      if (cols[c].kind != 0 || in[c].offsets) { set_error("device chunks: 8-byte columns only (column %d)", (int)c); return TQ_ERR_UNSUPPORTED_TYPE; }
+      if (cols[c].kind == 1) { set_error("device chunks: FLOAT columns are accepted from host memory only (column %d)", (int)c); return TQ_ERR_UNSUPPORTED_TYPE; }
+      if (cols[c].kind == 0 && in[c].offsets) { set_error("unsupport column type for encode (var-len data in fixed-width column %d)", (int)c); return TQ_ERR_UNSUPPORTED_TYPE; }
+      if (cols[c].kind == 2 && !in[c].offsets) { set_error("var-len column %d needs offsets", (int)c); return TQ_ERR_INVALID_ARG; }
       if (in[c].length != rows) { set_error("ragged input chunk"); return TQ_ERR_INVALID_ARG; }
-      if (rows && !in[c].data) return TQ_ERR_INVALID_ARG;
+      if (rows && cols[c].kind == 0 && !in[c].data) return TQ_ERR_INVALID_ARG;
     }
     device_mode = true;
     if (rows == 0) return TQ_OK;
     if (n + rows > 0xFFFFFFF0ll) { set_error("more than 2^32 rows in one sort / merge-join input"); return TQ_ERR_INVALID_ARG; }
+    // var-len cells first: they are the only part that can still be refused (bad offsets), and a refused chunk leaves the
+    // stores as they were
+    std::vector<std::pair<int64_t, int64_t>> before;
+    for (size_t c = 0; c < cols.size(); c++) {
+      StoreCol &sc = cols[c];
+      if (sc.kind != 2) continue;
+      before.emplace_back(sc.store.n, sc.store.nbytes);
+      int64_t longest = 0;
+      const int32_t st = append_cells_device(sc.store, in[c].offsets, in[c].data, rows, &longest, var_meta, s);
+      if (st != TQ_OK) {
+        size_t k = 0;
+        for (size_t d = 0; d <= c; d++)
+          if (cols[d].kind == 2) { cols[d].store.n = before[k].first; cols[d].store.nbytes = before[k].second; k++; }
+        return st;
+      }
+      sc.max_len = std::max(sc.max_len, longest);
+    }
     if (n + rows > dev_cap) {
       const int64_t new_cap = std::max<int64_t>(std::max<int64_t>(n + rows, dev_cap * 2), 1 << 16);
       for (StoreCol &sc : cols) {
+        if (sc.kind != 0) continue;
         DevBuf bigger;
         TQ_TRY(bigger.reserve((size_t)new_cap * 8 + 16));
         if (n) TQ_CUDA(cudaMemcpyAsync(bigger.p, sc.d_data.p, (size_t)n * 8, cudaMemcpyDeviceToDevice, s));
@@ -462,7 +598,7 @@ struct RowStore {
     std::vector<uint8_t> bits;
     for (size_t c = 0; c < cols.size(); c++) {
       StoreCol &sc = cols[c];
-      TQ_CUDA(cudaMemcpyAsync(sc.d_data.as<uint8_t>() + (size_t)n * 8, in[c].data, (size_t)rows * 8, cudaMemcpyDeviceToDevice, s));
+      if (sc.kind == 0) TQ_CUDA(cudaMemcpyAsync(sc.d_data.as<uint8_t>() + (size_t)n * 8, in[c].data, (size_t)rows * 8, cudaMemcpyDeviceToDevice, s));
       if (in[c].null_bitmap) {
         bits.assign(bitmap_bytes(rows), 0);
         TQ_CUDA(cudaMemcpyAsync(bits.data(), in[c].null_bitmap, bitmap_bytes(rows), cudaMemcpyDeviceToHost, s));
@@ -478,8 +614,13 @@ struct RowStore {
   int32_t upload(cudaStream_t s) {
     if (uploaded) return TQ_OK;
     for (StoreCol &sc : cols) {
-      if (sc.kind == 2) TQ_TRY(upload_store(sc.h_var, sc.store, s));
-      else if (!device_mode) {   // device mode: the data is in d_data already
+      if (sc.kind == 2) {
+        if (!device_mode) TQ_TRY(upload_store(sc.h_var, sc.store, s));
+        else {   // device mode: the cells are in the store already (an input without rows gets its offsets[0])
+          int64_t unused = 0;
+          TQ_TRY(append_cells_device(sc.store, nullptr, nullptr, 0, &unused, var_meta, s));
+        }
+      } else if (!device_mode) {   // device mode: the data is in d_data already
         TQ_TRY(sc.d_data.reserve(sc.h_data.size() + 16));
         if (!sc.h_data.empty()) TQ_CUDA(cudaMemcpyAsync(sc.d_data.p, sc.h_data.data(), sc.h_data.size(), cudaMemcpyHostToDevice, s));
       }

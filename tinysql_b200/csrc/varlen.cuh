@@ -56,4 +56,13 @@ int32_t narrow_f64(const uint64_t *src, int64_t n, uint32_t *dst, cudaStream_t s
 int32_t gather_cells(const SideStore &st, const uint64_t *rowids, const uint32_t *bm, int64_t n, VarOut &out, DevBuf &lens, DevBuf &scan_scratch,
                      cudaStream_t s);
 
+// Defined in sort.cu (the source the emulation build compiles).  Append the `rows` cells of a var-len column in DEVICE memory
+// (offsets[0..rows], offsets[0] may be non-zero; data = the bytes the offsets index) to the device store st (var-len, base 0), growing its arrays by doubling.  *max_len =
+// the longest appended cell.  One small read-back per call; synchronises s, so the caller may reuse its buffers on return.
+// rows == 0 only makes sure an empty store has its offsets[0].  The NOT-NULL bitmap is the caller's business.
+int32_t append_cells_device(SideStore &st, const int64_t *offsets, const uint8_t *data, int64_t rows, int64_t *max_len, DevBuf &meta,
+                            cudaStream_t s);
+// offsets[0] and offsets[rows] of a var-len column in DEVICE memory (one read-back; synchronises s)
+int32_t device_cell_span(const int64_t *offsets, int64_t rows, int64_t *first, int64_t *last, cudaStream_t s);
+
 }  // namespace tq
