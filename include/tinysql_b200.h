@@ -268,7 +268,23 @@ int32_t tq_expr_eval(int64_t n, int32_t n_inputs, const tq_column *inputs, int32
  *   tq_join_destroy                                  (Close; legal at any point)
  *
  * Output schema = left child columns ++ right child columns (executor/builder.go:443);
- * with outer_is_right != 0 the build (inner) side is the left child. */
+ * with outer_is_right != 0 the build (inner) side is the left child.
+ *
+ * Key-less join (n_keys == 0: cross joins, ON conditions without an equality, outer joins whose ON names one side only).
+ * With no key columns the reference puts every build row into one chain in insertion order (hash_table.go:146-169) and every
+ * selected probe row finds it (join.go:325-362, rowHashMap.Get hash_table.go:259-272), so:
+ *  - the candidates of a probe row are all build rows in insertion order; the OtherConditions filter the pairs
+ *    (joiner.go:155-167);
+ *  - an outer join emits a probe row once as its miss row (NULL / defaultInner inner side) when no pair survives, when
+ *    selected[i] == 0, or when the build side is empty; the conditions never run for the last two (joiner.go:225-228,288-291),
+ *    so those rows raise no error and no warning;
+ *  - the output is exactly the reference's row sequence: probe rows in input order, build rows in insertion order inside one.
+ * Same protocol, column layouts, selected[], defaultInner and conditions as the keyed join.  A probe batch is owned by the
+ * handle once put (device chunks are copied) and produces no rows by itself: result batches of at most probe_batch_rows rows
+ * are built only when tq_join_next / _next_bytes / _next_device needs rows (at most one ahead), so memory does not depend
+ * on |probe| x |build|, and tq_join_destroy mid-stream is cheap.  An overflow of a pair in the evaluation set is returned by
+ * the call that would deliver the first row of the probe-row sub-range it belongs to (DESIGN.md §3).
+ * tq_join_put_probe_segments answers a key-less handle with TQ_ERR_UNSUPPORTED_TYPE. */
 enum { TQ_JOIN_INNER = 0, TQ_JOIN_LEFT_OUTER = 1, TQ_JOIN_RIGHT_OUTER = 2 }; /* planner/core/logical_plans.go:52-57 */
 
 typedef struct tq_join_desc {
@@ -278,7 +294,8 @@ typedef struct tq_join_desc {
   const int32_t *build_types; /* TQ_TYPE_* per inner column                                   */
   int32_t n_probe_cols;       /* outer-side schema                                            */
   const int32_t *probe_types;
-  int32_t n_keys;             /* len(innerKeys) == len(outerKeys), 1..8; any supported column type (codec.go:216-236) */
+  int32_t n_keys;             /* len(innerKeys) == len(outerKeys), 0..8; any supported column type (codec.go:216-236).
+                               * 0 = the key-less join below: build_key_idx / probe_key_idx may be NULL */
   const int32_t *build_key_idx; /* innerKeys[i].Index                                         */
   const int32_t *probe_key_idx; /* outerKeys[i].Index                                         */
   int64_t probe_batch_rows;   /* device batch size the ≤1024-row chunks are accumulated into; 0 = default */
@@ -375,7 +392,9 @@ int32_t tq_join_destroy(tq_join *j);
 int32_t tq_join_next_device(tq_join *j, tq_column *out_cols, int64_t *n_rows, int32_t *eof);
 /* Statistics of the handle: [0] build rows inserted, [1] distinct build keys, [2] partitions,
  * [3] probe rows consumed, [4] joined rows produced, [5] last probe kernel time in ns,
- * [6] last build time in ns, [7] probe kernel launches.  */
+ * [6] last build time in ns, [7] probe kernel launches.
+ * Key-less handles: [0] build rows stored, [1] = [2] = 0, [4] rows of the result batches built so far, [5] device time of
+ * the last result batch's kernels.  */
 int32_t tq_join_stats(tq_join *j, int64_t *stats8);
 
 /* ------------------------------------------------------------------ chunk wire codec

@@ -98,6 +98,8 @@ func (e *GPUHashJoinExec) Open(ctx context.Context) error {
 	}
 	d.n_build_cols, d.build_types = C.int32_t(nb), cInt32s(nb, func(i int) C.int32_t { return tqType(innerTypes[i]) })
 	d.n_probe_cols, d.probe_types = C.int32_t(np), cInt32s(np, func(i int) C.int32_t { return tqType(outerTypes[i]) })
+	// nk == 0 (a cross join, or an ON without an equality: everything is in OtherConditions) is a key-less join, which
+	// runs on the device too; cInt32s(0, …) still allocates one slot, and the library does not read it.
 	d.n_keys = C.int32_t(nk)
 	d.build_key_idx = cInt32s(nk, func(i int) C.int32_t { return C.int32_t(e.innerKeys[i].Index) })
 	d.probe_key_idx = cInt32s(nk, func(i int) C.int32_t { return C.int32_t(e.outerKeys[i].Index) })

@@ -18,6 +18,7 @@
 //   (launch_probe_stream): k_scatter_aos -> k_part_bases -> k_probe_pos -> hole filling; the result is a multiset.
 //   Any other large build: k_probe_part_hist (only after a slab overflow) -> scan -> k_probe_scatter(_fast) (shared-memory
 //   counting sort of 4096-row tiles, coalesced full-sector stores) -> k_probe_part_fast / k_probe_part(_uniq).
+#include <chrono>
 #include <cstdlib>
 #include <deque>
 #include <memory>
@@ -29,6 +30,7 @@
 #include "strdict.cuh"
 #include "scatter.cuh"
 #include "othercond.cuh"
+#include "nlj.cuh"
 
 namespace tq {
 
@@ -1493,6 +1495,19 @@ struct PendingBatch {  // a launched probe batch whose row count has not been re
   cudaEvent_t ev_k = nullptr;
 };
 
+// Key-less join (n_keys == 0, nlj.cuh): one probe batch, owned by the handle, and its position in its pair space.  The batch is
+// walked in sub-ranges of whole probe rows; result batches are slices of the current sub-range's output.
+struct KlProbe {
+  ProbeInputSet in;            // the probe rows (+ FLOAT / var-len cells, selected bytes)
+  std::vector<DCol> view;
+  const uint8_t *d_sel = nullptr;
+  int64_t n = 0;
+  int64_t next_row = 0;        // first probe row of the next sub-range
+  int64_t r0 = 0, rows = 0;    // the current sub-range
+  uint64_t sub_total = 0, sub_pos = 0;
+  bool sub_open = false;
+};
+
 }  // namespace tq
 
 using namespace tq;
@@ -1599,6 +1614,12 @@ struct tq_join {
   bool probe_eof = false;
   int64_t probe_rows_total = 0, joined_rows_total = 0, probe_launches = 0, last_probe_ns = 0;
   cudaEvent_t ev_a[2] = {nullptr, nullptr}, ev_b[2] = {nullptr, nullptr};  // per cursor slot
+  // ---- key-less join (n_keys == 0): no table; probe batches become pair cursors, result batches are built on demand
+  bool keyless = false;
+  std::deque<std::unique_ptr<KlProbe>> kl;
+  DevBuf kl_mask, kl_wpre, kl_cnt, kl_off, kl_miss, kl_meta, kl_scan;
+  PinBuf kl_back;
+  bool kl_timed = false;                  // ev_a[0] / ev_b[0] bracket the last result batch's kernels
 
   ~tq_join() {
     if (pending.ev_k) cudaEventDestroy(pending.ev_k);
@@ -1626,17 +1647,18 @@ static bool type_ok(int t) { return t == TQ_TYPE_INT64 || t == TQ_TYPE_UINT64 ||
 static bool type_indirect(int t) { return t == TQ_TYPE_FLOAT32 || t == TQ_TYPE_BYTES; }
 
 // Result row ids -> cells, for every indirect column of a finished result batch.
-static int32_t materialize_indirect(tq_join *j, ResultBatch *rb, int slot) {
+static int32_t materialize_indirect(tq_join *j, ResultBatch *rb, const std::vector<SideStore> &probe_store) {
   const int ncols = j->n_build_cols + j->n_probe_cols;
   rb->var.resize(ncols);
   for (int ic = 0; ic < ncols; ic++) {
     if (!j->out_side[ic]) continue;
-    const SideStore &st = j->out_side[ic] == 1 ? j->b_store[j->out_col[ic]] : j->in_set[slot].store[j->out_col[ic]];
+    const SideStore &st = j->out_side[ic] == 1 ? j->b_store[j->out_col[ic]] : probe_store[j->out_col[ic]];
     TQ_TRY(gather_cells(st, rb->cols[ic].data.as<uint64_t>(), rb->cols[ic].bm.as<uint32_t>(), rb->n, rb->var[ic], j->lens_scratch, j->scan_scratch3,
                         rt().compute));
   }
   return TQ_OK;
 }
+static int32_t materialize_indirect(tq_join *j, ResultBatch *rb, int slot) { return materialize_indirect(j, rb, j->in_set[slot].store); }
 
 static int32_t upload_col(const HostAccum &h, DevColBuf &d, cudaStream_t s) {
   TQ_TRY(d.data.reserve((size_t)(h.n ? h.n : 1) * 8));
@@ -2567,6 +2589,211 @@ static int32_t start_batch(tq_join *j, const std::vector<DCol> &probe, const uin
   return TQ_OK;
 }
 
+// ---- key-less join (n_keys == 0) -------------------------------------------------------------------------------------------
+// A probe batch produces no rows when it arrives: it becomes a pair cursor (KlProbe) that owns its rows, and result batches of
+// at most batch_rows rows are built from it when a tq_join_next* call needs rows.  Memory does not depend on |probe| x |build|:
+// a sub-range's survivor bits are bounded by KL_MASK_WORDS (or one probe row's words), its counts by the batch's rows.
+static constexpr int64_t KL_MASK_WORDS = 1 << 23;   // survivor words of one sub-range: 32 MB, 2^28 pairs
+
+// Takes the probe rows of `in` (its buffers move into the cursor; `in` gets empty ones) as a new pair cursor.
+static void kl_take(tq_join *j, ProbeInputSet &in, const std::vector<DCol> &view, const uint8_t *d_sel, int64_t n) {
+  std::unique_ptr<KlProbe> k(new KlProbe());
+  std::swap(k->in.cols, in.cols);
+  std::swap(k->in.store, in.store);
+  std::swap(k->in.selected, in.selected);
+  k->view = view;
+  k->d_sel = d_sel;
+  k->n = n;
+  j->kl.push_back(std::move(k));
+  j->probe_rows_total += n;
+}
+
+// A device chunk: copied (D2D; var-len cells into the cursor's own store) so the cursor does not depend on the caller's buffers.
+static int32_t kl_put_device(tq_join *j, const tq_column *cols, const uint8_t *selected, int64_t rows) {
+  cudaStream_t s = rt().compute;
+  ProbeInputSet in;
+  in.cols.resize(j->n_probe_cols);
+  if (j->any_ind) in.store.resize(j->np_user);
+  std::vector<DCol> view(j->n_probe_cols);
+  for (int c = 0; c < j->np_user; c++) {
+    DevColBuf &d = in.cols[c];
+    TQ_TRY(d.data.reserve((size_t)rows * 8));
+    if (j->p_ind[c]) {   // (FLOAT columns were refused): row ids into the store
+      int64_t longest = 0;
+      TQ_TRY(append_cells_device(in.store[c], cols[c].offsets, cols[c].data, rows, &longest, j->var_meta, s));
+      TQ_TRY(iota_u64(d.data.as<uint64_t>(), rows, s));
+    } else {
+      TQ_CUDA(cudaMemcpyAsync(d.data.p, cols[c].data, (size_t)rows * 8, cudaMemcpyDeviceToDevice, s));
+    }
+    view[c].data = d.data.as<uint64_t>();
+    if (cols[c].null_bitmap) {
+      TQ_TRY(d.bm.reserve(bitmap_alloc_bytes(rows)));
+      TQ_CUDA(cudaMemcpyAsync(d.bm.p, cols[c].null_bitmap, bitmap_bytes(rows), cudaMemcpyDeviceToDevice, s));
+      view[c].bm = d.bm.as<uint32_t>();
+    }
+  }
+  const uint8_t *d_sel = nullptr;
+  if (selected) {   // host memory by contract
+    TQ_TRY(in.selected.reserve((size_t)rows));
+    TQ_CUDA(cudaMemcpyAsync(in.selected.p, selected, (size_t)rows, cudaMemcpyHostToDevice, s));
+    d_sel = in.selected.as<uint8_t>();
+  }
+  TQ_CUDA(cudaStreamSynchronize(s));   // the caller's columns are not read after the call
+  kl_take(j, in, view, d_sel, rows);
+  return TQ_OK;
+}
+
+// Opens the next sub-range of cursor k: survivor bits (conditions only), per-row counts, their 64-bit scan.  *err = the ops
+// that raised on a pair of the sub-range's evaluation set.
+static int32_t kl_open_subrange(tq_join *j, KlProbe &k, unsigned *err) {
+  cudaStream_t s = rt().compute;
+  const uint32_t B = (uint32_t)j->n_build;
+  const uint32_t W = (j->has_oc && B) ? (B + 31) / 32 : 0;
+  int64_t rows = k.n - k.next_row;
+  if (W) {
+    const int64_t fit = KL_MASK_WORDS / W;
+    if (rows > fit) rows = fit < 1 ? 1 : fit;
+  }
+  k.r0 = k.next_row;
+  k.rows = rows;
+  TQ_TRY(j->kl_cnt.reserve((size_t)rows * 8));
+  TQ_TRY(j->kl_off.reserve((size_t)(rows + 1) * 8));
+  TQ_TRY(j->kl_miss.reserve((size_t)rows));
+  TQ_TRY(j->kl_meta.reserve(16));
+  TQ_TRY(j->kl_back.reserve(32));
+  TQ_CUDA(cudaMemsetAsync(j->kl_meta.p, 0, 16, s));
+  if (W) {
+    TQ_TRY(j->kl_mask.reserve((size_t)rows * W * 4));
+    TQ_TRY(j->kl_wpre.reserve((size_t)rows * W * 4));
+    NljEvalParams e;
+    e.prog = j->oc.prog;
+    const int bbase = j->outer_is_right ? 0 : j->n_probe_cols, pbase = j->outer_is_right ? j->n_build_cols : 0;
+    for (int q = 0; q < e.prog.n_in; q++) {
+      const int ic = j->oc.prog.in_col[q];
+      const bool build = ic >= bbase && ic < bbase + j->n_build_cols;
+      e.in_build[q] = build ? 1 : 0;
+      e.in[q] = build ? j->b_view[ic - bbase] : k.view[ic - pbase];
+    }
+    e.selected = k.d_sel;
+    e.r0 = k.r0;
+    e.rows = rows;
+    e.n_build = B;
+    e.words = W;
+    e.mask = j->kl_mask.as<uint32_t>();
+    e.err = reinterpret_cast<unsigned *>(j->kl_meta.as<uint64_t>() + 1);
+    e.warn = j->kl_meta.as<unsigned long long>();
+    TQ_TRY(nlj_eval(e, s));
+  }
+  NljCountParams c;
+  c.selected = k.d_sel;
+  c.r0 = k.r0;
+  c.rows = rows;
+  c.n_build = B;
+  c.words = W;
+  c.mask = W ? j->kl_mask.as<uint32_t>() : nullptr;
+  c.wpre = W ? j->kl_wpre.as<uint32_t>() : nullptr;
+  c.outer = j->join_type != TQ_JOIN_INNER;
+  c.cnt = j->kl_cnt.as<uint64_t>();
+  c.miss = j->kl_miss.as<uint8_t>();
+  TQ_TRY(nlj_count(c, s));
+  TQ_TRY(nlj_scan_u64(j->kl_cnt.as<uint64_t>(), j->kl_off.as<uint64_t>(), rows, j->kl_scan, s));
+  uint64_t *back = j->kl_back.as<uint64_t>();
+  TQ_CUDA(cudaMemcpyAsync(back, j->kl_off.as<uint64_t>() + rows, 8, cudaMemcpyDeviceToHost, s));
+  TQ_CUDA(cudaMemcpyAsync(back + 1, j->kl_meta.p, 16, cudaMemcpyDeviceToHost, s));
+  TQ_CUDA(cudaStreamSynchronize(s));
+  k.sub_total = back[0];
+  k.sub_pos = 0;
+  k.sub_open = true;
+  j->oc_warnings += (int64_t)back[1];
+  *err = (unsigned)back[2];
+  return TQ_OK;
+}
+
+// Builds the next result batch of the key-less join and queues it; queues nothing when every cursor is drained.  A sub-range
+// whose pairs raised queues a batch that carries only the error: the call that takes it up returns the status, as on the keyed
+// path (DESIGN.md §3).
+static int32_t kl_produce(tq_join *j) {
+  Runtime &r = rt();
+  cudaStream_t s = r.compute;
+  while (!j->kl.empty()) {
+    KlProbe &k = *j->kl.front();
+    if (!k.sub_open) {
+      if (k.next_row >= k.n) {
+        TQ_CUDA(cudaStreamSynchronize(s));   // the last batch's kernels read the cursor's buffers
+        j->kl.pop_front();
+        continue;
+      }
+      unsigned err = 0;
+      TQ_TRY(kl_open_subrange(j, k, &err));
+      if (err) {
+        std::unique_ptr<ResultBatch> rb = get_result_batch(j);
+        rb->oc_err = err;
+        if (!rb->ev_ready) TQ_CUDA(cudaEventCreateWithFlags(&rb->ev_ready, cudaEventDisableTiming));
+        TQ_CUDA(cudaEventRecord(rb->ev_ready, s));
+        j->results.push_back(std::move(rb));
+        j->kl.clear();
+        return TQ_OK;
+      }
+    }
+    if (k.sub_pos == k.sub_total) {
+      k.sub_open = false;
+      k.next_row = k.r0 + k.rows;
+      continue;
+    }
+    const uint64_t left = k.sub_total - k.sub_pos;
+    const int64_t len = left < (uint64_t)j->batch_rows ? (int64_t)left : j->batch_rows;
+    std::unique_ptr<ResultBatch> rb = get_result_batch(j);
+    const int ncols = j->n_build_cols + j->n_probe_cols;
+    const int build_base = j->outer_is_right ? 0 : j->n_probe_cols, probe_base = j->outer_is_right ? j->n_build_cols : 0;
+    rb->cols.resize(ncols);
+    rb->capacity = (uint64_t)len;
+    for (int c = 0; c < ncols; c++) {
+      TQ_TRY(rb->cols[c].data.reserve((size_t)len * 8));
+      TQ_TRY(rb->cols[c].bm.reserve(bitmap_alloc_bytes(len)));
+    }
+    NljOutParams o;
+    o.n_probe_cols = j->n_probe_cols;
+    o.n_build_cols = j->n_build_cols;
+    for (int c = 0; c < j->n_probe_cols; c++) {
+      o.probe[c] = k.view[c];
+      o.out_probe[c].data = rb->cols[probe_base + c].data.as<uint64_t>();
+      o.out_probe[c].bm = rb->cols[probe_base + c].bm.as<uint32_t>();
+    }
+    for (int c = 0; c < j->n_build_cols; c++) {
+      o.build[c] = j->b_view[c];
+      o.out_build[c].data = rb->cols[build_base + c].data.as<uint64_t>();
+      o.out_build[c].bm = rb->cols[build_base + c].bm.as<uint32_t>();
+      o.def_val[c] = j->def_val[c];
+    }
+    o.def_mask = j->def_mask;
+    o.off = j->kl_off.as<uint64_t>();
+    o.miss = j->kl_miss.as<uint8_t>();
+    const bool masked = j->has_oc && j->n_build;
+    o.mask = masked ? j->kl_mask.as<uint32_t>() : nullptr;
+    o.wpre = masked ? j->kl_wpre.as<uint32_t>() : nullptr;
+    o.words = masked ? (uint32_t)((j->n_build + 31) / 32) : 0;
+    o.r0 = k.r0;
+    o.rows = k.rows;
+    o.q0 = k.sub_pos;
+    o.len = len;
+    TQ_CUDA(cudaEventRecord(j->ev_a[0], s));
+    TQ_TRY(nlj_materialize(o, s));
+    TQ_CUDA(cudaEventRecord(j->ev_b[0], s));
+    j->kl_timed = true;
+    j->probe_launches++;
+    rb->n = len;
+    rb->oc_err = 0;
+    if (j->any_ind) TQ_TRY(materialize_indirect(j, rb.get(), k.in.store));   // synchronises the compute stream
+    if (!rb->ev_ready) TQ_CUDA(cudaEventCreateWithFlags(&rb->ev_ready, cudaEventDisableTiming));
+    TQ_CUDA(cudaEventRecord(rb->ev_ready, s));   // the batch is complete: its D2H waits for this, next_device syncs on it
+    k.sub_pos += (uint64_t)len;
+    j->joined_rows_total += len;
+    j->results.push_back(std::move(rb));
+    return TQ_OK;
+  }
+  return TQ_OK;
+}
+
 // Ship one piece of host rows to the device (double-buffered input sets) and start its probe.
 static int32_t process_host_piece(tq_join *j, const tq_column *cols, int64_t row0, int64_t rows, const uint8_t *selected, bool eager_d2h = true) {
   Runtime &r = rt();
@@ -2622,6 +2849,13 @@ static int32_t process_host_piece(tq_join *j, const tq_column *cols, int64_t row
   }
   TQ_CUDA(cudaEventRecord(in.ev_h2d, r.h2d));
   TQ_CUDA(cudaStreamWaitEvent(r.compute, in.ev_h2d, 0));
+  if (j->keyless) {
+    // the rows become a pair cursor, which takes this input set's buffers: the slot is free again at once.  (p_sel_pin[slot]
+    // is refilled by the next piece of this slot, so its upload has to be complete.)
+    TQ_CUDA(cudaStreamSynchronize(r.h2d));
+    kl_take(j, in, view, d_sel, rows);
+    return TQ_OK;
+  }
   return start_batch(j, view, d_sel, rows, /*want_host=*/eager_d2h, slot);
 }
 
@@ -2670,7 +2904,7 @@ int32_t tq_join_create(const tq_join_desc *d, tq_join **out) {
     set_error("join sides must have 1..%d columns", MAXC);
     return TQ_ERR_INVALID_ARG;
   }
-  if (d->n_keys < 1 || d->n_keys > MK_MAX_KEYS) { set_error("hash join on %d key columns: 1..%d are supported", d->n_keys, MK_MAX_KEYS); return TQ_ERR_INVALID_ARG; }
+  if (d->n_keys < 0 || d->n_keys > MK_MAX_KEYS) { set_error("hash join on %d key columns: 0..%d are supported", d->n_keys, MK_MAX_KEYS); return TQ_ERR_INVALID_ARG; }
   for (int i = 0; i < d->n_keys; i++)
     if (d->build_key_idx[i] < 0 || d->build_key_idx[i] >= d->n_build_cols || d->probe_key_idx[i] < 0 || d->probe_key_idx[i] >= d->n_probe_cols) return TQ_ERR_INVALID_ARG;
   // a hidden key column per side: several key columns, or a FLOAT / var-len key (compared as float64 / byte string)
@@ -2712,7 +2946,12 @@ int32_t tq_join_create(const tq_join_desc *d, tq_join **out) {
   };
   auto kind_of = [](int t) { return t == TQ_TYPE_FLOAT32 ? 1 : (t == TQ_TYPE_BYTES ? 2 : 0); };
   j->key_hidden = hidden != 0;
-  if (!hidden) {
+  if (d->n_keys == 0) {
+    // key-less join (nlj.cuh): every build row is a candidate of every selected probe row; no key columns, no table
+    j->keyless = true;
+    j->build_key = j->probe_key = 0;
+    j->key_mode = KEYMODE_RAW;
+  } else if (!hidden) {
     j->build_key = d->build_key_idx[0];
     j->probe_key = d->probe_key_idx[0];
     j->key_mode = mode_of(j->build_types[j->build_key], j->probe_types[j->probe_key]);
@@ -2806,9 +3045,9 @@ static int32_t join_oc_settable(const tq_join *j) {
 // gets the hidden probe row-id column (last on the probe side), which moves the result-batch layout.
 static int32_t join_set_oc(tq_join *j, const JoinProg &prog, bool cmp_list) {
   const bool outer = j->join_type != TQ_JOIN_INNER;
-  if (outer && j->n_probe_cols + 1 > MAXC) { set_error("OtherConditions on an outer join need one spare probe column"); return TQ_ERR_INVALID_ARG; }
+  if (outer && !j->keyless && j->n_probe_cols + 1 > MAXC) { set_error("OtherConditions on an outer join need one spare probe column"); return TQ_ERR_INVALID_ARG; }
   const int n_user = j->nb_user + j->np_user;
-  if (outer) {
+  if (outer && !j->keyless) {   // (the key-less path knows each pair's probe row without a column)
     j->p_hidden_rowid = j->n_probe_cols;
     j->probe_types[j->n_probe_cols] = TQ_TYPE_INT64;
     j->n_probe_cols++;
@@ -3037,7 +3276,32 @@ int32_t tq_join_finalize_build(tq_join *j) {
     j->b_view[j->nb_user].data = j->mk_build_key.as<uint64_t>();
     j->b_view[j->nb_user].bm = any_bm ? j->mk_build_bm.as<uint32_t>() : nullptr;
   }
-  TQ_TRY(join_build(j));
+  if (j->keyless) {
+    // no table: the build rows stay as device columns in insertion order.  A single device chunk is still the caller's
+    // memory, which is only lent until this call returns, so it is copied.
+    const auto t0 = std::chrono::steady_clock::now();
+    if (j->n_build > 0xFFFFFFFFll) { set_error("key-less join: the build side holds 2^32 rows or more"); return TQ_ERR_INVALID_ARG; }
+    if (j->build_mem == TQ_MEM_DEVICE && j->b_dev_chunks.size() == 1) {
+      for (int c = 0; c < j->nb_user; c++) {
+        const tq_column &ch = j->b_dev_chunks[0][c];
+        if (!j->b_ind[c]) {
+          TQ_TRY(j->b_cols[c].data.reserve((size_t)j->n_build * 8));
+          TQ_CUDA(cudaMemcpyAsync(j->b_cols[c].data.p, ch.data, (size_t)j->n_build * 8, cudaMemcpyDeviceToDevice, r.compute));
+          j->b_view[c].data = j->b_cols[c].data.as<uint64_t>();
+        }
+        if (ch.null_bitmap) {
+          TQ_TRY(j->b_cols[c].bm.reserve(bitmap_alloc_bytes(j->n_build)));
+          TQ_CUDA(cudaMemcpyAsync(j->b_cols[c].bm.p, ch.null_bitmap, bitmap_bytes(j->n_build), cudaMemcpyDeviceToDevice, r.compute));
+          j->b_view[c].bm = j->b_cols[c].bm.as<uint32_t>();
+        }
+      }
+    }
+    TQ_CUDA(cudaStreamSynchronize(r.compute));   // the staging buffers are released below
+    j->n_valid = j->n_build;
+    j->build_ns = (int64_t)std::chrono::duration_cast<std::chrono::nanoseconds>(std::chrono::steady_clock::now() - t0).count();
+  } else {
+    TQ_TRY(join_build(j));
+  }
   j->mk_build_key.release();
   j->mk_build_bm.release();
   for (int i = 0; i < j->n_keys; i++) { j->kx_b_data[i].release(); j->kx_b_bm[i].release(); }
@@ -3069,6 +3333,7 @@ int32_t tq_join_put_probe(tq_join *j, const tq_column *cols, const uint8_t *sele
   std::lock_guard<std::recursive_mutex> lk(r.mu);
   if (mem == TQ_MEM_DEVICE) {
     TQ_TRY(flush_probe_staging(j));
+    if (j->keyless) return kl_put_device(j, cols, selected, rows);
     std::vector<DCol> view(j->n_probe_cols);
     for (int c = 0; c < j->np_user; c++) {
       view[c].data = (const uint64_t *)cols[c].data;
@@ -3135,7 +3400,7 @@ int32_t tq_join_put_probe_segments(tq_join *j, int32_t n_segs, const tq_column *
   if (j->probe_eof) { set_error("put_probe after probe_eof"); return TQ_ERR_STATE; }
   // segmented input can only run the streaming path (k_scatter_aos alone reads the regions), and it has no pass that would
   // encode a hidden key column or FLOAT / var-len columns
-  if (!stream_probe_ok(j) || j->key_hidden || j->any_ind) {
+  if (j->keyless || !stream_probe_ok(j) || j->key_hidden || j->any_ind) {
     set_error("segmented probe batches need the streaming PK-FK path (inner join, unique NOT NULL build side >= 2^18 rows, <= 4 columns per side)");
     return TQ_ERR_UNSUPPORTED_TYPE;
   }
@@ -3184,6 +3449,7 @@ static int32_t join_current_batch(tq_join *j, int64_t max_rows, int *have, int32
     if (j->host_cur) { recycle(j, std::move(j->host_cur)); j->host_cur_pos = 0; }
     // The batch in flight is only waited for at end of input: until then "no rows yet" means "feed more", so the
     // D2H of batch i overlaps the H2D + kernels of batch i+1.
+    if (j->results.empty() && j->keyless) TQ_TRY(kl_produce(j));
     if (j->results.empty() && j->probe_eof) TQ_TRY(finalize_pending(j));
     if (j->results.empty()) {
       *eof = j->probe_eof ? 1 : 0;
@@ -3193,6 +3459,11 @@ static int32_t join_current_batch(tq_join *j, int64_t max_rows, int *have, int32
     j->results.pop_front();
     j->host_cur_pos = 0;
     if (j->host_cur->oc_err) return xp_err_to_status(j->host_cur->oc_err, j->oc.prog.ops, "other conditions");
+    if (j->keyless && !j->host_cur->on_host) {
+      // copies of this batch wait for its kernels only; then the next batch is built while this one is copied and sliced
+      TQ_CUDA(cudaStreamWaitEvent(r.d2h, j->host_cur->ev_ready, 0));
+      if (j->results.empty()) TQ_TRY(kl_produce(j));
+    }
     if (!j->host_cur->on_host) {
       // Large consumer buffers: copy straight from HBM into the caller's columns (no staging, no CPU memcpy).
       // (a queued batch is complete: finalize_pending waited for its kernels — no stream-wide sync here, so the copy
@@ -3305,6 +3576,7 @@ int32_t tq_join_next_device(tq_join *j, tq_column *out_cols, int64_t *n_rows, in
   Runtime &r = rt();
   std::lock_guard<std::recursive_mutex> lk(r.mu);
   recycle(j, std::move(j->lent));
+  if (j->results.empty() && j->keyless) TQ_TRY(kl_produce(j));
   if (j->results.empty()) TQ_TRY(finalize_pending(j));
   if (j->results.empty()) {
     *eof = j->probe_eof ? 1 : 0;
@@ -3313,6 +3585,10 @@ int32_t tq_join_next_device(tq_join *j, tq_column *out_cols, int64_t *n_rows, in
   j->lent = std::move(j->results.front());
   j->results.pop_front();
   if (j->lent->oc_err) return xp_err_to_status(j->lent->oc_err, j->oc.prog.ops, "other conditions");
+  if (j->keyless) {   // build the next batch while the caller works on this one, which is complete when the call returns
+    if (j->results.empty()) TQ_TRY(kl_produce(j));
+    TQ_CUDA(cudaEventSynchronize(j->lent->ev_ready));
+  }
   const int ncols = j->nb_user + j->np_user;
   for (int c = 0; c < ncols; c++) {
     out_cols[c].length = j->lent->n;
@@ -3331,9 +3607,15 @@ int32_t tq_join_next_device(tq_join *j, tq_column *out_cols, int64_t *n_rows, in
 
 int32_t tq_join_stats(tq_join *j, int64_t *s) {
   if (!j || !s) return TQ_ERR_INVALID_ARG;
+  if (j->keyless && j->kl_timed) {   // [5]: the last result batch's kernels
+    float ms = 0;
+    if (cudaEventSynchronize(j->ev_b[0]) == cudaSuccess && cudaEventElapsedTime(&ms, j->ev_a[0], j->ev_b[0]) == cudaSuccess)
+      j->last_probe_ns = (int64_t)(ms * 1e6);
+    else cudaGetLastError();
+  }
   s[0] = j->n_valid;
   s[1] = j->n_distinct;
-  s[2] = 1ll << j->pbits;
+  s[2] = j->keyless ? 0 : 1ll << j->pbits;
   s[3] = j->probe_rows_total;
   s[4] = j->joined_rows_total;
   s[5] = j->last_probe_ns;
