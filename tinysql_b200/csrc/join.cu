@@ -15,7 +15,8 @@
 // Probe.  Small build (one table): k_probe, ordered output (probe row asc, build insertion asc) via
 //   ticketed tiles + decoupled look-back.
 //   Large build, PK-FK shape (stream_probe_ok, no probe NULL bitmap): the streaming positional path of join_stream.cuh
-//   (launch_probe_stream): k_scatter_aos -> k_part_bases -> k_probe_pos -> hole filling; the result is a multiset.
+//   (launch_probe_stream): k_pos_count -> k_pos_bases -> k_scatter_cols (the probe columns straight into their result slots)
+//   -> k_probe_pos (key column in, build columns out) -> hole filling; the result is a multiset.
 //   Any other large build: k_probe_part_hist (only after a slab overflow) -> scan -> k_probe_scatter(_fast) (shared-memory
 //   counting sort of 4096-row tiles, coalesced full-sector stores) -> k_probe_part_fast / k_probe_part(_uniq).
 #include <chrono>
@@ -1490,7 +1491,6 @@ struct PendingBatch {  // a launched probe batch whose row count has not been re
   const uint8_t *d_selected = nullptr;
   int64_t n = 0;
   bool want_host = false;
-  SegSpec seg;                  // the regions of a segmented batch (re-read by the re-run after a slab overflow)
   int cursor_slot = 0;
   cudaEvent_t ev_k = nullptr;
 };
@@ -1596,13 +1596,12 @@ struct tq_join {
   DevBuf tile_state[2];                   // per cursor slot: look-back words + ticket
   std::vector<DevColBuf> part_cols[2];    // per cursor slot: probe columns in partition order
   DevBuf part_cnt[2], part_off[2], part_cursor[2], part_lim[2];
-  bool optimistic_scatter = true;         // skip the probe-side histogram pass: fixed slabs with 25% slack (falls back on overflow)
-  // streaming PK-FK pipeline (join_stream.cuh): AoS slabs, positional output, hole filling
-  DevBuf part_aos[2], pos_base[2], pos_valid[2], hole_pos[2], hole_src[2], hole_scan;
+  bool optimistic_scatter = true;         // general partitioned path: skip the histogram pass, fixed slabs with 25% slack (falls back on overflow)
+  // streaming PK-FK pipeline (join_stream.cuh): exact partition counts, positional output, hole filling
+  DevBuf pos_meta[2], pos_valid[2], hole_pos[2], hole_src[2], hole_scan;
   DevBuf b_aos;                           // build-side AoS slabs (released after the build)
   // segmented probe batch (tq_join_put_probe_segments): consumed by the next launch_probe_stream
   SegSpec seg;
-  DevBuf seg_gather[4];                   // a segmented batch whose slab overflowed, gathered into one range per column
   DevBuf scan_scratch2;
   PinBuf cursors_host;
   PendingBatch pending;
@@ -1702,8 +1701,8 @@ static bool stream_build_ok(const tq_join *j) {
 
 // Whether probe batches may take the streaming positional path (launch_probe_stream) as far as the operator and its table
 // decide: a partitioned ROW-mode table with unique NOT NULL build rows, an inner join without OtherConditions, and at most 4
-// columns per side.  The callers add what depends on the batch: launch_probe requires optimistic slabs (no slab has
-// overflowed yet) for ordinary batches; a segmented batch always starts on this path (only k_scatter_aos reads regions).
+// columns per side.  launch_probe adds what depends on the batch: no probe NULL bitmap.  Segmented batches only ever take
+// this path (only its scatter reads regions).
 static bool stream_probe_ok(const tq_join *j) {
   return j->pbits > 0 && j->pbits <= SA_MAX_PBITS && j->row_mode && j->join_type == TQ_JOIN_INNER && !j->build_has_nulls &&
          j->n_probe_cols <= 4 && j->n_build_cols <= 4 && !j->has_oc && !g_no_fast_kernel;
@@ -2026,19 +2025,17 @@ static std::unique_ptr<ResultBatch> get_result_batch(tq_join *j) {
 
 // Hole filling, fast path: when every probe row of the batch found its match (the foreign-key join) the only holes of the
 // positional result are the pads that round each partition up to 32 slots, and both lists — the pad slots below M and the real
-// rows at or above M — follow from the partition bases alone: one small kernel instead of passes over the validity bitmap.
-// A batch with misses (M != rows in the slabs) is completed by fill_holes_host once the counts are on the host.
+// rows at or above M — follow from the partition counts and bases alone: one small kernel instead of passes over the validity
+// bitmap.  A batch with misses (M != rows scattered) is completed by fill_holes_host once the counts are on the host.
 static constexpr int HOLE_PAD_THREADS = 512;   // >= partitions of the streaming path (SA_MAX_PBITS)
-__global__ void __launch_bounds__(HOLE_PAD_THREADS) k_hole_pads(const uint32_t *lo, const uint32_t *hi, const uint32_t *lim, const uint32_t *out_base, int n_parts,
-                                                                 unsigned long long *cur, uint32_t *hole_pos, uint32_t *tail_src) {
+__global__ void __launch_bounds__(HOLE_PAD_THREADS) k_hole_pads(const uint32_t *part_cnt, const uint32_t *out_base, int n_parts, unsigned long long *cur,
+                                                                 uint32_t *hole_pos, uint32_t *tail_src) {
   __shared__ uint32_t s_warp[33];
   const int q = threadIdx.x;
   const uint64_t M = cur[0];
   uint32_t cnt = 0, base = 0, h = 0, t = 0;
   if (q < n_parts) {
-    uint32_t e = hi[q];
-    if (lim && e > lim[q]) e = lim[q];
-    cnt = e - lo[q];
+    cnt = part_cnt[q];
     base = out_base[q];
     const uint64_t pad_lo = (uint64_t)base + cnt, pad_hi = out_base[q + 1];        // pad slots of this partition
     const uint64_t hole_hi = pad_hi < M ? pad_hi : M;
@@ -2086,24 +2083,35 @@ __global__ void __launch_bounds__(256) k_hole_move_pads(const HoleMoveDevParams 
   }
 }
 
-// scatter (AoS, TMA-fed) -> partition bases -> positional probe -> device-driven hole filling
+// exact partition counts -> bases -> column-wise scatter into the result -> key-only positional probe -> device-driven hole
+// filling.  Nothing is read back to the host.
 static int32_t launch_probe_stream(tq_join *j, const ProbeParams &p, const std::vector<DCol> &probe, const uint8_t *d_selected, int64_t n,
                                    unsigned long long *cur, int slot, uint64_t alloc_rows) {
   cudaStream_t s = rt().compute;
   const int P = 1 << j->pbits, NP = j->n_probe_cols, NB = j->n_build_cols;
-  DevBuf &off = j->part_off[slot], &cur_b = j->part_cursor[slot], &lim = j->part_lim[slot];
-  TQ_TRY(j->pos_base[slot].reserve((size_t)(P + 2) * 4));
+  if (n + 32ll * P > 0xFFFFFFF0ll) { set_error("probe batch too large for 32-bit result slots; feed smaller batches"); return TQ_ERR_INVALID_ARG; }
+  TQ_TRY(j->pos_meta[slot].reserve((size_t)4 * (P + 1) * 4));
+  PosMeta m;
+  m.cnt = j->pos_meta[slot].as<uint32_t>();
+  m.base = m.cnt + (P + 1);
+  m.cursor = m.base + (P + 1);
+  m.chunk = m.cursor + (P + 1);
   const int64_t n_words_max = (int64_t)(alloc_rows >> 5) + 1;
   TQ_TRY(j->pos_valid[slot].reserve((size_t)(n_words_max + 2) * 4));
   TQ_TRY(j->hole_pos[slot].reserve((size_t)(32 * (P + 2)) * 4));   // at most 31 pad slots per partition
   TQ_TRY(j->hole_src[slot].reserve((size_t)(32 * (P + 2)) * 4));
+  const ProbePosVariant pv = probe_pos_kernel(NB);
+  if (!pv.k || NP < 1 || NP > 4) { set_error("internal: positional probe of %d x %d columns", NP, NB); return TQ_ERR_INVALID_ARG; }
   ScatterAosParams q{};
   q.sp.n_cols = NP;
-  for (int c = 0; c < NP; c++) q.sp.in[c] = probe[c];
+  for (int c = 0; c < NP; c++) {
+    q.sp.in[c] = probe[c];
+    q.sp.out[c].data = p.out_probe[c].data;   // the result's probe columns
+  }
+  int64_t seg_rows = 0;
   if (j->seg.n) {  // regions filled by the peers' push kernels; row counts live on the device
-    const int T = scatter_aos_tile(NP, P + 2);
+    seg_rows = (j->seg.cap + POS_SEG_ROWS_ALIGN - 1) / POS_SEG_ROWS_ALIGN * POS_SEG_ROWS_ALIGN;
     q.n_segs = j->seg.n;
-    q.seg_tiles = (int)((j->seg.cap + T - 1) / T);
     for (int g = 0; g < j->seg.n; g++) {
       q.seg_cnt[g] = j->seg.cnt[g];
       for (int c = 0; c < NP; c++) q.seg_in[g][c] = j->seg.col[g][c];
@@ -2114,35 +2122,26 @@ static int32_t launch_probe_stream(tq_join *j, const ProbeParams &p, const std::
   q.sp.key_mode = j->key_mode;
   q.sp.pbits = j->pbits;
   q.sp.n = n;
-  q.sp.overflow = cur + 2;
-  TQ_TRY(scatter_aos(q, j->part_aos[slot], off, cur_b, lim, s));
-  k_part_bases<<<1, PART_BASES_THREADS, 0, s>>>(off.as<uint32_t>(), cur_b.as<uint32_t>(), lim.as<uint32_t>(), P, j->pos_base[slot].as<uint32_t>(), cur + 3);
-  count_launch();
+  TQ_TRY(launch_pos_scatter(q, seg_rows, m, pv.tile, cur + 3, s));
   ProbePosParams pp{};
-  pp.slab = j->part_aos[slot].as<uint64_t>();
-  pp.lo = off.as<uint32_t>();
-  pp.hi = cur_b.as<uint32_t>();
-  pp.lim = lim.as<uint32_t>();
-  pp.out_base = j->pos_base[slot].as<uint32_t>();
-  for (int c = 0; c < NP; c++) pp.out_probe[c] = p.out_probe[c].data;
+  pp.keys = p.out_probe[j->probe_key].data;
+  pp.cnt = m.cnt;
+  pp.base = m.base;
+  pp.chunk = m.chunk;
+  pp.n_parts = P;
   for (int c = 0; c < NB; c++) { pp.out_build[c] = p.out_build[c].data; pp.build_word[c] = p.build_word[c]; }
   pp.valid = j->pos_valid[slot].as<uint32_t>();
   pp.cursor = cur;
-  pp.key_col = j->probe_key;
   { const char *e = getenv("TQ_JOIN_PP_DEBUG"); const int f = e ? atoi(e) : 0; pp.dbg_no_tma = f & 1; pp.dbg_late_release = (f >> 1) & 1; }
-  const ProbePosVariant pv = probe_pos_kernel(NP, NB);
-  const int64_t rows_per_cta = g_tiles_per_cta * 1024;   // ~8K rows per CTA: enough CTAs per partition that only a handful of partitions are live at once
-  int64_t split = (n / P) / rows_per_cta;
-  if (split < 1) split = 1;
-  pp.split = (int)split;
-  const int smem = PP_STAGES * pv.tile * NP * 8;
+  // CTAs: at most one per PP_CHUNK_TILES tiles of rows plus one per partition (its last, partial chunk); the unused ones exit
+  const int64_t grid = n / ((int64_t)pv.tile * PP_CHUNK_TILES) + P + 1;
+  const int smem = PP_STAGES * pv.tile * 8;
   TQ_CUDA(cudaFuncSetAttribute(pv.k, cudaFuncAttributeMaxDynamicSharedMemorySize, smem));
-  pv.k<<<(unsigned)(P * split), pv.threads, smem, s>>>(pp, j->table);
+  pv.k<<<(unsigned)grid, pv.threads, smem, s>>>(pp, j->table);
   count_launch();
   TQ_TRY(check_launch("k_probe_pos"));
   // holes: the padding of every partition to 32 slots (filled here) + probe rows without a match (finalize_pending)
-  k_hole_pads<<<1, HOLE_PAD_THREADS, 0, s>>>(off.as<uint32_t>(), cur_b.as<uint32_t>(), lim.as<uint32_t>(), j->pos_base[slot].as<uint32_t>(), P, cur,
-                                            j->hole_pos[slot].as<uint32_t>(), j->hole_src[slot].as<uint32_t>());
+  k_hole_pads<<<1, HOLE_PAD_THREADS, 0, s>>>(m.cnt, m.base, P, cur, j->hole_pos[slot].as<uint32_t>(), j->hole_src[slot].as<uint32_t>());
   HoleMoveDevParams hm{};
   hm.n_cols = NP + NB;
   for (int c = 0; c < NP; c++) hm.col[c] = p.out_probe[c].data;
@@ -2152,9 +2151,8 @@ static int32_t launch_probe_stream(tq_join *j, const ProbeParams &p, const std::
   hm.cur = cur;
   k_hole_move_pads<<<32, 256, 0, s>>>(hm);
   count_launch(2);
-  j->probe_launches += 3;
   TQ_TRY(check_launch("k_hole_move_pads"));
-  j->probe_launches += 3;
+  j->probe_launches += 6;
   return TQ_OK;
 }
 
@@ -2215,7 +2213,7 @@ static int32_t launch_probe(tq_join *j, const std::vector<DCol> &probe, const ui
   p.def_mask = j->def_mask;
   p.n = n;
   p.capacity = capacity;
-  unsigned long long *cur = j->cursors.as<unsigned long long>() + 8 * cursor_slot;  // [0] rows, [1] matched probe rows, [2] slab overflow, [3] span of the positional result, [5] pad holes, [6] rows the scatter placed
+  unsigned long long *cur = j->cursors.as<unsigned long long>() + 8 * cursor_slot;  // [0] rows, [1] matched probe rows, [2] slab overflow (general path), [3] span of the positional result, [5] pad holes, [6] rows the scatter placed
   p.cursor = cur;
   TQ_CUDA(cudaMemsetAsync(cur, 0, 64, s));
   {
@@ -2230,7 +2228,7 @@ static int32_t launch_probe(tq_join *j, const std::vector<DCol> &probe, const ui
   // result is positional: room for the padding of every partition to 32 rows.
   bool any_in_bm = false;
   for (int c = 0; c < j->n_probe_cols; c++) any_in_bm |= (probe[c].bm != nullptr);
-  const bool pos_path = stream_probe_ok(j) && !any_in_bm && (j->optimistic_scatter || j->seg.n);
+  const bool pos_path = stream_probe_ok(j) && !any_in_bm;
   const uint64_t alloc_rows = capacity + (pos_path ? 32ull * ((1ull << j->pbits) + 2) : 0);
   for (int c = 0; c < ncols; c++) {
     TQ_TRY(rb->cols[c].data.reserve((size_t)(alloc_rows ? alloc_rows : 1) * 8));
@@ -2451,37 +2449,6 @@ static int32_t apply_other_conditions(tq_join *j, ResultBatch *rb, int64_t n_pro
   return TQ_OK;
 }
 
-// A segmented batch whose optimistic slab overflowed: the exact histogram path reads one contiguous range, so the regions'
-// rows are copied into one buffer per column.  The batch's kernels are complete, so the counts are read on the host here
-// (a region whose count exceeds its capacity reads as empty, as in k_scatter_aos).  pb then describes the gathered batch.
-static int32_t gather_segments(tq_join *j, PendingBatch &pb) {
-  cudaStream_t s = rt().compute;
-  const SegSpec &g = pb.seg;
-  const int T = scatter_aos_tile(j->n_probe_cols, (1 << j->pbits) + 2);
-  const uint64_t seg_rows = (uint64_t)((g.cap + T - 1) / T * T);
-  unsigned long long cnt[SA_MAX_SEGS];
-  for (int r = 0; r < g.n; r++) TQ_CUDA(cudaMemcpyAsync(&cnt[r], g.cnt[r], 8, cudaMemcpyDeviceToHost, s));
-  TQ_CUDA(cudaStreamSynchronize(s));
-  uint64_t total = 0;
-  for (int r = 0; r < g.n; r++) {
-    if (cnt[r] > seg_rows) cnt[r] = 0;
-    total += cnt[r];
-  }
-  for (int c = 0; c < j->n_probe_cols; c++) {
-    TQ_TRY(j->seg_gather[c].reserve((size_t)(total ? total : 1) * 8));
-    uint64_t at = 0;
-    for (int r = 0; r < g.n; r++) {
-      if (cnt[r]) TQ_CUDA(cudaMemcpyAsync(j->seg_gather[c].as<uint64_t>() + at, g.col[r][c], (size_t)cnt[r] * 8, cudaMemcpyDeviceToDevice, s));
-      at += cnt[r];
-    }
-    pb.probe[c].data = j->seg_gather[c].as<uint64_t>();
-    pb.probe[c].bm = nullptr;
-  }
-  pb.n = (int64_t)total;
-  pb.seg.n = 0;
-  return TQ_OK;
-}
-
 // Wait for the pending batch, re-run it if the output did not fit, queue its result.
 static int32_t finalize_pending(tq_join *j) {
   PendingBatch &pb = j->pending;
@@ -2494,10 +2461,9 @@ static int32_t finalize_pending(tq_join *j) {
   if (cudaEventElapsedTime(&ms, j->ev_a[pb.cursor_slot], j->ev_b[pb.cursor_slot]) == cudaSuccess) j->last_probe_ns = (int64_t)(ms * 1e6);
   else cudaGetLastError();
   if (hc[2]) {
-    // a partition slab of the optimistic (histogram-free) scatter was too small — skewed keys: exact offsets from now on
-    // (for ordinary batches; a segmented batch always tries the slabs first, and is gathered for its re-run)
+    // a partition slab of the general path's optimistic (histogram-free) scatter was too small — skewed keys: exact offsets
+    // from now on (the positional path counts exactly and never overflows)
     j->optimistic_scatter = false;
-    if (pb.seg.n) TQ_TRY(gather_segments(j, pb));
     TQ_TRY(launch_probe(j, pb.probe, pb.d_selected, pb.n, pb.rb.get(), pb.rb->capacity, pb.cursor_slot));
     TQ_CUDA(cudaStreamSynchronize(r.compute));
     produced = hc[0];
@@ -2568,7 +2534,6 @@ static int32_t start_batch(tq_join *j, const std::vector<DCol> &probe, const uin
   const uint64_t capacity = (uint64_t)n;
   std::unique_ptr<ResultBatch> rb = get_result_batch(j);
   TQ_TRY(launch_probe(j, *pin, d_selected, n, rb.get(), capacity, slot));
-  const SegSpec seg = j->seg;
   j->seg.n = 0;  // consumed by this launch: a re-run of the previous batch in finalize_pending must not read these regions
   cudaEvent_t ev = nullptr;
   TQ_CUDA(cudaEventCreateWithFlags(&ev, cudaEventDisableTiming));
@@ -2583,7 +2548,6 @@ static int32_t start_batch(tq_join *j, const std::vector<DCol> &probe, const uin
   pb.d_selected = d_selected;
   pb.n = n;
   pb.want_host = want_host;
-  pb.seg = seg;
   pb.cursor_slot = slot;
   j->probe_rows_total += n;
   return TQ_OK;
@@ -3398,7 +3362,7 @@ int32_t tq_join_put_probe_segments(tq_join *j, int32_t n_segs, const tq_column *
   TQ_TRY(ensure_init());
   if (j->state != tq_join::PROBING) { set_error("put_probe before finalize_build"); return TQ_ERR_STATE; }
   if (j->probe_eof) { set_error("put_probe after probe_eof"); return TQ_ERR_STATE; }
-  // segmented input can only run the streaming path (k_scatter_aos alone reads the regions), and it has no pass that would
+  // segmented input can only run the streaming path (its scatter alone reads the regions), and it has no pass that would
   // encode a hidden key column or FLOAT / var-len columns
   if (j->keyless || !stream_probe_ok(j) || j->key_hidden || j->any_ind) {
     set_error("segmented probe batches need the streaming PK-FK path (inner join, unique NOT NULL build side >= 2^18 rows, <= 4 columns per side)");
@@ -3407,8 +3371,7 @@ int32_t tq_join_put_probe_segments(tq_join *j, int32_t n_segs, const tq_column *
   Runtime &r = rt();
   std::lock_guard<std::recursive_mutex> lk(r.mu);
   TQ_TRY(flush_probe_staging(j));
-  const int T = scatter_aos_tile(j->n_probe_cols, (1 << j->pbits) + 2);
-  const int64_t seg_rows = (seg_cap + T - 1) / T * T;
+  const int64_t seg_rows = (seg_cap + POS_SEG_ROWS_ALIGN - 1) / POS_SEG_ROWS_ALIGN * POS_SEG_ROWS_ALIGN;
   std::vector<DCol> view(j->n_probe_cols);
   j->seg.n = n_segs;
   j->seg.cap = seg_cap;

@@ -1,19 +1,23 @@
 // join_stream.cuh — the streaming PK-FK pipeline of HashJoinExec (included by join.cu, which defines ScatterParams,
 // ProbeParams, JoinTable, ld_pair and the TMA / mbarrier helpers it uses).
 //
-// Three kernels, all HBM/L2-bound integer work (no tensor cores: nothing here is a contraction):
+// The kernels, all HBM/L2-bound integer work (no tensor cores: nothing here is a contraction):
 //
-//   k_scatter_aos<NC>   radix scatter of NC 8-byte columns into array-of-structs partition slabs.  Input tiles arrive in
-//                       shared memory by TMA bulk copies (cp.async.bulk + mbarrier, SASS UBLKCP) one tile ahead; a row's rank
-//                       inside its partition is the return value of one shared-memory histogram atomic; rows leave through
-//                       an AoS staging area as full-sector 16-byte stores.
-//   k_probe_pos<NP,NB>  probe of one partition against its L2-resident table.  Slab tiles are TMA-streamed through a ring of
-//                       shared-memory stages by a producer warp; every consumer warp is independent (no CTA barrier, no
-//                       output cursor): the output position of a probe row is its position in the partition order, so a
-//                       warp's 32 rows go to 32 consecutive slots of every output column, and a ballot word records which
-//                       slots are real.  The holes (misses, and the padding of each partition to a multiple of 32) are
-//                       filled afterwards from the tail of the result (k_hole_*): for a foreign-key join that is a few
-//                       thousand rows.  The contract is the result MULTISET (SURVEY Appendix B); order is not.
+//   k_scatter_aos<NC>   radix scatter of NC 8-byte columns into array-of-structs partition slabs (the build side, and the
+//                       aggregation's pre-pass).  Input tiles arrive in shared memory by TMA bulk copies (cp.async.bulk +
+//                       mbarrier, SASS UBLKCP) one tile ahead; a row's rank inside its partition is the return value of one
+//                       shared-memory histogram atomic; rows leave through an AoS staging area as full-sector 16-byte stores.
+//   k_pos_count         the probe side's exact partition counts (key column only), then k_pos_bases: the partition bases of
+//                       the positional result (each partition padded to 32 slots), the scatter cursors and the probe's work list.
+//   k_scatter_cols<NC>  the probe side's scatter: k_scatter_aos's tiles and ranking, but every column is written straight into
+//                       its RESULT column, at the row's final slot (base of its partition + its place in the partition order).
+//   k_probe_pos<NB>     probe of one partition against its L2-resident table.  Tiles of the result's probe KEY column are
+//                       TMA-streamed through a ring of shared-memory stages by a producer warp; every consumer warp is
+//                       independent (no CTA barrier, no output cursor): the probe columns are already in place, so a warp's 32
+//                       rows write 32 consecutive slots of every BUILD column, and a ballot word records which slots are real.
+//                       The holes (misses, and the padding of each partition to a multiple of 32) are filled afterwards from
+//                       the tail of the result (k_hole_*): for a foreign-key join that is a few thousand rows.  The contract
+//                       is the result MULTISET (SURVEY Appendix B); order is not.
 //   k_build_cluster<NB> build of the partition tables from build-side AoS slabs (one per sub-table): one 8-CTA cluster per
 //                       slab builds its sub-table in distributed shared memory and writes it out once.
 #pragma once
@@ -50,8 +54,8 @@ static constexpr int SA_MAX_BINS = (1 << SA_MAX_PBITS) + 2;
 
 static constexpr int SA_MAX_SEGS = 8;
 struct ScatterAosParams {
-  ScatterParams sp;        // columns, key, selected, pbits, cursors, slab limits (sp.out is unused)
-  uint64_t *out;           // AoS slabs: row r = out[r * NC .. r * NC + NC)
+  ScatterParams sp;        // columns, key, selected, pbits, cursors, slab limits; sp.out: the result columns of k_scatter_cols
+  uint64_t *out;           // AoS slabs of k_scatter_aos: row r = out[r * NC .. r * NC + NC)
   int use_tma;             // every input column is 16-byte aligned: whole tiles are fetched by TMA bulk copies
   // Segmented input (multi-GPU receive buffers: one region per source rank, filled by the peers' push kernels): the batch is
   // the concatenation of n_segs regions of `seg_tiles` tiles each; region g holds *seg_cnt[g] rows (a DEVICE value the
@@ -321,35 +325,315 @@ __device__ __forceinline__ uint32_t block_excl_scan(uint32_t v, uint32_t *s_warp
   return res;
 }
 
-// output base of every partition: its rows rounded up to 32 slots, so a warp's 32 rows never straddle two partitions
-static constexpr int PART_BASES_THREADS = 512;   // >= partitions of the streaming path (SA_MAX_PBITS)
-__global__ void __launch_bounds__(PART_BASES_THREADS) k_part_bases(const uint32_t *lo, const uint32_t *hi, const uint32_t *lim, int n_parts, uint32_t *out_base,
-                                                                    unsigned long long *span) {
+// Per-partition words of a positional batch, (n_parts + 1) of each.  cnt: rows of the partition (k_pos_count); base: its first
+// slot in the result, base[n_parts] = the span S (k_pos_bases); cursor: the scatter's claim cursor, from base[q] up to
+// base[q] + cnt[q]; chunk: the first probe CTA of the partition, chunk[n_parts] = the probe CTAs in all.
+struct PosMeta {
+  uint32_t *cnt, *base, *cursor, *chunk;
+};
+
+// Rows of tile `tile` of a batch (T rows per tile) and where its column c starts: one range (sp.in / sp.n), or the segmented
+// regions as k_scatter_aos reads them (region g = tiles [g * seg_tiles, (g + 1) * seg_tiles)).
+__device__ __forceinline__ int stream_tile_rows(const ScatterAosParams &q, int T, int64_t tile) {
+  if (q.n_segs == 0) {
+    const int64_t left = q.sp.n - tile * T;
+    return (int)(left < T ? left : T);
+  }
+  const int g = (int)(tile / q.seg_tiles);
+  const int64_t r0 = (tile % q.seg_tiles) * (int64_t)T;
+  const unsigned long long cnt = *q.seg_cnt[g];
+  int64_t left = cnt > (unsigned long long)q.seg_tiles * T ? 0 : (int64_t)cnt - r0;  // (an overflowed / unpublished region reads as empty)
+  if (left < 0) left = 0;
+  return (int)(left < T ? left : T);
+}
+__device__ __forceinline__ const uint64_t *stream_tile_col(const ScatterAosParams &q, int T, int64_t tile, int c) {
+  if (q.n_segs == 0) return q.sp.in[c].data + tile * T;
+  return q.seg_in[tile / q.seg_tiles][c] + (tile % q.seg_tiles) * (int64_t)T;
+}
+// The partition of a probe row on the positional path (an inner join), or -1 for a row that produces nothing: k_scatter_aos's
+// bin rule.  `row` indexes `selected` (single-range batches only).
+template <bool PLAIN>
+__device__ __forceinline__ int stream_part(const ScatterParams &p, uint64_t key, int64_t row) {
+  if constexpr (!PLAIN) {
+    const bool sel = p.selected ? (p.selected[row] != 0) : true;
+    if (!sel || !key_valid(key, true, p.key_mode)) return -1;
+  }
+  return (int)part_of_hash(tqd::hash_key(key), p.pbits);
+}
+
+// ---- exact partition counts: reads the key column alone, in the scatter's tiles (so segmented regions read the same way).
+// One shared-memory histogram per warp keeps the atomics of different warps apart; the CTA adds its histograms into cnt once.
+static constexpr int PC_THREADS = 256;
+template <int T, bool PLAIN>
+__global__ void __launch_bounds__(PC_THREADS, 8) k_pos_count(const ScatterAosParams q, uint32_t *cnt) {
+  constexpr int R = T / PC_THREADS;  // rows per thread per tile
+  constexpr int W = PC_THREADS / 32;
+  extern __shared__ uint32_t s_cnt[];  // [W][n_parts]
+  const ScatterParams &p = q.sp;
+  const int n_parts = 1 << p.pbits;
+  const int tid = threadIdx.x;
+  for (int i = tid; i < W * n_parts; i += PC_THREADS) s_cnt[i] = 0;
+  __syncthreads();
+  uint32_t *h = s_cnt + (tid >> 5) * n_parts;
+  const int64_t n_tiles = q.n_segs ? (int64_t)q.n_segs * q.seg_tiles : (p.n + T - 1) / T;
+  for (int64_t tile = blockIdx.x; tile < n_tiles; tile += gridDim.x) {
+    const int rows = stream_tile_rows(q, T, tile);
+    const uint64_t *keys = stream_tile_col(q, T, tile, p.key_col);
+    uint64_t key[R];
+#pragma unroll
+    for (int k = 0; k < R; k++) {  // R independent loads in flight
+      const int row = k * PC_THREADS + tid;
+      key[k] = row < rows ? tqd::ld_stream_u64(keys + row) : 0;
+    }
+#pragma unroll
+    for (int k = 0; k < R; k++) {
+      const int row = k * PC_THREADS + tid;
+      if (row >= rows) continue;
+      const int b = stream_part<PLAIN>(p, key[k], tile * T + row);
+      if (b >= 0) atomicAdd(&h[b], 1u);
+    }
+  }
+  __syncthreads();
+  for (int b = tid; b < n_parts; b += PC_THREADS) {
+    uint32_t s = 0;
+#pragma unroll
+    for (int w = 0; w < W; w++) s += s_cnt[w * n_parts + b];
+    if (s) atomicAdd(&cnt[b], s);
+  }
+}
+
+// ---- partition bases (one CTA): partition q's rows take slots [base[q], base[q] + cnt[q]) of the result and its run is
+// padded to a multiple of 32 slots, so a warp's 32 slots never straddle two partitions and every base is 256-byte aligned
+// in an 8-byte column (the probe's bulk copies start there).  Also the scatter cursors, the span S (*span) and the probe's
+// work list: ceil(cnt[q] / tile_rows) tiles per partition, PP_CHUNK_TILES tiles per CTA, consecutive CTAs on one partition.
+static constexpr int POS_BASES_THREADS = 512;   // >= partitions of the streaming path (SA_MAX_PBITS)
+static constexpr int PP_CHUNK_TILES = 11;       // probe tiles per CTA (~8K rows): enough CTAs per partition that only a handful of partitions are live at once
+__global__ void __launch_bounds__(POS_BASES_THREADS) k_pos_bases(const PosMeta m, int n_parts, int tile_rows, unsigned long long *span) {
   __shared__ uint32_t s_warp[33];
   const int q = threadIdx.x;
-  uint32_t padded = 0;
+  const uint32_t c = q < n_parts ? m.cnt[q] : 0u;
+  uint32_t total, ctas;
+  const uint32_t base = block_excl_scan((c + 31u) & ~31u, s_warp, &total);
+  const uint32_t tiles = (c + (uint32_t)tile_rows - 1) / (uint32_t)tile_rows;
+  const uint32_t first = block_excl_scan((tiles + PP_CHUNK_TILES - 1) / PP_CHUNK_TILES, s_warp, &ctas);
   if (q < n_parts) {
-    uint32_t h = hi[q];
-    if (lim && h > lim[q]) h = lim[q];
-    padded = ((h - lo[q]) + 31u) & ~31u;
+    m.base[q] = base;
+    m.cursor[q] = base;
+    m.chunk[q] = first;
   }
-  uint32_t total;
-  const uint32_t base = block_excl_scan(padded, s_warp, &total);
-  if (q < n_parts) out_base[q] = base;
-  if (q == 0) { out_base[n_parts] = total; *span = total; }
+  if (q == 0) {
+    m.base[n_parts] = total;
+    m.chunk[n_parts] = ctas;
+    *span = total;
+  }
+}
+
+// ---- column-wise scatter into the result: k_scatter_aos's TMA-fed tiles and shared-memory ranking; a row's slot is the run
+// its tile claims on cursor[q] (which starts at base[q]) plus its rank.  The counts are exact, so nothing can overflow.  The
+// staging area is column-major, so each column leaves as runs of consecutive 8-byte stores (consecutive threads, consecutive
+// slots).  Same shared-memory image as k_scatter_aos (sa_smem_bytes; its slab-fit table is not needed here), hence the same
+// tile size and the same segmented-region geometry.
+template <int NC, int T, bool PLAIN>
+__global__ void __launch_bounds__(SA_THREADS, sa_occ<T>(NC)) k_scatter_cols(const ScatterAosParams q) {
+  constexpr int R = T / SA_THREADS;  // rows per thread per tile
+  extern __shared__ __align__(128) unsigned char s_raw[];
+  const ScatterParams &p = q.sp;
+  const int n_parts = 1 << p.pbits;
+  const int trash = n_parts;                    // rows that produce nothing
+  const int n_bins = n_parts + 1;
+  const int bstride = (n_bins + 3) & ~3;
+  uint64_t *s_in = reinterpret_cast<uint64_t *>(s_raw);                       // [2][NC][T]
+  uint64_t *s_sorted = s_in + 2 * NC * T;                                      // [NC][T]
+  uint32_t *s_dst = reinterpret_cast<uint32_t *>(s_sorted + NC * T);           // [T] result slot of sorted position i
+  uint32_t *s_hist = s_dst + T;                                                // [n_bins] tile histogram (zero between tiles)
+  uint2 *s_bin = reinterpret_cast<uint2 *>(s_hist + bstride);                  // [n_bins] {first sorted position of the bin, slot of its first row}
+  uint64_t *s_mbar = reinterpret_cast<uint64_t *>(s_bin + bstride);            // [2]
+  __shared__ uint32_t s_warp[SA_WARPS + 1];
+
+  const int tid = threadIdx.x, lane = tid & 31, warp = tid >> 5;
+  const int kc = p.key_col;
+  const int64_t n_tiles = q.n_segs ? (int64_t)q.n_segs * q.seg_tiles : (p.n + T - 1) / T;
+  const int bpt = (n_bins + SA_THREADS - 1) / SA_THREADS;
+
+  for (int i = tid; i < n_bins; i += SA_THREADS) s_hist[i] = 0;
+  if (tid == 0) {
+    mbar_init(&s_mbar[0], 1);
+    mbar_init(&s_mbar[1], 1);
+    asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
+  }
+  __syncthreads();
+  auto tile_is_tma = [&](int64_t tile) { return q.use_tma && stream_tile_rows(q, T, tile) == T; };
+  auto issue = [&](int64_t tile, int stage) {  // thread 0 only
+    mbar_expect_tx(&s_mbar[stage], (uint32_t)(NC * T * 8));
+#pragma unroll
+    for (int c = 0; c < NC; c++) tma_load_1d(s_in + (stage * NC + c) * T, stream_tile_col(q, T, tile, c), (uint32_t)(T * 8), &s_mbar[stage]);
+  };
+  if (tid == 0) {
+    const int64_t t0 = blockIdx.x, t1 = t0 + gridDim.x;
+    if (t0 < n_tiles && tile_is_tma(t0)) issue(t0, 0);
+    if (t1 < n_tiles && tile_is_tma(t1)) issue(t1, 1);
+  }
+  int it = 0;
+  int uses0 = 0, uses1 = 0;  // TMA fills consumed per stage = the mbarrier phase to wait for (ragged tiles do not use the barrier)
+  for (int64_t tile = blockIdx.x; tile < n_tiles; tile += gridDim.x, it++) {
+    const int stage = it & 1;
+    const int rows = stream_tile_rows(q, T, tile);
+    uint64_t *in_s = s_in + stage * NC * T;
+    if (q.use_tma && rows == T) {
+      mbar_spin(&s_mbar[stage], (uint32_t)((stage ? uses1 : uses0) & 1));
+      if (stage) uses1++; else uses0++;
+    } else {  // unaligned caller buffers or a ragged / empty tile: plain loads
+#pragma unroll
+      for (int c = 0; c < NC; c++) {
+        const uint64_t *src = stream_tile_col(q, T, tile, c);
+        for (int i = tid; i < rows; i += SA_THREADS) in_s[c * T + i] = tqd::ld_stream_u64(src + i);
+      }
+      __syncthreads();
+    }
+    // ---- bin + rank of every row (rank = the histogram atomic's return value)
+    uint16_t pid[R], rank[R];
+#pragma unroll
+    for (int k = 0; k < R; k++) {
+      const int row = k * SA_THREADS + tid;
+      int b = trash;
+      if (row < rows) {
+        b = stream_part<PLAIN>(p, in_s[kc * T + row], tile * T + row);
+        if (b < 0) b = trash;
+      }
+      pid[k] = (uint16_t)b;
+      rank[k] = (uint16_t)atomicAdd(&s_hist[b], 1u);
+    }
+    __syncthreads();
+    // ---- exclusive scan over the bins; every non-empty partition claims its run of slots with ONE global atomic
+    uint32_t tsum = 0;
+    for (int j = 0; j < bpt; j++) {
+      const int b = tid * bpt + j;
+      if (b < n_bins) tsum += s_hist[b];
+    }
+    uint32_t inc = tsum;
+#pragma unroll
+    for (int d = 1; d < 32; d <<= 1) { const uint32_t x = __shfl_up_sync(0xffffffffu, inc, d); if (lane >= d) inc += x; }
+    if (lane == 31) s_warp[warp] = inc;
+    __syncthreads();
+    if (warp == 0) {
+      uint32_t w = (lane < SA_WARPS) ? s_warp[lane] : 0, winc = w;
+#pragma unroll
+      for (int d = 1; d < 32; d <<= 1) { const uint32_t x = __shfl_up_sync(0xffffffffu, winc, d); if (lane >= d) winc += x; }
+      if (lane < SA_WARPS) s_warp[lane] = winc - w;
+    }
+    __syncthreads();
+    uint32_t run = inc - tsum + s_warp[warp];
+    for (int j = 0; j < bpt; j++) {
+      const int b = tid * bpt + j;
+      if (b < n_bins) {
+        const uint32_t c = s_hist[b];
+        s_hist[b] = 0;  // ready for the next tile (its ranking starts behind two more barriers)
+        const uint32_t g = (c && b != trash) ? atomicAdd(&p.part_cursor[b], c) : 0u;
+        s_bin[b] = make_uint2(run, g);
+        run += c;
+      }
+    }
+    __syncthreads();
+    const uint32_t total = s_bin[trash].x;  // rows that go somewhere
+    // ---- place the rows at their sorted positions (column-major) together with their result slot
+#pragma unroll
+    for (int k = 0; k < R; k++) {
+      const uint32_t b = pid[k];
+      if (b == (uint32_t)trash) continue;
+      const int row = k * SA_THREADS + tid;
+      const uint2 bin = s_bin[b];
+      const uint32_t sp = bin.x + rank[k];
+      s_dst[sp] = bin.y + rank[k];
+#pragma unroll
+      for (int c = 0; c < NC; c++) s_sorted[c * T + sp] = in_s[c * T + row];
+    }
+    __syncthreads();
+    // the input stage is free again: fetch the tile this CTA handles two iterations from now
+    if (tid == 0) {
+      const int64_t nt = tile + 2 * (int64_t)gridDim.x;
+      if (nt < n_tiles && tile_is_tma(nt)) issue(nt, stage);
+    }
+    // ---- stream the sorted tile out: consecutive threads write consecutive slots of every result column
+    for (uint32_t i = tid; i < total; i += SA_THREADS) {
+      const uint32_t d = s_dst[i];
+#pragma unroll
+      for (int c = 0; c < NC; c++) tqd::st_stream_u64(p.out[c].data + d, s_sorted[c * T + i]);
+    }
+    __syncthreads();  // the staging area and the bin tables are rewritten by the next tile
+  }
+}
+
+typedef void (*ScatterColsKernel)(const ScatterAosParams);
+template <int T, bool PLAIN>
+static ScatterColsKernel scatter_cols_kernel_t(int nc) {
+  if (T == 4096) return nc == 1 ? k_scatter_cols<1, 4096, PLAIN> : (nc == 2 ? k_scatter_cols<2, 4096, PLAIN> : nullptr);
+  switch (nc) {
+    case 1: return k_scatter_cols<1, 2048, PLAIN>;
+    case 2: return k_scatter_cols<2, 2048, PLAIN>;
+    case 3: return k_scatter_cols<3, 2048, PLAIN>;
+    case 4: return k_scatter_cols<4, 2048, PLAIN>;
+  }
+  return nullptr;
+}
+// Rows per tile of the column scatter: 4096 where that shared-memory image fits an SM (one or two columns), else 2048.  A run
+// a tile claims in one partition is then ~T / P rows of every column: at C3 (128 partitions) 4096-row tiles write runs of
+// 256 bytes per column, which measured 1.39 ms against 1.65 ms for 2048-row tiles (H100 80GB HBM3, 700 W).
+static int scatter_cols_tile(int nc, int bins) { return sa_smem_bytes<4096>(nc, bins) <= 220 * 1024 ? 4096 : 2048; }
+// Segmented regions are counted and scattered in tiles of different sizes, so a region's rows are a multiple of the largest.
+static constexpr int POS_SEG_ROWS_ALIGN = 4096;
+static constexpr int PC_TILE = 2048;  // rows per tile of k_pos_count
+
+// count -> bases -> column-wise scatter of one positional batch into the result columns q.sp.out[c] (every slot of
+// [0, S) belongs to exactly one partition run or pad).  q describes the input as for k_scatter_aos (columns, key, key_mode,
+// selected, pbits, n, segments of seg_rows rows each, a multiple of POS_SEG_ROWS_ALIGN); m's words are reserved by the caller.
+static int32_t launch_pos_scatter(ScatterAosParams &q, int64_t seg_rows, const PosMeta &m, int probe_tile, unsigned long long *span, cudaStream_t s) {
+  const int nc = q.sp.n_cols, P = 1 << q.sp.pbits;
+  const bool plain = !q.sp.selected && q.sp.key_mode == KEYMODE_RAW;
+  auto n_tiles = [&](int T) { return q.n_segs ? (int64_t)q.n_segs * (seg_rows / T) : (q.sp.n + T - 1) / T; };
+  // counts
+  TQ_CUDA(cudaMemsetAsync(m.cnt, 0, (size_t)P * 4, s));
+  q.seg_tiles = (int)(seg_rows / PC_TILE);
+  const int cnt_smem = (PC_THREADS / 32) * P * 4;
+  const int64_t cnt_tiles = n_tiles(PC_TILE), cnt_cap = (int64_t)rt().sm_count * 8;
+  const int cnt_grid = (int)(cnt_tiles < cnt_cap ? (cnt_tiles < 1 ? 1 : cnt_tiles) : cnt_cap);
+  (plain ? k_pos_count<PC_TILE, true> : k_pos_count<PC_TILE, false>)<<<cnt_grid, PC_THREADS, cnt_smem, s>>>(q, m.cnt);
+  TQ_TRY(check_launch("k_pos_count"));
+  k_pos_bases<<<1, POS_BASES_THREADS, 0, s>>>(m, P, probe_tile, span);
+  TQ_TRY(check_launch("k_pos_bases"));
+  // scatter
+  const int T = scatter_cols_tile(nc, P + 1);
+  ScatterColsKernel k = T == 4096 ? (plain ? scatter_cols_kernel_t<4096, true>(nc) : scatter_cols_kernel_t<4096, false>(nc))
+                                  : (plain ? scatter_cols_kernel_t<2048, true>(nc) : scatter_cols_kernel_t<2048, false>(nc));
+  const int smem = T == 4096 ? sa_smem_bytes<4096>(nc, P + 1) : sa_smem_bytes<2048>(nc, P + 1);
+  int per_sm = T == 4096 ? sa_occ<4096>(nc) : sa_occ<2048>(nc);
+  if (!k || smem > 227 * 1024) { set_error("internal: column scatter of %d columns into %d partitions does not fit shared memory", nc, P); return TQ_ERR_INVALID_ARG; }
+  TQ_CUDA(cudaFuncSetAttribute(k, cudaFuncAttributeMaxDynamicSharedMemorySize, smem));
+  while (per_sm > 1 && (int64_t)smem * per_sm > 224 * 1024) per_sm--;
+  const int64_t tiles = n_tiles(T), cap = (int64_t)rt().sm_count * per_sm;
+  q.seg_tiles = (int)(seg_rows / T);
+  q.sp.part_cursor = m.cursor;
+  auto aligned = [](const void *ptr) { return (reinterpret_cast<uintptr_t>(ptr) & 15) == 0; };
+  q.use_tma = 1;
+  for (int c = 0; c < nc; c++) {
+    if (!aligned(q.sp.in[c].data)) q.use_tma = 0;
+    for (int g = 0; g < q.n_segs; g++)
+      if (!aligned(q.seg_in[g][c])) q.use_tma = 0;
+  }
+  k<<<(int)(tiles < cap ? (tiles < 1 ? 1 : tiles) : cap), SA_THREADS, smem, s>>>(q);
+  count_launch(3);
+  return check_launch("k_scatter_cols");
 }
 
 static constexpr int PP_STAGES = 4;
 
 struct ProbePosParams {
-  const uint64_t *slab;              // AoS probe rows (NP words each), partition q = rows [lo[q], min(hi[q], lim[q]))
-  const uint32_t *lo, *hi, *lim;
-  const uint32_t *out_base;          // k_part_bases
-  uint64_t *out_probe[4], *out_build[4];
+  const uint64_t *keys;              // the result's probe key column: partition q = slots [base[q], base[q] + cnt[q])
+  const uint32_t *cnt, *base, *chunk;  // PosMeta
+  int n_parts;
+  uint64_t *out_build[4];
   int build_word[4];                 // word of build column c inside a table entry
   uint32_t *valid;                   // one bit per output slot
   unsigned long long *cursor;        // [0] += matched rows
-  int key_col, split;
   int dbg_no_tma, dbg_late_release;  // diagnostics (TQ_JOIN_PP_DEBUG bit 0 / bit 1): plain copies by the producer warp; release a stage only after the step
 };
 
@@ -387,25 +671,33 @@ __device__ __forceinline__ bool probe_find(const uint64_t *words, uint32_t cap, 
 }
 
 // R rows per lane per step, CW consumer warps (+ 1 producer warp), OCC resident CTAs per SM asked of the compiler.
-// One tile = CW * 32 * R rows.
-template <int NP, int NB, int R, int CW, int OCC>
+// One tile = CW * 32 * R rows.  The probe columns are already in their result slots (k_scatter_cols): this kernel reads the
+// key column back and writes the build columns and the validity ballots.
+template <int NB, int R, int CW, int OCC>
 __global__ void __launch_bounds__((CW + 1) * 32, OCC) k_probe_pos(const ProbePosParams p, const JoinTable t) {
   constexpr int PP_TILE = CW * 32 * R;
   constexpr int PP_CONSUMER_WARPS = CW;
   constexpr int SHIFT = NB > 2 ? 2 : 1;  // words per entry = 1 << SHIFT (the host builds the table the same way)
   extern __shared__ __align__(128) unsigned char s_raw[];
-  uint64_t *s_tile = reinterpret_cast<uint64_t *>(s_raw);  // [PP_STAGES][PP_TILE][NP]
+  uint64_t *s_tile = reinterpret_cast<uint64_t *>(s_raw);  // [PP_STAGES][PP_TILE] probe keys
   __shared__ __align__(8) uint64_t s_full[PP_STAGES], s_empty[PP_STAGES];
   __shared__ uint64_t s_sink[CW];
   const int tid = threadIdx.x, lane = tid & 31, warp = tid >> 5;
-  const uint32_t part = blockIdx.x / p.split, sub = blockIdx.x % p.split;
-  const int64_t p_lo = p.lo[part];
-  int64_t p_hi = p.hi[part];
-  if (p.lim && p_hi > (int64_t)p.lim[part]) p_hi = p.lim[part];
-  const int64_t p_rows = p_hi - p_lo;
+  // this CTA's partition and tiles, from the work list of k_pos_bases: chunk[part] <= blockIdx.x < chunk[part + 1]
+  const uint32_t cta = blockIdx.x;
+  if (cta >= p.chunk[p.n_parts]) return;  // (the grid is sized for the worst case)
+  uint32_t part = 0, hi = (uint32_t)p.n_parts;
+  while (hi - part > 1) {
+    const uint32_t mid = (part + hi) >> 1;
+    if (p.chunk[mid] <= cta) part = mid;
+    else hi = mid;
+  }
+  const int64_t p_rows = p.cnt[part];
   const int64_t p_tiles = (p_rows + PP_TILE - 1) / PP_TILE;
-  const int64_t t_lo = p_tiles * sub / p.split, t_hi = p_tiles * (sub + 1) / p.split;
-  if (t_lo >= t_hi) return;
+  const int64_t t_lo = (int64_t)(cta - p.chunk[part]) * PP_CHUNK_TILES;
+  const int64_t t_hi = t_lo + PP_CHUNK_TILES < p_tiles ? t_lo + PP_CHUNK_TILES : p_tiles;
+  const uint64_t p_base = p.base[part];
+  const uint64_t *keys = p.keys + p_base;  // 256-byte aligned: the bases are multiples of 32 slots
   if (tid == 0) {
     for (int s = 0; s < PP_STAGES; s++) { mbar_init(&s_full[s], 1); mbar_init(&s_empty[s], PP_CONSUMER_WARPS); }
     asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
@@ -418,16 +710,16 @@ __global__ void __launch_bounds__((CW + 1) * 32, OCC) k_probe_pos(const ProbePos
       if (it >= PP_STAGES) mbar_spin(&s_empty[s], (uint32_t)(((it / PP_STAGES) - 1) & 1));
       const int64_t r0 = tile * PP_TILE;
       const int64_t rows = (p_rows - r0) < PP_TILE ? (p_rows - r0) : PP_TILE;
-      uint64_t *dst = s_tile + (size_t)s * PP_TILE * NP;
-      const uint64_t *srcg = p.slab + (p_lo + r0) * NP;
-      for (int64_t i = lane; i < rows * NP; i += 32) dst[i] = srcg[i];
+      uint64_t *dst = s_tile + (size_t)s * PP_TILE;
+      for (int64_t i = lane; i < rows; i += 32) dst[i] = keys[r0 + i];
       __syncwarp();
       if (lane == 0) mbar_arrive(&s_full[s]);
     }
     return;
   }
   if (warp == PP_CONSUMER_WARPS) {
-    // ---- producer: keeps PP_STAGES slab tiles in flight (TMA bulk copies; bytes rounded up to 16: the slab allocation is padded)
+    // ---- producer: keeps PP_STAGES key tiles in flight (TMA bulk copies; bytes rounded up to 16: an odd row count ends
+    // inside the partition's pad)
     if (lane == 0) {
       int it = 0;
       for (int64_t tile = t_lo; tile < t_hi; tile++, it++) {
@@ -435,9 +727,9 @@ __global__ void __launch_bounds__((CW + 1) * 32, OCC) k_probe_pos(const ProbePos
         if (it >= PP_STAGES) mbar_spin(&s_empty[s], (uint32_t)(((it / PP_STAGES) - 1) & 1));
         const int64_t r0 = tile * PP_TILE;
         const int64_t rows = (p_rows - r0) < PP_TILE ? (p_rows - r0) : PP_TILE;
-        const uint32_t bytes = (uint32_t)((rows * NP * 8 + 15) & ~15ll);
+        const uint32_t bytes = (uint32_t)((rows * 8 + 15) & ~15ll);
         mbar_expect_tx(&s_full[s], bytes);
-        tma_load_1d(s_tile + (size_t)s * PP_TILE * NP, p.slab + (p_lo + r0) * NP, bytes, &s_full[s]);
+        tma_load_1d(s_tile + (size_t)s * PP_TILE, keys + r0, bytes, &s_full[s]);
       }
     }
     return;
@@ -445,13 +737,10 @@ __global__ void __launch_bounds__((CW + 1) * 32, OCC) k_probe_pos(const ProbePos
   // ---- consumers: warp w owns rows [w * 32 * R, (w + 1) * 32 * R) of every tile.  The table may be split finer than the
   // probe partitions (k_build_cluster's sub-tables), so a row's table comes from its own hash.
   const uint32_t cap = t.cap;
-  const int kc = p.key_col;
   const int woff = warp * (32 * R) + lane;                      // this lane's first row inside a tile
-  const uint64_t obase = (uint64_t)p.out_base[part] + woff;     // ... and its output slot inside the partition's range
-  uint64_t *op[NP], *ob[NB];
+  const uint64_t obase = p_base + woff;                         // ... and its output slot inside the partition's range
+  uint64_t *ob[NB];
   int bw[NB];
-#pragma unroll
-  for (int c = 0; c < NP; c++) op[c] = p.out_probe[c] + obase;
 #pragma unroll
   for (int c = 0; c < NB; c++) { ob[c] = p.out_build[c] + obase; bw[c] = p.build_word[c]; }
   uint32_t *vword = p.valid + ((obase - lane) >> 5);
@@ -461,43 +750,27 @@ __global__ void __launch_bounds__((CW + 1) * 32, OCC) k_probe_pos(const ProbePos
     const int s = it % PP_STAGES;
     mbar_spin(&s_full[s], (uint32_t)((it / PP_STAGES) & 1));
     const int64_t t0 = tile * PP_TILE;                              // first row of the tile inside the partition
-    const uint64_t *src = s_tile + ((size_t)s * PP_TILE + woff) * NP;
-    uint64_t v[R][NP];
+    const uint64_t *src = s_tile + (size_t)s * PP_TILE + woff;
+    uint64_t key[R];
 #pragma unroll
-    for (int k = 0; k < R; k++) {
-      if constexpr (NP == 2) {
-        const ulonglong2 x = *reinterpret_cast<const ulonglong2 *>(src + (size_t)k * 32 * NP);
-        v[k][0] = x.x;
-        v[k][1] = x.y;
-      } else {
-#pragma unroll
-        for (int c = 0; c < NP; c++) v[k][c] = src[(size_t)k * 32 * NP + c];
-      }
-    }
+    for (int k = 0; k < R; k++) key[k] = src[k * 32];
     // The stage may be refilled (a TMA write) as soon as every warp has released it, so the values must have LEFT shared
     // memory first.  An issued LDS is not a completed one: SASS showed LDS.128 x4, WARPSYNC, SYNCS.ARRIVE with no scoreboard
     // wait in between, and the refill then tore rows (first 16 bytes of one tile, last 16 of another).  The register scoreboard is per warp, so ONE instruction that reads every loaded
     // register waits for the whole warp's loads: lane 0 stores their XOR to a sink word before it arrives on the barrier.
     uint64_t dep = 0;
 #pragma unroll
-    for (int k = 0; k < R; k++) {
-#pragma unroll
-      for (int c = 0; c < NP; c++) dep ^= v[k][c];
-    }
+    for (int k = 0; k < R; k++) dep ^= key[k];
     __syncwarp();
     if (lane == 0) {
       *reinterpret_cast<volatile uint64_t *>(&s_sink[warp]) = dep;
       if (!p.dbg_late_release) mbar_arrive(&s_empty[s]);  // the stage can be refilled while this warp probes
     }
-    uint64_t key[R];
     uint32_t loc[R];  // entry index in the whole table (probe_find)
     bool inb[R];
     ulonglong2 ea[R], eb[R];
 #pragma unroll
     for (int k = 0; k < R; k++) {  // R independent sector loads in flight
-      key[k] = v[k][0];
-#pragma unroll
-      for (int c = 1; c < NP; c++) if (c == kc) key[k] = v[k][c];
       inb[k] = (t0 + woff + k * 32) < p_rows;
       const uint64_t h = tqd::hash_key(key[k]);
       loc[k] = (uint32_t)part_of_hash(h, t.pbits) * cap + home_slot(h, cap, SHIFT);
@@ -508,7 +781,7 @@ __global__ void __launch_bounds__((CW + 1) * 32, OCC) k_probe_pos(const ProbePos
         else ea[k] = ld_entry(t.words, loc[k], SHIFT);
       }
     }
-    const int64_t oslot = t0;  // output slot of this lane's k-th row = op[c] + oslot + k * 32
+    const int64_t oslot = t0;  // output slot of this lane's k-th row = ob[c] + oslot + k * 32
 #pragma unroll
     for (int k = 0; k < R; k++) {
       uint64_t w1 = 0;
@@ -528,8 +801,6 @@ __global__ void __launch_bounds__((CW + 1) * 32, OCC) k_probe_pos(const ProbePos
         matched += __popc(bal);
       }
       if (hit) {
-#pragma unroll
-        for (int c = 0; c < NP; c++) tqd::st_stream_u64(op[c] + oslot + k * 32, v[k][c]);
 #pragma unroll
         for (int c = 0; c < NB; c++) {
           uint64_t x;
@@ -553,28 +824,18 @@ struct ProbePosVariant {
   ProbePosKernel k;
   int tile, threads;
 };
-template <int NP, int NB>
+template <int NB>
 static ProbePosVariant probe_pos_variant() {
   // 2 rows per lane x 12 consumer warps x 3 CTAs per SM: more warps in flight hide the L2 latency of the table gathers better
   // than more loads per warp (4 rows per lane spills at 3 CTAs per SM).
-  return {k_probe_pos<NP, NB, 2, 12, 3>, 12 * 32 * 2, 13 * 32};
+  return {k_probe_pos<NB, 2, 12, 3>, 12 * 32 * 2, 13 * 32};
 }
-template <int NP>
-static ProbePosVariant probe_pos_nb(int nb) {
+static ProbePosVariant probe_pos_kernel(int nb) {
   switch (nb) {
-    case 1: return probe_pos_variant<NP, 1>();
-    case 2: return probe_pos_variant<NP, 2>();
-    case 3: return probe_pos_variant<NP, 3>();
-    case 4: return probe_pos_variant<NP, 4>();
-  }
-  return {nullptr, 0, 0};
-}
-static ProbePosVariant probe_pos_kernel(int np, int nb) {
-  switch (np) {
-    case 1: return probe_pos_nb<1>(nb);
-    case 2: return probe_pos_nb<2>(nb);
-    case 3: return probe_pos_nb<3>(nb);
-    case 4: return probe_pos_nb<4>(nb);
+    case 1: return probe_pos_variant<1>();
+    case 2: return probe_pos_variant<2>();
+    case 3: return probe_pos_variant<3>();
+    case 4: return probe_pos_variant<4>();
   }
   return {nullptr, 0, 0};
 }
