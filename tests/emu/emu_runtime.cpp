@@ -6,6 +6,8 @@
 #include <cstdio>
 
 #include "common.cuh"
+#include "dict.cuh"
+#include "strdict.cuh"
 #include "varlen.cuh"
 
 namespace tq_emu {
@@ -219,3 +221,60 @@ extern "C" int32_t tq_memcpy_d2d(void *dst, const void *src, size_t bytes) { if 
 extern "C" int32_t tq_memset_device(void *dst, int32_t v, size_t bytes) { if (bytes) memset(dst, v, bytes); return TQ_OK; }
 extern "C" int32_t tq_device_alloc(size_t bytes, void **out) { *out = malloc(bytes ? bytes : 1); return *out ? TQ_OK : TQ_ERR_OOM; }
 extern "C" int32_t tq_device_free(void *p) { free(p); return TQ_OK; }
+
+// The key dictionaries (dict.cu, strdict.cu), for tests/test_emu_dicts.py: the string hash of one byte range through k_sd_hash,
+// and thin handles that encode one batch of a StringDict / MultiKeyEncoder and report the table geometry it grew to.
+// Test-only exports, not part of the product ABI.
+namespace tq {
+void k_sd_hash(const StrView v, const uint32_t *bm, int64_t n, uint64_t *row_hash);
+}
+extern "C" uint64_t tq_emu_sd_hash(const uint8_t *bytes, int64_t len) {
+  const int64_t off[2] = {0, len};
+  tq::StrView v;
+  v.off = off;
+  v.bytes = bytes;
+  uint64_t h = 0;
+  TQ_LAUNCH(tq::k_sd_hash, 1, 32, 0, nullptr, v, nullptr, 1, &h);
+  return h;
+}
+
+extern "C" void *tq_emu_sd_new() { return new tq::StringDict(); }
+extern "C" void tq_emu_sd_free(void *d) { delete static_cast<tq::StringDict *>(d); }
+// cells r = bytes[off[r], off[r + 1]); bm: optional NOT-NULL bitmap (32-bit words).  out_geom = {count, n_slots}.
+extern "C" int32_t tq_emu_sd_encode(void *d, const int64_t *off, const uint8_t *bytes, const uint32_t *bm, int64_t n, int32_t insert, uint64_t *ids_out,
+                                    uint32_t *valid_out, uint64_t *out_geom) {
+  auto *sd = static_cast<tq::StringDict *>(d);
+  tq::StrView v;
+  v.off = off;
+  v.base = 0;
+  v.bytes = bytes;
+  const int32_t rc = sd->encode(v, bm, n, n > 0 ? off[n] - off[0] : 0, insert != 0, ids_out, valid_out, nullptr);
+  out_geom[0] = sd->count;
+  out_geom[1] = sd->n_slots;
+  return rc;
+}
+
+extern "C" void *tq_emu_mk_new(int32_t k) {
+  auto *e = new tq::MultiKeyEncoder();
+  e->k = k;
+  return e;
+}
+extern "C" void tq_emu_mk_free(void *e) { delete static_cast<tq::MultiKeyEncoder *>(e); }
+// cols[i] / bms[i]: column i of the k key columns (bms[i] may be null).  out_geom = {count, n_slots} of col[0..k) followed by
+// those of the pair dictionaries fold[1..k-1).
+extern "C" int32_t tq_emu_mk_encode(void *h, const uint64_t *const *cols, const uint32_t *const *bms, const uint8_t *no_signbit, int64_t n, int32_t insert,
+                                    int32_t null_is_value, uint64_t *out_comb, uint32_t *out_bm, uint64_t *out_geom) {
+  auto *e = static_cast<tq::MultiKeyEncoder *>(h);
+  tq::DCol kc[tq::MK_MAX_KEYS];
+  bool ns[tq::MK_MAX_KEYS] = {};
+  for (int i = 0; i < e->k && i < tq::MK_MAX_KEYS; i++) {
+    kc[i].data = cols[i];
+    kc[i].bm = bms ? bms[i] : nullptr;
+    ns[i] = no_signbit && no_signbit[i];
+  }
+  const int32_t rc = e->encode(kc, ns, n, insert != 0, null_is_value != 0, out_comb, out_bm, nullptr);
+  int g = 0;
+  for (int i = 0; i < e->k; i++) { out_geom[g++] = e->col[i].count; out_geom[g++] = e->col[i].n_slots; }
+  for (int i = 1; i < e->k - 1; i++) { out_geom[g++] = e->fold[i].count; out_geom[g++] = e->fold[i].n_slots; }
+  return rc;
+}

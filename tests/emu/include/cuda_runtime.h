@@ -1,6 +1,6 @@
 // cuda_runtime.h of the CPU EMULATION build (tests/emu) — TEST INFRASTRUCTURE, never part of the product library.
 //
-// tests/emu compiles product sources (tinysql_b200/csrc/sort.cu, codec.cu) unchanged with g++: this header stands in for the CUDA
+// tests/emu compiles product sources (tinysql_b200/csrc/sort.cu, codec.cu, dict.cu, strdict.cu ...) unchanged with g++: this header stands in for the CUDA
 // runtime and maps the handful of device primitives those kernels use onto host threads — ONE OS thread per CUDA thread of a
 // block, blocks run one after another, __syncthreads() and the warp collectives are pthread barriers.  Slow, but it executes
 // the real kernel code (indexing, ranking, masks, binary searches) so `-m "not gpu"` can check it against the oracle.
@@ -79,6 +79,20 @@ static inline T __shfl_xor_sync(unsigned, T v, int lane_mask) {
   memcpy(&r, &got, sizeof(T));
   return r;
 }
+template <typename T>
+static inline T __shfl_sync(unsigned, T v, int src_lane) {
+  static_assert(sizeof(T) <= 8, "shuffle of at most 8 bytes");
+  const int w = tq_emu::cur >> 5, lane = tq_emu::cur & 31;
+  uint64_t bits = 0;
+  memcpy(&bits, &v, sizeof(T));
+  tq_emu::warp_slot[w][lane] = bits;
+  tq_emu::warp_sync();
+  const uint64_t got = tq_emu::warp_slot[w][src_lane & 31];
+  tq_emu::warp_sync();
+  T r;
+  memcpy(&r, &got, sizeof(T));
+  return r;
+}
 static inline unsigned __ballot_sync(unsigned, bool pred) {
   const int w = tq_emu::cur >> 5, lane = tq_emu::cur & 31;
   tq_emu::warp_slot[w][lane] = pred ? 1 : 0;
@@ -88,6 +102,7 @@ static inline unsigned __ballot_sync(unsigned, bool pred) {
   tq_emu::warp_sync();
   return m;
 }
+static inline int __any_sync(unsigned mask, int pred) { return __ballot_sync(mask, pred != 0) != 0; }
 static inline unsigned __match_any_sync(unsigned, unsigned v) {
   const int w = tq_emu::cur >> 5, lane = tq_emu::cur & 31;
   tq_emu::warp_slot[w][lane] = v;
@@ -101,6 +116,14 @@ static inline int __popc(unsigned v) { return __builtin_popcount(v); }
 
 static inline unsigned atomicAdd(unsigned *p, unsigned v) { return __atomic_fetch_add(p, v, __ATOMIC_SEQ_CST); }
 static inline unsigned long long atomicAdd(unsigned long long *p, unsigned long long v) { return __atomic_fetch_add(p, v, __ATOMIC_SEQ_CST); }
+static inline unsigned atomicCAS(unsigned *p, unsigned expected, unsigned v) {
+  __atomic_compare_exchange_n(p, &expected, v, false, __ATOMIC_SEQ_CST, __ATOMIC_SEQ_CST);
+  return expected;   // the old value, whether or not it was swapped
+}
+static inline unsigned long long atomicCAS(unsigned long long *p, unsigned long long expected, unsigned long long v) {
+  __atomic_compare_exchange_n(p, &expected, v, false, __ATOMIC_SEQ_CST, __ATOMIC_SEQ_CST);
+  return expected;
+}
 static inline unsigned long long atomicMax(unsigned long long *p, unsigned long long v) {
   unsigned long long cur = __atomic_load_n(p, __ATOMIC_SEQ_CST);
   while (cur < v && !__atomic_compare_exchange_n(p, &cur, v, false, __ATOMIC_SEQ_CST, __ATOMIC_SEQ_CST)) {}

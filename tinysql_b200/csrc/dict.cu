@@ -117,13 +117,13 @@ int32_t KeyDict::ensure(uint64_t extra, cudaStream_t s) {
   DevBuf nk, ni;
   TQ_TRY(nk.reserve(want * 8));
   TQ_TRY(ni.reserve(want * 4));
-  k_dict_fill<<<dict_grid((int64_t)want), 256, 0, s>>>(nk.as<uint64_t>(), want);
+  TQ_LAUNCH(k_dict_fill, dict_grid((int64_t)want), 256, 0, s, nk.as<uint64_t>(), want);
   count_launch();
   if (n_slots == 0) {
     TQ_TRY(meta.reserve(64));
     TQ_CUDA(cudaMemsetAsync(meta.p, 0, 64, s));
   } else {
-    k_dict_rehash<<<dict_grid((int64_t)n_slots), 256, 0, s>>>(keys.as<uint64_t>(), ids.as<uint32_t>(), n_slots, nk.as<uint64_t>(), ni.as<uint32_t>(), want - 1);
+    TQ_LAUNCH(k_dict_rehash, dict_grid((int64_t)n_slots), 256, 0, s, keys.as<uint64_t>(), ids.as<uint32_t>(), n_slots, nk.as<uint64_t>(), ni.as<uint32_t>(), want - 1);
     count_launch();
   }
   TQ_TRY(check_launch("k_dict_rehash"));
@@ -138,7 +138,7 @@ int32_t KeyDict::insert(const uint64_t *vals, const uint32_t *bm, int64_t n, boo
   for (int64_t off = 0; off < n; off += DICT_SUB_BATCH) {
     const int64_t m = n - off < DICT_SUB_BATCH ? n - off : DICT_SUB_BATCH;
     TQ_TRY(ensure((uint64_t)m, s));
-    k_dict_insert<<<dict_grid(m), 256, 0, s>>>(keys.as<uint64_t>(), ids.as<uint32_t>(), n_slots - 1, meta.as<unsigned>(), vals, bm, off, m, skip_miss ? 1 : 0);
+    TQ_LAUNCH(k_dict_insert, dict_grid(m), 256, 0, s, keys.as<uint64_t>(), ids.as<uint32_t>(), n_slots - 1, meta.as<unsigned>(), vals, bm, off, m, skip_miss ? 1 : 0);
     count_launch();
     TQ_TRY(check_launch("k_dict_insert"));
     uint32_t c = 0;
@@ -154,8 +154,8 @@ int32_t KeyDict::lookup(const uint64_t *vals, const uint32_t *bm, int64_t n, uin
                         cudaStream_t s) const {
   if (n <= 0) return TQ_OK;
   if (n_slots == 0) { set_error("internal: lookup in an unallocated key dictionary"); return TQ_ERR_STATE; }
-  k_dict_lookup<<<dict_grid(n), 256, 0, s>>>(keys.as<uint64_t>(), ids.as<uint32_t>(), n_slots - 1, vals, bm, n, null_id, no_signbit ? 1 : 0,
-                                              skip_miss ? 1 : 0, out);
+  TQ_LAUNCH(k_dict_lookup, dict_grid(n), 256, 0, s, keys.as<uint64_t>(), ids.as<uint32_t>(), n_slots - 1, vals, bm, n, null_id, no_signbit ? 1 : 0,
+            skip_miss ? 1 : 0, out);
   count_launch();
   return check_launch("k_dict_lookup");
 }
@@ -179,7 +179,7 @@ int32_t MultiKeyEncoder::encode(const DCol *keycols, const bool *no_signbit, int
   for (int i = 1; i < k; i++) {
     TQ_TRY(col[i].lookup(keycols[i].data, keycols[i].bm, n, null_id, no_signbit && no_signbit[i], false, tmp.as<uint32_t>(), s));
     uint64_t *dst = (i == k - 1) ? out_comb : pair.as<uint64_t>();
-    k_dict_pair<<<dict_grid(n), 256, 0, s>>>(acc.as<uint32_t>(), tmp.as<uint32_t>(), n, dst);
+    TQ_LAUNCH(k_dict_pair, dict_grid(n), 256, 0, s, acc.as<uint32_t>(), tmp.as<uint32_t>(), n, dst);
     count_launch();
     TQ_TRY(check_launch("k_dict_pair"));
     if (i < k - 1) {
@@ -188,7 +188,7 @@ int32_t MultiKeyEncoder::encode(const DCol *keycols, const bool *no_signbit, int
     }
   }
   if (out_bm) {
-    k_dict_valid_bitmap<<<dict_grid(n), 256, 0, s>>>(out_comb, n, out_bm);
+    TQ_LAUNCH(k_dict_valid_bitmap, dict_grid(n), 256, 0, s, out_comb, n, out_bm);
     count_launch();
     TQ_TRY(check_launch("k_dict_valid_bitmap"));
   }

@@ -215,7 +215,7 @@ int32_t StringDict::ensure(uint64_t extra_strings, uint64_t extra_bytes, cudaStr
     TQ_TRY(ns.reserve((size_t)want * 4));
     TQ_CUDA(cudaMemsetAsync(ns.p, 0xFF, (size_t)want * 4, s));
     if (count) {
-      k_sd_rehash<<<sd_thread_grid((int64_t)count), 256, 0, s>>>(ns.as<uint32_t>(), want - 1, a_hash.as<uint64_t>(), count);
+      TQ_LAUNCH(k_sd_rehash, sd_thread_grid((int64_t)count), 256, 0, s, ns.as<uint32_t>(), want - 1, a_hash.as<uint64_t>(), count);
       count_launch();
       TQ_TRY(check_launch("k_sd_rehash"));
     }
@@ -232,7 +232,7 @@ int32_t StringDict::encode(const StrView &v, const uint32_t *bm, int64_t n, int6
   TQ_TRY(ensure(insert ? (uint64_t)n : 0, insert ? (uint64_t)(batch_bytes > 0 ? batch_bytes : 0) : 0, s));
   if (n <= 0) return TQ_OK;
   TQ_TRY(row_hash.reserve((size_t)n * 8));
-  k_sd_hash<<<sd_warp_grid(n), 256, 0, s>>>(v, bm, n, row_hash.as<uint64_t>());
+  TQ_LAUNCH(k_sd_hash, sd_warp_grid(n), 256, 0, s, v, bm, n, row_hash.as<uint64_t>());
   count_launch();
   TQ_TRY(check_launch("k_sd_hash"));
   if (insert) {
@@ -242,10 +242,10 @@ int32_t StringDict::encode(const StrView &v, const uint32_t *bm, int64_t n, int6
     unsigned *d_n_new = meta.as<unsigned>();
     uint64_t *d_total = reinterpret_cast<uint64_t *>(meta.as<uint8_t>() + 8);
     TQ_CUDA(cudaMemsetAsync(meta.p, 0, 16, s));
-    k_sd_insert<<<sd_warp_grid(n), 256, 0, s>>>(v, bm, n, row_hash.as<uint64_t>(), slots.as<uint32_t>(), n_slots - 1, arena.offsets.as<int64_t>(), a_hash.as<uint64_t>(),
-                                                arena.bytes.as<uint8_t>());
-    k_sd_assign<<<sd_thread_grid((int64_t)n_slots), 256, 0, s>>>(slots.as<uint32_t>(), n_slots, v, row_hash.as<uint64_t>(), (uint32_t)count, d_n_new, new_src.as<uint32_t>(),
-                                                                 new_len.as<uint32_t>(), a_hash.as<uint64_t>());
+    TQ_LAUNCH(k_sd_insert, sd_warp_grid(n), 256, 0, s, v, bm, n, row_hash.as<uint64_t>(), slots.as<uint32_t>(), n_slots - 1, arena.offsets.as<int64_t>(), a_hash.as<uint64_t>(),
+              arena.bytes.as<uint8_t>());
+    TQ_LAUNCH(k_sd_assign, sd_thread_grid((int64_t)n_slots), 256, 0, s, slots.as<uint32_t>(), n_slots, v, row_hash.as<uint64_t>(), (uint32_t)count, d_n_new, new_src.as<uint32_t>(),
+              new_len.as<uint32_t>(), a_hash.as<uint64_t>());
     count_launch(2);
     TQ_TRY(check_launch("k_sd_assign"));
     unsigned n_new = 0;
@@ -253,8 +253,8 @@ int32_t StringDict::encode(const StrView &v, const uint32_t *bm, int64_t n, int6
     TQ_CUDA(cudaStreamSynchronize(s));
     if (n_new) {
       TQ_TRY(exclusive_scan_u32(new_len.as<uint32_t>(), 1, new_off.as<uint32_t>(), 1, (int64_t)n_new, d_total, scan_scratch, s));
-      k_sd_copy<<<sd_warp_grid((int64_t)n_new), 256, 0, s>>>(v, new_src.as<uint32_t>(), new_off.as<uint32_t>(), n_new, used_bytes, (uint32_t)count, d_total,
-                                                              arena.offsets.as<int64_t>(), arena.bytes.as<uint8_t>());
+      TQ_LAUNCH(k_sd_copy, sd_warp_grid((int64_t)n_new), 256, 0, s, v, new_src.as<uint32_t>(), new_off.as<uint32_t>(), n_new, used_bytes, (uint32_t)count, d_total,
+                arena.offsets.as<int64_t>(), arena.bytes.as<uint8_t>());
       count_launch();
       TQ_TRY(check_launch("k_sd_copy"));
       uint64_t total = 0;
@@ -266,8 +266,8 @@ int32_t StringDict::encode(const StrView &v, const uint32_t *bm, int64_t n, int6
       arena.n = (int64_t)count;
     }
   }
-  k_sd_lookup<<<sd_warp_grid((n + 31) >> 5), 256, 0, s>>>(v, bm, n, row_hash.as<uint64_t>(), slots.as<uint32_t>(), n_slots - 1, arena.offsets.as<int64_t>(),
-                                                          a_hash.as<uint64_t>(), arena.bytes.as<uint8_t>(), ids_out, valid_out);
+  TQ_LAUNCH(k_sd_lookup, sd_warp_grid((n + 31) >> 5), 256, 0, s, v, bm, n, row_hash.as<uint64_t>(), slots.as<uint32_t>(), n_slots - 1, arena.offsets.as<int64_t>(),
+            a_hash.as<uint64_t>(), arena.bytes.as<uint8_t>(), ids_out, valid_out);
   count_launch();
   return check_launch("k_sd_lookup");
 }
