@@ -1,7 +1,7 @@
 // emu_runtime.cpp — the host pieces the emulated sources link against (TEST INFRASTRUCTURE, see include/cuda_runtime.h):
 // the block / warp scheduler, "device" memory = malloc, and plain serial versions of the library helpers that live in
-// runtime.cu / varlen.cu of the product (exclusive scan, cell gather, bitmap copies) — those are exercised on the GPU by the
-// existing parity tests; here they only have to be correct.
+// runtime.cu / varlen.cu of the product (cell gather, bitmap copies) — those are exercised on the GPU by the existing parity
+// tests; here they only have to be correct.  The exclusive scan is not stood in for: scan.cu is compiled in.
 #include <cstdarg>
 #include <cstdio>
 
@@ -140,13 +140,6 @@ void host_bitmap_extract(uint8_t *dst, const uint8_t *src, int64_t src_off, int6
     const int64_t o = src_off + i;
     if ((src[o >> 3] >> (o & 7)) & 1) dst[i >> 3] |= (uint8_t)(1u << (i & 7));
   }
-}
-
-int32_t exclusive_scan_u32(const uint32_t *d_in, int in_stride, uint32_t *d_out, int out_stride, int64_t n, uint64_t *d_total, DevBuf &, cudaStream_t) {
-  uint64_t run = 0;
-  for (int64_t i = 0; i < n; i++) { const uint32_t v = d_in[i * in_stride]; d_out[i * out_stride] = (uint32_t)run; run += v; }
-  if (d_total) *d_total = run;
-  return TQ_OK;
 }
 
 int32_t upload_store(const HostVarAccum &h, SideStore &st, cudaStream_t) {

@@ -93,6 +93,20 @@ static inline T __shfl_sync(unsigned, T v, int src_lane) {
   memcpy(&r, &got, sizeof(T));
   return r;
 }
+template <typename T>
+static inline T __shfl_up_sync(unsigned, T v, unsigned delta) {
+  static_assert(sizeof(T) <= 8, "shuffle of at most 8 bytes");
+  const int w = tq_emu::cur >> 5, lane = tq_emu::cur & 31;
+  uint64_t bits = 0;
+  memcpy(&bits, &v, sizeof(T));
+  tq_emu::warp_slot[w][lane] = bits;
+  tq_emu::warp_sync();
+  const uint64_t got = tq_emu::warp_slot[w][lane >= (int)delta ? lane - (int)delta : lane];   // lanes below delta keep their own value
+  tq_emu::warp_sync();
+  T r;
+  memcpy(&r, &got, sizeof(T));
+  return r;
+}
 static inline unsigned __ballot_sync(unsigned, bool pred) {
   const int w = tq_emu::cur >> 5, lane = tq_emu::cur & 31;
   tq_emu::warp_slot[w][lane] = pred ? 1 : 0;

@@ -109,7 +109,8 @@ struct DColMut {
   uint32_t *bm = nullptr;
 };
 
-// device-wide exclusive scan of u32 counts (in place ok); total written to *d_total (u64) if non-null.
+// device-wide exclusive scan of u32 counts (in place ok; scan.cu); the exact 64-bit total is written to *d_total if non-null.
+// The offsets are 32-bit and exact only while the total is below 2^32: a caller checks *d_total or bounds it by construction.
 int32_t exclusive_scan_u32(const uint32_t *d_in, int in_stride_words, uint32_t *d_out, int out_stride_words,
                            int64_t n, uint64_t *d_total, DevBuf &scratch, cudaStream_t s);
 
