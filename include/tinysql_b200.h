@@ -396,6 +396,12 @@ int32_t tq_join_next_device(tq_join *j, tq_column *out_cols, int64_t *n_rows, in
  * Key-less handles: [0] build rows stored, [1] = [2] = 0, [4] rows of the result batches built so far, [5] device time of
  * the last result batch's kernels.  */
 int32_t tq_join_stats(tq_join *j, int64_t *stats8);
+/* Which build made the handle's hash table (after tq_join_finalize_build): the general build, or the streaming build of a
+ * large unique NOT NULL build side with each sub-table built in one thread-block cluster's or in one CTA's shared memory. */
+#define TQ_JOIN_BUILD_GENERAL 0
+#define TQ_JOIN_BUILD_CLUSTER 1
+#define TQ_JOIN_BUILD_CTA 2
+int32_t tq_join_build_path(tq_join *j, int32_t *path);
 
 /* ------------------------------------------------------------------ chunk wire codec
  * chunk.Codec.Encode / DecodeToChunk (util/chunk/codec.go:42-143) — the bytes child readers hand up.  Decoding fills

@@ -110,6 +110,7 @@ SYMBOLS = {
     "tq_join_next_device": (_I32, [_P, _COL, C.POINTER(_I64), C.POINTER(_I32)]),
     "tq_join_next_bytes": (_I32, [_P, _I64, C.POINTER(_I64)]),
     "tq_join_stats": (_I32, [_P, C.POINTER(_I64)]), "tq_join_destroy": (_I32, [_P]),
+    "tq_join_build_path": (_I32, [_P, C.POINTER(_I32)]),
     "tq_chunk_decode_device": (_I32, [_P, _I64, _I32, C.POINTER(_I32), C.POINTER(_P), _COL, C.POINTER(_I64)]),
     "tq_chunk_device_free": (_I32, [_P]),
     "tq_vec_filter_string": (_I32, [_I64, _COL, _P, _I32]),
@@ -161,6 +162,7 @@ TQ_TYPE_INT64, TQ_TYPE_UINT64, TQ_TYPE_FLOAT64, TQ_TYPE_FLOAT32, TQ_TYPE_BYTES =
 TQ_TYPE_NOT_NULL = 0x100
 TQ_MEM_HOST, TQ_MEM_DEVICE = 0, 1
 TQ_JOIN_STABLE_INPUT = 1
+TQ_JOIN_BUILD_GENERAL, TQ_JOIN_BUILD_CLUSTER, TQ_JOIN_BUILD_CTA = 0, 1, 2
 
 _lib = None
 

@@ -11,7 +11,8 @@
 //       row-major in key order; duplicates keep build insertion order (rowHashMap.Get, hash_table.go:259-272).
 //       Build: insert+count, exclusive scan, fill, sort duplicate segments, gather rows.
 //   Large NOT NULL build sides that fit an entry first try the streaming build (try_stream_build, gated by stream_build_ok):
-//       k_scatter_aos into one AoS slab per sub-table, then k_build_cluster builds each sub-table in cluster shared memory.
+//       k_scatter_aos into AoS slabs, then k_build_cta builds each sub-table in one CTA's shared memory (k_build_cluster, in
+//       cluster shared memory, where no sub-table size that one CTA holds stays within PART_MAX_BITS).
 // Probe.  Small build (one table): k_probe, ordered output (probe row asc, build insertion asc) via
 //   ticketed tiles + decoupled look-back.
 //   Large build, PK-FK shape (stream_probe_ok, no probe NULL bitmap): the streaming positional path of join_stream.cuh
@@ -1583,6 +1584,7 @@ struct tq_join {
   int64_t n_valid = 0, n_distinct = 0;
   bool build_unique = true;
   int64_t build_ns = 0;
+  int32_t build_path = TQ_JOIN_BUILD_GENERAL;
   int64_t part_rows = PART_TARGET_ROWS;   // build rows per partition table (TQ_JOIN_PART_ROWS at tq_join_create, tests)
 
   // ---- probe side
@@ -1708,9 +1710,10 @@ static bool stream_probe_ok(const tq_join *j) {
          j->n_probe_cols <= 4 && j->n_build_cols <= 4 && !j->has_oc && !g_no_fast_kernel;
 }
 
-// Partition-local build (join_stream.cuh): scatter the build rows into one AoS slab per sub-table, then one thread-block
-// cluster per slab builds its sub-table in distributed shared memory (k_build_cluster).  The table has 2^(pbits + sbits)
-// sub-tables; the probe side keeps the 2^pbits coarse partitions.  Covers the PK-FK shape — NOT NULL build columns that fit
+// Partition-local build (join_stream.cuh): scatter the build rows into AoS slabs, then build every sub-table in shared
+// memory: one CTA per sub-table where a sub-table fits one CTA (k_build_cta), else one thread-block cluster per slab, in
+// distributed shared memory (k_build_cluster).  The table has 2^(pbits + sbits) sub-tables; the probe side keeps the 2^pbits
+// coarse partitions.  Covers the PK-FK shape — NOT NULL build columns that fit
 // a table entry, unique keys; anything else (*done == false) takes the general build below.
 static int32_t try_stream_build(tq_join *j, bool *done) {
   *done = false;
@@ -1724,41 +1727,62 @@ static int32_t try_stream_build(tq_join *j, bool *done) {
   const int P = 1 << pbits;
   // Table capacity from the row count alone (no host round trip for the partition histogram): hash partitions of m rows hold
   // m +- a few sqrt(m); a sub-table that turns out fuller than the load limit allows is flagged by the build kernel and the
-  // general path takes over.  sbits: the fewest sub-tables per partition for which one fits the shared memory of a cluster.
-  // cap is that estimate at the load limit, rounded up to 16 entries so that every CTA's slice holds whole 32-byte sectors.
+  // general path takes over.  cap is that estimate at the load limit, rounded up to 16 entries so that every CTA's slice of a
+  // cluster-built sub-table holds whole 32-byte sectors.  sbits: the fewest sub-tables per partition for which one fits the
+  // shared memory of ONE CTA (k_build_cta) — or, where no such sbits stays within PART_MAX_BITS (the general probe path
+  // scatters into one bin per sub-table), of a cluster (k_build_cluster).
   const int shift = NB > 2 ? 2 : 1;
+  auto cap_of = [&](int sb) {
+    const double mean = (double)n / (double)((uint64_t)P << sb);
+    const uint64_t est_max = (uint64_t)(mean + 8.0 * sqrt(mean) + 64.0);
+    return (est_max * 100 / (uint64_t)g_max_load_pct + 15) & ~15ull;
+  };
   int sbits = 0;
   uint64_t cap = 0;
-  for (;; sbits++) {
-    if (pbits + sbits > PART_MAX_BITS) return TQ_OK;  // (the general probe path scatters into one bin per sub-table)
-    const double mean = (double)n / (double)((uint64_t)P << sbits);
-    const uint64_t est_max = (uint64_t)(mean + 8.0 * sqrt(mean) + 64.0);
-    cap = (est_max * 100 / (uint64_t)g_max_load_pct + 15) & ~15ull;
-    if (((cap << shift) * 8) / BC_CLUSTER <= (uint64_t)BC_MAX_SLICE_BYTES) break;
+  bool cta = false;
+  for (sbits = 0; pbits + sbits <= PART_MAX_BITS; sbits++) {
+    cap = cap_of(sbits);
+    if (((cap << shift) * 8) <= (uint64_t)BT_MAX_BYTES) { cta = true; break; }
+  }
+  if (!cta) {
+    for (sbits = 0;; sbits++) {
+      if (pbits + sbits > PART_MAX_BITS) return TQ_OK;
+      cap = cap_of(sbits);
+      if (((cap << shift) * 8) / BC_CLUSTER <= (uint64_t)BC_MAX_SLICE_BYTES) break;
+    }
   }
   const uint64_t n_slots = ((uint64_t)P << sbits) * cap;
   if (n_slots > (uint64_t)n * 12 + 4096 || n_slots > 0xFFFFFFF0ull) return TQ_OK;
   // The build rows are scattered straight into one slab per sub-table when the scatter has that many bins; beyond
-  // SA_MAX_PBITS bits each slab holds 2^(pbits + sbits - bbits) sub-tables, which its cluster builds one after another.
+  // SA_MAX_PBITS bits each slab holds 2^(pbits + sbits - bbits) sub-tables: one CTA each reads the slab (k_build_cta), or
+  // the slab's cluster builds them one after another (k_build_cluster).
   const int tbits = pbits + sbits;
   const int bbits = tbits < SA_MAX_PBITS ? tbits : SA_MAX_PBITS;
   const int n_bins = 1 << bbits;
   const uint64_t bin_slab = slab_rows(n, n_bins, true);
   if (bin_slab * n_bins > 0xFFFFFFF0ull) return TQ_OK;
-  const BuildClusterKernel kb = build_cluster_kernel(NB);
-  const int slice_bytes = (int)(((cap << shift) * 8) / BC_CLUSTER);
+  const int table_bytes = (int)((cap << shift) * 8);  // one sub-table
   cudaLaunchConfig_t cfg{};
   cudaLaunchAttribute cl[1];
-  cl[0].id = cudaLaunchAttributeClusterDimension;
-  cl[0].val.clusterDim.x = BC_CLUSTER;
-  cl[0].val.clusterDim.y = 1;
-  cl[0].val.clusterDim.z = 1;
-  cfg.gridDim = dim3((unsigned)(n_bins * BC_CLUSTER));
-  cfg.blockDim = dim3(BC_THREADS);
+  cfg.blockDim = dim3(cta ? BT_THREADS : BC_THREADS);
   cfg.stream = s;
-  cfg.attrs = cl;
-  cfg.numAttrs = 1;
-  {
+  const BuildKernel kb = cta ? build_cta_kernel(NB) : build_cluster_kernel(NB);
+  if (cta) {
+    static bool smem_set[5] = {false, false, false, false, false};
+    if (!smem_set[NB]) {
+      TQ_CUDA(cudaFuncSetAttribute(kb, cudaFuncAttributeMaxDynamicSharedMemorySize, BT_MAX_BYTES));
+      smem_set[NB] = true;
+    }
+    cfg.gridDim = dim3(1u << tbits);  // one CTA per sub-table, those of one slab adjacent
+    cfg.dynamicSmemBytes = (size_t)table_bytes;
+  } else {
+    cl[0].id = cudaLaunchAttributeClusterDimension;
+    cl[0].val.clusterDim.x = BC_CLUSTER;
+    cl[0].val.clusterDim.y = 1;
+    cl[0].val.clusterDim.z = 1;
+    cfg.gridDim = dim3((unsigned)(n_bins * BC_CLUSTER));
+    cfg.attrs = cl;
+    cfg.numAttrs = 1;
     // once per kernel: the largest slice must fit, and the device must be able to run such a cluster at all
     static int cluster_ok[5] = {-1, -1, -1, -1, -1};
     if (cluster_ok[NB] < 0) {
@@ -1769,8 +1793,8 @@ static int32_t try_stream_build(tq_join *j, bool *done) {
       cluster_ok[NB] = n_clusters > 0 ? 1 : 0;
     }
     if (!cluster_ok[NB]) return TQ_OK;
+    cfg.dynamicSmemBytes = (size_t)(table_bytes / BC_CLUSTER);
   }
-  cfg.dynamicSmemBytes = (size_t)slice_bytes;
   DevBuf &off = j->part_off[0], &hi = j->part_cursor[0], &lim = j->part_lim[0];
   unsigned long long *cur = j->cursors.as<unsigned long long>();
   TQ_CUDA(cudaMemsetAsync(cur, 0, 64, s));
@@ -1785,7 +1809,7 @@ static int32_t try_stream_build(tq_join *j, bool *done) {
   TQ_TRY(scatter_aos(q, j->b_aos, off, hi, lim, s));
   TQ_TRY(j->slots.reserve(((n_slots + 1) << shift) * 8));  // (+ the side entry of the empty-marker key, unused on this path)
   uint64_t *words = j->slots.as<uint64_t>();
-  BuildClusterParams bp{};
+  BuildParams bp{};
   bp.slab = j->b_aos.as<uint64_t>();
   bp.lo = off.as<uint32_t>();
   bp.hi = hi.as<uint32_t>();
@@ -1804,19 +1828,18 @@ static int32_t try_stream_build(tq_join *j, bool *done) {
     }
     j->row_mask_word = -1;
   }
+  bp.rows = cur;
   bp.flags = reinterpret_cast<unsigned *>(cur + 3);
   TQ_CUDA(cudaLaunchKernelEx(&cfg, kb, bp));
   count_launch();
-  TQ_TRY(check_launch("k_build_cluster"));
-  std::vector<uint32_t> h_hi((size_t)n_bins);
-  unsigned long long h_cur[4] = {0, 0, 0, 0};
-  TQ_CUDA(cudaMemcpyAsync(h_hi.data(), hi.p, (size_t)n_bins * 4, cudaMemcpyDeviceToHost, s));
-  TQ_CUDA(cudaMemcpyAsync(h_cur, cur, 32, cudaMemcpyDeviceToHost, s));
+  TQ_TRY(check_launch(cta ? "k_build_cta" : "k_build_cluster"));
+  // {rows inserted, -, slab overflow, flags}: one copy into pinned memory
+  const unsigned long long *h_cur = j->cursors_host.as<unsigned long long>();
+  TQ_CUDA(cudaMemcpyAsync(j->cursors_host.p, cur, 32, cudaMemcpyDeviceToHost, s));
   TQ_CUDA(cudaStreamSynchronize(s));
   if (h_cur[2]) return TQ_OK;  // a slab overflowed: skewed hash partitions
   if (h_cur[3]) return TQ_OK;  // duplicate keys, the empty-marker key, or a partition over the load limit: the general build handles them
-  uint64_t n_valid = 0;
-  for (int q2 = 0; q2 < n_bins; q2++) n_valid += h_hi[q2] - (uint64_t)q2 * bin_slab;
+  const uint64_t n_valid = h_cur[0];
   j->shift = shift;
   j->pbits = pbits;
   j->n_slots = n_slots;
@@ -1831,6 +1854,7 @@ static int32_t try_stream_build(tq_join *j, bool *done) {
   j->table.row_mode = 1;
   j->table.sent_off = (uint32_t)n_slots;
   j->table.sent_cnt = 0;
+  j->build_path = cta ? TQ_JOIN_BUILD_CTA : TQ_JOIN_BUILD_CLUSTER;
   *done = true;
   return TQ_OK;
 }
@@ -1845,6 +1869,7 @@ static int32_t join_build(tq_join *j) {
   uint32_t *counters = j->counters.as<uint32_t>();
   TQ_CUDA(cudaMemsetAsync(counters, 0, 64, s));
   j->build_has_nulls = false;
+  j->build_path = TQ_JOIN_BUILD_GENERAL;
   for (int c = 0; c < j->n_build_cols; c++) j->build_has_nulls |= (j->b_view[c].bm != nullptr);
   if (stream_build_ok(j)) {
     bool done = false;
@@ -3584,6 +3609,12 @@ int32_t tq_join_stats(tq_join *j, int64_t *s) {
   s[5] = j->last_probe_ns;
   s[6] = j->build_ns;
   s[7] = j->probe_launches;
+  return TQ_OK;
+}
+
+int32_t tq_join_build_path(tq_join *j, int32_t *path) {
+  if (!j || !path) return TQ_ERR_INVALID_ARG;
+  *path = j->build_path;
   return TQ_OK;
 }
 
