@@ -16,8 +16,8 @@
 // Probe.  Small build (one table): k_probe, ordered output (probe row asc, build insertion asc) via
 //   ticketed tiles + decoupled look-back.
 //   Large build, PK-FK shape (stream_probe_ok, no probe NULL bitmap): the streaming positional path of join_stream.cuh
-//   (launch_probe_stream): k_pos_count -> k_pos_bases -> k_scatter_cols (the probe columns straight into their result slots)
-//   -> k_probe_pos (key column in, build columns out) -> hole filling; the result is a multiset.
+//   (launch_probe_stream): k_pos_reset -> k_scatter_cols (the probe columns straight into result pages claimed on the fly)
+//   -> k_pos_pages -> k_probe_pos (key column in, build columns out) -> hole filling; the result is a multiset.
 //   Any other large build: k_probe_part_hist (only after a slab overflow) -> scan -> k_probe_scatter(_fast) (shared-memory
 //   counting sort of 4096-row tiles, coalesced full-sector stores) -> k_probe_part_fast / k_probe_part(_uniq).
 #include <chrono>
@@ -1600,7 +1600,9 @@ struct tq_join {
   DevBuf part_cnt[2], part_off[2], part_cursor[2], part_lim[2];
   bool optimistic_scatter = true;         // general partitioned path: skip the histogram pass, fixed slabs with 25% slack (falls back on overflow)
   // streaming PK-FK pipeline (join_stream.cuh): exact partition counts, positional output, hole filling
-  DevBuf pos_meta[2], pos_valid[2], hole_pos[2], hole_src[2], hole_scan;
+  DevBuf pos_meta[2], pos_pt[2], pos_valid[2], hole_runs[2], hole_scan;
+  uint32_t pos_epoch[2] = {0, 0};          // page-table epoch of the last positional batch in each cursor slot
+  size_t pos_pt_cleared[2] = {0, 0};       // bytes of pos_pt cleared since it was allocated
   DevBuf b_aos;                           // build-side AoS slabs (released after the build)
   // segmented probe batch (tq_join_put_probe_segments): consumed by the next launch_probe_stream
   SegSpec seg;
@@ -2049,82 +2051,142 @@ static std::unique_ptr<ResultBatch> get_result_batch(tq_join *j) {
 }
 
 // Hole filling, fast path: when every probe row of the batch found its match (the foreign-key join) the only holes of the
-// positional result are the pads that round each partition up to 32 slots, and both lists — the pad slots below M and the real
-// rows at or above M — follow from the partition counts and bases alone: one small kernel instead of passes over the validity
-// bitmap.  A batch with misses (M != rows scattered) is completed by fill_holes_host once the counts are on the host.
+// positional result are the unfilled tails of the partitions' last pages, and both lists — the hole slots below M and the real
+// rows at or above M — are a few runs of slots that follow from the final cursors and the page table alone: one run of holes
+// per partition, and one run of real rows per page at or above M (at most P such pages, since the P last pages leave less
+// than P pages unfilled).  k_hole_pages writes the runs with their prefix offsets; k_hole_move_pages finds the k-th hole and
+// the k-th tail row by binary search over them.  A batch with misses (M != rows scattered) is completed by fill_holes_host
+// once the counts are on the host.
 static constexpr int HOLE_PAD_THREADS = 512;   // >= partitions of the streaming path (SA_MAX_PBITS)
-__global__ void __launch_bounds__(HOLE_PAD_THREADS) k_hole_pads(const uint32_t *part_cnt, const uint32_t *out_base, int n_parts, unsigned long long *cur,
-                                                                 uint32_t *hole_pos, uint32_t *tail_src) {
+struct HoleRuns {
+  uint32_t *h_start, *h_off;   // [n_parts], [n_parts + 1]: partition q's holes below M start at h_start[q], the h_off[q]-th hole
+  uint32_t *t_start, *t_off;   // [n_parts], [n_parts + 1]: the i-th page at or above M: its real rows there, likewise
+};
+__global__ void __launch_bounds__(HOLE_PAD_THREADS) k_hole_pages(const PosPages m, int n_parts, unsigned long long *cur, const HoleRuns h) {
   __shared__ uint32_t s_warp[33];
+  __shared__ uint32_t s_fill[HOLE_PAD_THREADS];
   const int q = threadIdx.x;
-  const uint64_t M = cur[0];
-  uint32_t cnt = 0, base = 0, h = 0, t = 0;
-  if (q < n_parts) {
-    cnt = part_cnt[q];
-    base = out_base[q];
-    const uint64_t pad_lo = (uint64_t)base + cnt, pad_hi = out_base[q + 1];        // pad slots of this partition
-    const uint64_t hole_hi = pad_hi < M ? pad_hi : M;
-    h = hole_hi > pad_lo ? (uint32_t)(hole_hi - pad_lo) : 0u;                      // ... that lie below M
-    const uint64_t real_lo = (uint64_t)base > M ? (uint64_t)base : M;
-    t = pad_lo > real_lo ? (uint32_t)(pad_lo - real_lo) : 0u;                      // real rows of this partition at or above M
+  const uint64_t M = cur[0], PG = m.page_rows;
+  uint32_t c = 0, n_h = 0;
+  uint64_t last = 0, fill = 0, h_lo = 0;
+  if (q < n_parts) c = m.cursor[q];
+  if (c) {
+    const uint32_t k = (c - 1) / (uint32_t)PG;
+    last = (uint32_t)m.pt[(uint64_t)q * m.kmax + k];   // the partition's last page, filled up to `fill`
+    fill = c - (uint64_t)k * PG;
+    h_lo = last * PG + fill;
+    const uint64_t h_hi = (last + 1) * PG < M ? (last + 1) * PG : M;
+    n_h = h_hi > h_lo ? (uint32_t)(h_hi - h_lo) : 0u;
   }
-  uint32_t rows, n_holes, n_tail;
-  block_excl_scan(cnt, s_warp, &rows);
-  const uint32_t h_off = block_excl_scan(h, s_warp, &n_holes);
-  const uint32_t t_off = block_excl_scan(t, s_warp, &n_tail);
+  uint32_t rows, n_holes;
+  block_excl_scan(c, s_warp, &rows);
+  const uint32_t h_off = block_excl_scan(n_h, s_warp, &n_holes);
   if (q == 0) {
     cur[6] = rows;                    // rows the scatter placed: == M iff no probe row missed
-    cur[5] = n_holes;                 // holes to fill (== n_tail when nothing missed)
+    cur[5] = n_holes;                 // holes to fill
   }
   if ((uint64_t)rows != M) return;    // misses among the probe rows: fill_holes_host builds exact lists (CTA-uniform exit)
   if (q < n_parts) {
-    const uint64_t pad_lo = (uint64_t)base + cnt;
-    for (uint32_t i = 0; i < h; i++) hole_pos[h_off + i] = (uint32_t)(pad_lo + i);   // at most 31 per partition
+    h.h_start[q] = (uint32_t)h_lo;
+    h.h_off[q] = h_off;
   }
-  // the real rows at or above M sit in the last partition(s), up to 31 * P of them in one partition: written by the whole CTA
-  __shared__ uint32_t s_t[HOLE_PAD_THREADS], s_toff[HOLE_PAD_THREADS], s_lo[HOLE_PAD_THREADS];
-  s_t[q] = t;
-  s_toff[q] = t_off;
-  s_lo[q] = (uint32_t)((uint64_t)base > M ? (uint64_t)base : M);
+  // pages first .. n_pages - 1 hold the real rows at or above M: every one full but the partitions' last pages
+  const uint64_t first = M / PG, n_tail = m.cursor[n_parts] - first;
+  s_fill[q] = (uint32_t)PG;
   __syncthreads();
-  for (int pq = 0; pq < n_parts; pq++) {
-    const uint32_t tq = s_t[pq];
-    for (uint32_t i = q; i < tq; i += HOLE_PAD_THREADS) tail_src[s_toff[pq] + i] = s_lo[pq] + i;
+  if (c && last >= first) s_fill[last - first] = (uint32_t)fill;
+  __syncthreads();
+  uint32_t n_t = 0;
+  uint64_t t_lo = 0;
+  if ((uint64_t)q < n_tail) {
+    const uint64_t pb = (first + q) * PG;
+    t_lo = pb > M ? pb : M;
+    n_t = pb + s_fill[q] > t_lo ? (uint32_t)(pb + s_fill[q] - t_lo) : 0u;
+  }
+  uint32_t n_tail_rows;
+  const uint32_t t_off = block_excl_scan(n_t, s_warp, &n_tail_rows);   // == n_holes
+  if (q < n_parts) {
+    h.t_start[q] = (uint32_t)t_lo;
+    h.t_off[q] = (uint64_t)q < n_tail ? t_off : n_tail_rows;   // (past the tail pages: no row, never found)
+  }
+  if (q == 0) {
+    h.h_off[n_parts] = n_holes;
+    h.t_off[n_parts] = n_tail_rows;
   }
 }
 struct HoleMoveDevParams {
-  int n_cols;
+  int n_cols, n_parts;
   uint64_t *col[8];
-  const uint32_t *hole_pos, *tail_src;
+  HoleRuns runs;
   const unsigned long long *cur;
 };
-__global__ void __launch_bounds__(256) k_hole_move_pads(const HoleMoveDevParams h) {
+// the last index i < n with off[i] <= k (off ascending, off[0] = 0)
+__device__ __forceinline__ int run_of(const uint32_t *off, int n, uint32_t k) {
+  int lo = 0, hi = n;
+  while (hi - lo > 1) {
+    const int mid = (lo + hi) >> 1;
+    if (off[mid] <= k) lo = mid;
+    else hi = mid;
+  }
+  return lo;
+}
+__global__ void __launch_bounds__(256) k_hole_move_pages(const HoleMoveDevParams h) {
+  __shared__ uint32_t s_hs[HOLE_PAD_THREADS], s_ho[HOLE_PAD_THREADS], s_ts[HOLE_PAD_THREADS], s_to[HOLE_PAD_THREADS];
   if (h.cur[6] != h.cur[0]) return;  // misses: the host-sized pass does the whole job
   const uint64_t H = h.cur[5];
+  if ((uint64_t)blockIdx.x * blockDim.x >= H) return;
+  for (int i = threadIdx.x; i < h.n_parts; i += blockDim.x) {
+    s_hs[i] = h.runs.h_start[i];
+    s_ho[i] = h.runs.h_off[i];
+    s_ts[i] = h.runs.t_start[i];
+    s_to[i] = h.runs.t_off[i];
+  }
+  __syncthreads();
   const uint64_t stride = (uint64_t)gridDim.x * blockDim.x;
   for (uint64_t k = (uint64_t)blockIdx.x * blockDim.x + threadIdx.x; k < H; k += stride) {
-    const uint32_t d = h.hole_pos[k], sidx = h.tail_src[k];
-    for (int c = 0; c < h.n_cols; c++) h.col[c][d] = h.col[c][sidx];
+    const int a = run_of(s_ho, h.n_parts, (uint32_t)k), b = run_of(s_to, h.n_parts, (uint32_t)k);
+    const uint32_t d = s_hs[a] + ((uint32_t)k - s_ho[a]), sidx = s_ts[b] + ((uint32_t)k - s_to[b]);
+#pragma unroll
+    for (int c = 0; c < 8; c++)
+      if (c < h.n_cols) h.col[c][d] = h.col[c][sidx];
   }
 }
 
-// exact partition counts -> bases -> column-wise scatter into the result -> key-only positional probe -> device-driven hole
-// filling.  Nothing is read back to the host.
+// column-wise scatter into result pages claimed on the fly -> key-only positional probe -> device-driven hole filling.
+// Nothing is read back to the host.
 static int32_t launch_probe_stream(tq_join *j, const ProbeParams &p, const std::vector<DCol> &probe, const uint8_t *d_selected, int64_t n,
                                    unsigned long long *cur, int slot, uint64_t alloc_rows) {
   cudaStream_t s = rt().compute;
   const int P = 1 << j->pbits, NP = j->n_probe_cols, NB = j->n_build_cols;
-  if (n + 32ll * P > 0xFFFFFFF0ll) { set_error("probe batch too large for 32-bit result slots; feed smaller batches"); return TQ_ERR_INVALID_ARG; }
-  TQ_TRY(j->pos_meta[slot].reserve((size_t)4 * (P + 1) * 4));
-  PosMeta m;
-  m.cnt = j->pos_meta[slot].as<uint32_t>();
-  m.base = m.cnt + (P + 1);
-  m.cursor = m.base + (P + 1);
+  const uint32_t page = pos_page_rows(n, P, NP);
+  if (n + (int64_t)P * page > 0xFFFFFFF0ll) { set_error("probe batch too large for 32-bit result slots; feed smaller batches"); return TQ_ERR_INVALID_ARG; }
+  TQ_TRY(j->pos_meta[slot].reserve((size_t)2 * (P + 1) * 4));
+  PosPages m;
+  m.cursor = j->pos_meta[slot].as<uint32_t>();
   m.chunk = m.cursor + (P + 1);
+  m.page_rows = page;
+  m.kmax = (uint32_t)(n / page + 1);   // virtual pages of one partition holding the whole batch
+  // The page table is cleared only when a batch needs more of it than was cleared before (the first batch of a handle) and
+  // when the epoch wraps; otherwise a batch writes only the entries it uses, and older entries carry an older epoch.
+  const size_t pt_bytes = (size_t)P * m.kmax * 8;
+  uint32_t &epoch = j->pos_epoch[slot];
+  if (j->pos_pt_cleared[slot] < pt_bytes || epoch == 0xFFFFFFFFu) {
+    TQ_TRY(j->pos_pt[slot].reserve(pt_bytes));
+    TQ_CUDA(cudaMemsetAsync(j->pos_pt[slot].p, 0, pt_bytes, s));   // (not the whole block: a cached one may be far larger)
+    j->pos_pt_cleared[slot] = pt_bytes;
+    epoch = 0;
+  }
+  m.epoch = ++epoch;
+  m.pt = j->pos_pt[slot].as<unsigned long long>();
+  m.err = cur + 4;
   const int64_t n_words_max = (int64_t)(alloc_rows >> 5) + 1;
   TQ_TRY(j->pos_valid[slot].reserve((size_t)(n_words_max + 2) * 4));
-  TQ_TRY(j->hole_pos[slot].reserve((size_t)(32 * (P + 2)) * 4));   // at most 31 pad slots per partition
-  TQ_TRY(j->hole_src[slot].reserve((size_t)(32 * (P + 2)) * 4));
+  TQ_TRY(j->hole_runs[slot].reserve((size_t)4 * (P + 1) * 4));
+  HoleRuns hr;
+  hr.h_start = j->hole_runs[slot].as<uint32_t>();
+  hr.h_off = hr.h_start + (P + 1);
+  hr.t_start = hr.h_off + (P + 1);
+  hr.t_off = hr.t_start + (P + 1);
   const ProbePosVariant pv = probe_pos_kernel(NB);
   if (!pv.k || NP < 1 || NP > 4) { set_error("internal: positional probe of %d x %d columns", NP, NB); return TQ_ERR_INVALID_ARG; }
   ScatterAosParams q{};
@@ -2147,12 +2209,14 @@ static int32_t launch_probe_stream(tq_join *j, const ProbeParams &p, const std::
   q.sp.key_mode = j->key_mode;
   q.sp.pbits = j->pbits;
   q.sp.n = n;
-  TQ_TRY(launch_pos_scatter(q, seg_rows, m, pv.tile, cur + 3, s));
+  TQ_TRY(launch_pos_scatter(q, seg_rows, m, cur + 3, s));
   ProbePosParams pp{};
   pp.keys = p.out_probe[j->probe_key].data;
-  pp.cnt = m.cnt;
-  pp.base = m.base;
+  pp.cnt = m.cursor;
   pp.chunk = m.chunk;
+  pp.pt = m.pt;
+  pp.page_rows = m.page_rows;
+  pp.kmax = m.kmax;
   pp.n_parts = P;
   for (int c = 0; c < NB; c++) { pp.out_build[c] = p.out_build[c].data; pp.build_word[c] = p.build_word[c]; }
   pp.valid = j->pos_valid[slot].as<uint32_t>();
@@ -2165,18 +2229,18 @@ static int32_t launch_probe_stream(tq_join *j, const ProbeParams &p, const std::
   pv.k<<<(unsigned)grid, pv.threads, smem, s>>>(pp, j->table);
   count_launch();
   TQ_TRY(check_launch("k_probe_pos"));
-  // holes: the padding of every partition to 32 slots (filled here) + probe rows without a match (finalize_pending)
-  k_hole_pads<<<1, HOLE_PAD_THREADS, 0, s>>>(m.cnt, m.base, P, cur, j->hole_pos[slot].as<uint32_t>(), j->hole_src[slot].as<uint32_t>());
+  // holes: the unfilled tails of the last pages (filled here) + probe rows without a match (finalize_pending)
+  k_hole_pages<<<1, HOLE_PAD_THREADS, 0, s>>>(m, P, cur, hr);
   HoleMoveDevParams hm{};
   hm.n_cols = NP + NB;
+  hm.n_parts = P;
   for (int c = 0; c < NP; c++) hm.col[c] = p.out_probe[c].data;
   for (int c = 0; c < NB; c++) hm.col[NP + c] = p.out_build[c].data;
-  hm.hole_pos = j->hole_pos[slot].as<uint32_t>();
-  hm.tail_src = j->hole_src[slot].as<uint32_t>();
+  hm.runs = hr;
   hm.cur = cur;
-  k_hole_move_pads<<<32, 256, 0, s>>>(hm);
+  k_hole_move_pages<<<rt().sm_count * 4, 256, 0, s>>>(hm);
   count_launch(2);
-  TQ_TRY(check_launch("k_hole_move_pads"));
+  TQ_TRY(check_launch("k_hole_move_pages"));
   j->probe_launches += 6;
   return TQ_OK;
 }
@@ -2238,7 +2302,7 @@ static int32_t launch_probe(tq_join *j, const std::vector<DCol> &probe, const ui
   p.def_mask = j->def_mask;
   p.n = n;
   p.capacity = capacity;
-  unsigned long long *cur = j->cursors.as<unsigned long long>() + 8 * cursor_slot;  // [0] rows, [1] matched probe rows, [2] slab overflow (general path), [3] span of the positional result, [5] pad holes, [6] rows the scatter placed
+  unsigned long long *cur = j->cursors.as<unsigned long long>() + 8 * cursor_slot;  // [0] rows, [1] matched probe rows, [2] slab overflow (general path), [3] span of the positional result, [4] a result page id never appeared, [5] page-tail holes, [6] rows the scatter placed
   p.cursor = cur;
   TQ_CUDA(cudaMemsetAsync(cur, 0, 64, s));
   {
@@ -2250,11 +2314,11 @@ static int32_t launch_probe(tq_join *j, const std::vector<DCol> &probe, const ui
     p.ticket = reinterpret_cast<unsigned *>(ts.as<unsigned long long>() + n_tiles);
   }
   // The streaming PK-FK pipeline (join_stream.cuh) when the operator allows it and this batch has no probe NULL bitmap.  Its
-  // result is positional: room for the padding of every partition to 32 rows.
+  // result is paged: room for the unfilled tail of every partition's last page.
   bool any_in_bm = false;
   for (int c = 0; c < j->n_probe_cols; c++) any_in_bm |= (probe[c].bm != nullptr);
   const bool pos_path = stream_probe_ok(j) && !any_in_bm;
-  const uint64_t alloc_rows = capacity + (pos_path ? 32ull * ((1ull << j->pbits) + 2) : 0);
+  const uint64_t alloc_rows = capacity + (pos_path ? (uint64_t)pos_page_rows(n, 1 << j->pbits, j->n_probe_cols) << j->pbits : 0);
   for (int c = 0; c < ncols; c++) {
     TQ_TRY(rb->cols[c].data.reserve((size_t)(alloc_rows ? alloc_rows : 1) * 8));
     TQ_TRY(rb->cols[c].bm.reserve(bitmap_alloc_bytes((int64_t)alloc_rows)));
@@ -2493,6 +2557,7 @@ static int32_t finalize_pending(tq_join *j) {
     TQ_CUDA(cudaStreamSynchronize(r.compute));
     produced = hc[0];
   }
+  if (hc[4]) { set_error("internal: a page of the positional result was never handed out"); return TQ_ERR_CUDA; }
   if (hc[3] && hc[6] != hc[0]) TQ_TRY(fill_holes_host(j, pb.rb.get(), pb.cursor_slot, hc[0], hc[3]));  // positional result with misses among the probe rows
   if (produced > pb.rb->capacity) {
     // duplicate build keys: the first launch served as the count pass; run again with the exact size

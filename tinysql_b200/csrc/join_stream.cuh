@@ -7,17 +7,19 @@
 //                       aggregation's pre-pass).  Input tiles arrive in shared memory by TMA bulk copies (cp.async.bulk +
 //                       mbarrier, SASS UBLKCP) one tile ahead; a row's rank inside its partition is the return value of one
 //                       shared-memory histogram atomic; rows leave through an AoS staging area as full-sector 16-byte stores.
-//   k_pos_count         the probe side's exact partition counts (key column only), then k_pos_bases: the partition bases of
-//                       the positional result (each partition padded to 32 slots), the scatter cursors and the probe's work list.
 //   k_scatter_cols<NC>  the probe side's scatter: k_scatter_aos's tiles and ranking, but every column is written straight into
-//                       its RESULT column, at the row's final slot (base of its partition + its place in the partition order).
+//                       its RESULT column.  The result is cut into pages of page_rows slots, each owned by one partition and
+//                       handed out while the scatter runs (a page table maps a partition's virtual pages to physical ones), so
+//                       no pass has to count the partitions first.  k_pos_reset clears the cursors before it, k_pos_pages
+//                       turns the final cursors into the span and the probe's work list after it.
 //   k_probe_pos<NB>     probe of one partition against its L2-resident table.  Tiles of the result's probe KEY column are
-//                       TMA-streamed through a ring of shared-memory stages by a producer warp; every consumer warp is
-//                       independent (no CTA barrier, no output cursor): the probe columns are already in place, so a warp's 32
-//                       rows write 32 consecutive slots of every BUILD column, and a ballot word records which slots are real.
-//                       The holes (misses, and the padding of each partition to a multiple of 32) are filled afterwards from
-//                       the tail of the result (k_hole_*): for a foreign-key join that is a few thousand rows.  The contract
-//                       is the result MULTISET (SURVEY Appendix B); order is not.
+//                       TMA-streamed through a ring of shared-memory stages by a producer warp that takes each tile's address
+//                       from the page table; every consumer warp is independent (no CTA barrier, no output cursor): the probe
+//                       columns are already in place, so a warp's 32 rows write 32 consecutive slots of every BUILD column,
+//                       and a ballot word records which slots are real.  The holes (misses, and the unfilled tail of each
+//                       partition's last page) are filled afterwards from the tail of the result (k_hole_*): for a
+//                       foreign-key join that is about P * page_rows / 2 rows.  The contract is the result MULTISET (SURVEY
+//                       Appendix B); order is not.
 //   k_build_cta<NB>     build of the partition tables from build-side AoS slabs: one CTA per sub-table builds it in its own
 //                       shared memory and writes it out once (the 2^lbits CTAs of a slab read it once from DRAM, then from L2).
 //   k_build_cluster<NB> the same for sub-tables too large for one CTA: one 8-CTA cluster per slab builds its sub-tables in
@@ -303,7 +305,6 @@ static int32_t launch_scatter_aos(const ScatterAosParams &q, int nc, cudaStream_
 }
 
 // ------------------------------------------------------------------------------------------------ positional probe
-// out_base[q] = first output slot of partition q (a multiple of 32), out_base[n_parts] = the span S of the result.
 // exclusive scan of one value per thread over a CTA of up to 1024 threads (s_warp: 33 words); returns the prefix, *total = the sum
 __device__ __forceinline__ uint32_t block_excl_scan(uint32_t v, uint32_t *s_warp, uint32_t *total) {
   const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5, n_warps = (blockDim.x + 31) >> 5;
@@ -327,12 +328,28 @@ __device__ __forceinline__ uint32_t block_excl_scan(uint32_t v, uint32_t *s_warp
   return res;
 }
 
-// Per-partition words of a positional batch, (n_parts + 1) of each.  cnt: rows of the partition (k_pos_count); base: its first
-// slot in the result, base[n_parts] = the span S (k_pos_bases); cursor: the scatter's claim cursor, from base[q] up to
-// base[q] + cnt[q]; chunk: the first probe CTA of the partition, chunk[n_parts] = the probe CTAs in all.
-struct PosMeta {
-  uint32_t *cnt, *base, *cursor, *chunk;
+// The paged result of a positional batch.  The result's slots are cut into pages of page_rows slots (whole probe tiles); a
+// page belongs to one partition.  Partition q's rows take VIRTUAL slots 0, 1, ... (cursor[q] counts them); its virtual page k
+// is physical page pt[q * kmax + k], and physical page i holds result slots [i * page_rows, (i + 1) * page_rows).
+//   cursor  [n_parts + 1]  rows of each partition so far; cursor[n_parts] = physical pages handed out
+//   chunk   [n_parts + 1]  first probe CTA of each partition (k_pos_pages); chunk[n_parts] = the probe CTAs in all
+//   pt      [n_parts * kmax]  page table: (epoch << 32) | physical page.  An entry with another epoch belongs to an earlier
+//                          batch, so the table is never cleared: each batch only writes the entries it uses.
+//   err     set when a page id did not appear in time (the batch fails with an internal error instead of hanging)
+struct PosPages {
+  uint32_t *cursor, *chunk;
+  unsigned long long *pt;
+  uint32_t page_rows, kmax, epoch;
+  unsigned long long *err;
 };
+__device__ __forceinline__ unsigned long long ld_relaxed_u64(const unsigned long long *p) {
+  unsigned long long v;
+  asm volatile("ld.relaxed.gpu.global.u64 %0, [%1];" : "=l"(v) : "l"(p));
+  return v;
+}
+__device__ __forceinline__ void st_relaxed_u64(unsigned long long *p, unsigned long long v) {
+  asm volatile("st.relaxed.gpu.global.u64 [%0], %1;" ::"l"(p), "l"(v) : "memory");
+}
 
 // Rows of tile `tile` of a batch (T rows per tile) and where its column c starts: one range (sp.in / sp.n), or the segmented
 // regions as k_scatter_aos reads them (region g = tiles [g * seg_tiles, (g + 1) * seg_tiles)).
@@ -363,93 +380,63 @@ __device__ __forceinline__ int stream_part(const ScatterParams &p, uint64_t key,
   return (int)part_of_hash(tqd::hash_key(key), p.pbits);
 }
 
-// ---- exact partition counts: reads the key column alone, in the scatter's tiles (so segmented regions read the same way).
-// One shared-memory histogram per warp keeps the atomics of different warps apart; the CTA adds its histograms into cnt once.
-static constexpr int PC_THREADS = 256;
-template <int T, bool PLAIN>
-__global__ void __launch_bounds__(PC_THREADS, 8) k_pos_count(const ScatterAosParams q, uint32_t *cnt) {
-  constexpr int R = T / PC_THREADS;  // rows per thread per tile
-  constexpr int W = PC_THREADS / 32;
-  extern __shared__ uint32_t s_cnt[];  // [W][n_parts]
-  const ScatterParams &p = q.sp;
-  const int n_parts = 1 << p.pbits;
-  const int tid = threadIdx.x;
-  for (int i = tid; i < W * n_parts; i += PC_THREADS) s_cnt[i] = 0;
-  __syncthreads();
-  uint32_t *h = s_cnt + (tid >> 5) * n_parts;
-  const int64_t n_tiles = q.n_segs ? (int64_t)q.n_segs * q.seg_tiles : (p.n + T - 1) / T;
-  for (int64_t tile = blockIdx.x; tile < n_tiles; tile += gridDim.x) {
-    const int rows = stream_tile_rows(q, T, tile);
-    const uint64_t *keys = stream_tile_col(q, T, tile, p.key_col);
-    uint64_t key[R];
-#pragma unroll
-    for (int k = 0; k < R; k++) {  // R independent loads in flight
-      const int row = k * PC_THREADS + tid;
-      key[k] = row < rows ? tqd::ld_stream_u64(keys + row) : 0;
-    }
-#pragma unroll
-    for (int k = 0; k < R; k++) {
-      const int row = k * PC_THREADS + tid;
-      if (row >= rows) continue;
-      const int b = stream_part<PLAIN>(p, key[k], tile * T + row);
-      if (b >= 0) atomicAdd(&h[b], 1u);
-    }
-  }
-  __syncthreads();
-  for (int b = tid; b < n_parts; b += PC_THREADS) {
-    uint32_t s = 0;
-#pragma unroll
-    for (int w = 0; w < W; w++) s += s_cnt[w * n_parts + b];
-    if (s) atomicAdd(&cnt[b], s);
-  }
+// ---- batch start (one CTA): every partition's cursor and the page counter back to zero.
+static constexpr int POS_BASES_THREADS = 512;   // >= partitions of the streaming path (SA_MAX_PBITS)
+__global__ void __launch_bounds__(POS_BASES_THREADS) k_pos_reset(uint32_t *cursor, int n) {
+  for (int i = threadIdx.x; i < n; i += POS_BASES_THREADS) cursor[i] = 0;
 }
 
-// ---- partition bases (one CTA): partition q's rows take slots [base[q], base[q] + cnt[q]) of the result and its run is
-// padded to a multiple of 32 slots, so a warp's 32 slots never straddle two partitions and every base is 256-byte aligned
-// in an 8-byte column (the probe's bulk copies start there).  Also the scatter cursors, the span S (*span) and the probe's
-// work list: ceil(cnt[q] / tile_rows) tiles per partition, PP_CHUNK_TILES tiles per CTA, consecutive CTAs on one partition.
-static constexpr int POS_BASES_THREADS = 512;   // >= partitions of the streaming path (SA_MAX_PBITS)
+// ---- after the scatter (one CTA): from the final cursors (rows per partition) the span S = pages * page_rows (*span) and the
+// probe's work list: ceil(cursor[q] / tile_rows) tiles per partition, PP_CHUNK_TILES tiles per CTA, consecutive CTAs on one
+// partition (so its table stays in L2 while they run).
 static constexpr int PP_CHUNK_TILES = 11;       // probe tiles per CTA (~8K rows): enough CTAs per partition that only a handful of partitions are live at once
-__global__ void __launch_bounds__(POS_BASES_THREADS) k_pos_bases(const PosMeta m, int n_parts, int tile_rows, unsigned long long *span) {
+__global__ void __launch_bounds__(POS_BASES_THREADS) k_pos_pages(const PosPages m, int n_parts, int tile_rows, unsigned long long *span) {
   __shared__ uint32_t s_warp[33];
   const int q = threadIdx.x;
-  const uint32_t c = q < n_parts ? m.cnt[q] : 0u;
-  uint32_t total, ctas;
-  const uint32_t base = block_excl_scan((c + 31u) & ~31u, s_warp, &total);
+  const uint32_t c = q < n_parts ? m.cursor[q] : 0u;
   const uint32_t tiles = (c + (uint32_t)tile_rows - 1) / (uint32_t)tile_rows;
+  uint32_t ctas;
   const uint32_t first = block_excl_scan((tiles + PP_CHUNK_TILES - 1) / PP_CHUNK_TILES, s_warp, &ctas);
-  if (q < n_parts) {
-    m.base[q] = base;
-    m.cursor[q] = base;
-    m.chunk[q] = first;
-  }
+  if (q < n_parts) m.chunk[q] = first;
   if (q == 0) {
-    m.base[n_parts] = total;
     m.chunk[n_parts] = ctas;
-    *span = total;
+    *span = (unsigned long long)m.cursor[n_parts] * m.page_rows;
   }
 }
 
-// ---- column-wise scatter into the result: k_scatter_aos's TMA-fed tiles and shared-memory ranking; a row's slot is the run
-// its tile claims on cursor[q] (which starts at base[q]) plus its rank.  The counts are exact, so nothing can overflow.  The
-// staging area is column-major, so each column leaves as runs of consecutive 8-byte stores (consecutive threads, consecutive
-// slots).  Same shared-memory image as k_scatter_aos (sa_smem_bytes; its slab-fit table is not needed here), hence the same
-// tile size and the same segmented-region geometry.
+// ---- column-wise scatter into the result: k_scatter_aos's TMA-fed tiles and shared-memory ranking; a row's virtual slot is
+// the run its tile claims on cursor[q] plus its rank.  Pages are handed out as the claims reach them: the claim whose run
+// contains the first slot of virtual page k allocates a physical page (one atomic on the page counter) and publishes its id in
+// pt.  A page is at least one tile, so a run crosses at most one page boundary: it lies in the page its first slot falls in
+// (allocated by this claim when the run starts it, else by an earlier claim) and, past the boundary, in the page it opens.
+// An earlier claim's page id is loaded right after the claim and only needed once the rows are placed; a thread makes all its
+// claims and allocations before it waits on any id, so every id it waits for belongs to a claim that has nothing left to
+// wait for (no deadlock), and the wait is bounded besides.  Rows are placed as (bin, rank) and mapped to physical slots in
+// the write-out loop through a per-bin record.  Every page is whole tiles of the probe, so nothing can overflow and a skewed
+// batch stays on this path.  The staging area is column-major, so each column leaves as runs of consecutive 8-byte stores
+// (consecutive threads, consecutive slots).  k_scatter_aos's shared-memory image plus one more per-bin table (sc_smem_bytes),
+// and the same segmented-region geometry.
+template <int T>
+__host__ __device__ constexpr int sc_smem_bytes(int nc, int bins) { return sa_smem_bytes<T>(nc, bins) + ((bins * 4 + 15) & ~15); }
+static constexpr uint32_t PAGE_WAIT_SPINS = 1u << 20;   // ~0.1 s of polling for a page id before the batch is failed
 template <int NC, int T, bool PLAIN>
-__global__ void __launch_bounds__(SA_THREADS, sa_occ<T>(NC)) k_scatter_cols(const ScatterAosParams q) {
+__global__ void __launch_bounds__(SA_THREADS, sa_occ<T>(NC)) k_scatter_cols(const ScatterAosParams q, const PosPages pg) {
   constexpr int R = T / SA_THREADS;  // rows per thread per tile
+  constexpr int BPT = (SA_MAX_BINS + SA_THREADS - 1) / SA_THREADS;  // bins per thread, at most
   extern __shared__ __align__(128) unsigned char s_raw[];
   const ScatterParams &p = q.sp;
   const int n_parts = 1 << p.pbits;
   const int trash = n_parts;                    // rows that produce nothing
   const int n_bins = n_parts + 1;
   const int bstride = (n_bins + 3) & ~3;
+  const uint32_t PG = pg.page_rows;
   uint64_t *s_in = reinterpret_cast<uint64_t *>(s_raw);                       // [2][NC][T]
   uint64_t *s_sorted = s_in + 2 * NC * T;                                      // [NC][T]
-  uint32_t *s_dst = reinterpret_cast<uint32_t *>(s_sorted + NC * T);           // [T] result slot of sorted position i
+  uint32_t *s_dst = reinterpret_cast<uint32_t *>(s_sorted + NC * T);           // [T] (bin << 16) | rank of sorted position i
   uint32_t *s_hist = s_dst + T;                                                // [n_bins] tile histogram (zero between tiles)
-  uint2 *s_bin = reinterpret_cast<uint2 *>(s_hist + bstride);                  // [n_bins] {first sorted position of the bin, slot of its first row}
-  uint64_t *s_mbar = reinterpret_cast<uint64_t *>(s_bin + bstride);            // [2]
+  uint2 *s_bin = reinterpret_cast<uint2 *>(s_hist + bstride);                  // [n_bins] {first sorted position of the bin, rows of its run before the page boundary}
+  uint2 *s_map = s_bin + bstride;                                              // [n_bins] {physical slot of rank 0, physical slot of rank e minus e}
+  uint64_t *s_mbar = reinterpret_cast<uint64_t *>(s_map + bstride);            // [2]
   __shared__ uint32_t s_warp[SA_WARPS + 1];
 
   const int tid = threadIdx.x, lane = tid & 31, warp = tid >> 5;
@@ -469,6 +456,12 @@ __global__ void __launch_bounds__(SA_THREADS, sa_occ<T>(NC)) k_scatter_cols(cons
     mbar_expect_tx(&s_mbar[stage], (uint32_t)(NC * T * 8));
 #pragma unroll
     for (int c = 0; c < NC; c++) tma_load_1d(s_in + (stage * NC + c) * T, stream_tile_col(q, T, tile, c), (uint32_t)(T * 8), &s_mbar[stage]);
+  };
+  // a new physical page for virtual page slot `e` of the page table: its id
+  auto alloc_page = [&](unsigned long long *e) {
+    const uint32_t id = atomicAdd(&pg.cursor[n_parts], 1u);
+    st_relaxed_u64(e, ((unsigned long long)pg.epoch << 32) | id);  // (the id is the only datum: nothing else to release)
+    return id;
   };
   if (tid == 0) {
     const int64_t t0 = blockIdx.x, t1 = t0 + gridDim.x;
@@ -506,7 +499,7 @@ __global__ void __launch_bounds__(SA_THREADS, sa_occ<T>(NC)) k_scatter_cols(cons
       rank[k] = (uint16_t)atomicAdd(&s_hist[b], 1u);
     }
     __syncthreads();
-    // ---- exclusive scan over the bins; every non-empty partition claims its run of slots with ONE global atomic
+    // ---- exclusive scan over the bins; every non-empty partition claims its run of virtual slots with ONE global atomic
     uint32_t tsum = 0;
     for (int j = 0; j < bpt; j++) {
       const int b = tid * bpt + j;
@@ -525,29 +518,61 @@ __global__ void __launch_bounds__(SA_THREADS, sa_occ<T>(NC)) k_scatter_cols(cons
     }
     __syncthreads();
     uint32_t run = inc - tsum + s_warp[warp];
-    for (int j = 0; j < bpt; j++) {
+    // a run that starts inside a page an earlier claim opened: that page's table entry (loaded now, awaited after placement)
+    const unsigned long long *wait_e[BPT];
+    unsigned long long wait_v[BPT];
+    uint32_t wait_o[BPT], wait_d1[BPT];
+#pragma unroll
+    for (int j = 0; j < BPT; j++) {
       const int b = tid * bpt + j;
-      if (b < n_bins) {
+      wait_e[j] = nullptr;
+      if (j < bpt && b < n_bins) {
         const uint32_t c = s_hist[b];
         s_hist[b] = 0;  // ready for the next tile (its ranking starts behind two more barriers)
-        const uint32_t g = (c && b != trash) ? atomicAdd(&p.part_cursor[b], c) : 0u;
-        s_bin[b] = make_uint2(run, g);
+        uint32_t e = 0;
+        if (c && b != trash) {
+          const uint32_t g = atomicAdd(&pg.cursor[b], c);
+          unsigned long long *row = pg.pt + (uint64_t)b * pg.kmax;
+          const uint32_t k0 = g / PG, o = g - k0 * PG;
+          e = PG - o;                                              // rows of the run inside its first page
+          const uint32_t d1 = c > e ? alloc_page(row + k0 + 1) * PG - e : 0u;   // (rank r >= e lands at d1 + r)
+          if (o == 0) {
+            s_map[b] = make_uint2(alloc_page(row + k0) * PG, d1);
+          } else {
+            wait_e[j] = row + k0;
+            wait_v[j] = ld_relaxed_u64(row + k0);
+            wait_o[j] = o;
+            wait_d1[j] = d1;
+          }
+        }
+        s_bin[b] = make_uint2(run, e);
         run += c;
       }
     }
     __syncthreads();
     const uint32_t total = s_bin[trash].x;  // rows that go somewhere
-    // ---- place the rows at their sorted positions (column-major) together with their result slot
+    // ---- place the rows at their sorted positions (column-major) together with their bin and rank
 #pragma unroll
     for (int k = 0; k < R; k++) {
       const uint32_t b = pid[k];
       if (b == (uint32_t)trash) continue;
       const int row = k * SA_THREADS + tid;
-      const uint2 bin = s_bin[b];
-      const uint32_t sp = bin.x + rank[k];
-      s_dst[sp] = bin.y + rank[k];
+      const uint32_t sp = s_bin[b].x + rank[k];
+      s_dst[sp] = (b << 16) | rank[k];
 #pragma unroll
       for (int c = 0; c < NC; c++) s_sorted[c * T + sp] = in_s[c * T + row];
+    }
+    // ---- the page ids of runs that started inside an earlier claim's page
+#pragma unroll
+    for (int j = 0; j < BPT; j++) {
+      if (!wait_e[j]) continue;
+      unsigned long long v = wait_v[j];
+      for (uint32_t spins = 0; (uint32_t)(v >> 32) != pg.epoch; spins++) {
+        if (spins == PAGE_WAIT_SPINS) { atomicOr(pg.err, 1ull); v = 0; break; }   // (page 0: writes stay in bounds)
+        __nanosleep(64);
+        v = ld_relaxed_u64(wait_e[j]);
+      }
+      s_map[tid * bpt + j] = make_uint2((uint32_t)v * PG + wait_o[j], wait_d1[j]);
     }
     __syncthreads();
     // the input stage is free again: fetch the tile this CTA handles two iterations from now
@@ -557,7 +582,9 @@ __global__ void __launch_bounds__(SA_THREADS, sa_occ<T>(NC)) k_scatter_cols(cons
     }
     // ---- stream the sorted tile out: consecutive threads write consecutive slots of every result column
     for (uint32_t i = tid; i < total; i += SA_THREADS) {
-      const uint32_t d = s_dst[i];
+      const uint32_t u = s_dst[i], b = u >> 16, r = u & 0xFFFFu;
+      const uint2 m = s_map[b];
+      const uint32_t d = (r < s_bin[b].y ? m.x : m.y) + r;
 #pragma unroll
       for (int c = 0; c < NC; c++) tqd::st_stream_u64(p.out[c].data + d, s_sorted[c * T + i]);
     }
@@ -565,12 +592,11 @@ __global__ void __launch_bounds__(SA_THREADS, sa_occ<T>(NC)) k_scatter_cols(cons
   }
 }
 
-typedef void (*ScatterColsKernel)(const ScatterAosParams);
+typedef void (*ScatterColsKernel)(const ScatterAosParams, const PosPages);
 template <int T, bool PLAIN>
 static ScatterColsKernel scatter_cols_kernel_t(int nc) {
   if (T == 4096) return nc == 1 ? k_scatter_cols<1, 4096, PLAIN> : (nc == 2 ? k_scatter_cols<2, 4096, PLAIN> : nullptr);
-  switch (nc) {
-    case 1: return k_scatter_cols<1, 2048, PLAIN>;
+  switch (nc) {  // (one column always takes 4096-row tiles: that image fits at every partition count)
     case 2: return k_scatter_cols<2, 2048, PLAIN>;
     case 3: return k_scatter_cols<3, 2048, PLAIN>;
     case 4: return k_scatter_cols<4, 2048, PLAIN>;
@@ -580,40 +606,41 @@ static ScatterColsKernel scatter_cols_kernel_t(int nc) {
 // Rows per tile of the column scatter: 4096 where that shared-memory image fits an SM (one or two columns), else 2048.  A run
 // a tile claims in one partition is then ~T / P rows of every column: at C3 (128 partitions) 4096-row tiles write runs of
 // 256 bytes per column, which measured 1.39 ms against 1.65 ms for 2048-row tiles (H100 80GB HBM3, 700 W).
-static int scatter_cols_tile(int nc, int bins) { return sa_smem_bytes<4096>(nc, bins) <= 220 * 1024 ? 4096 : 2048; }
-// Segmented regions are counted and scattered in tiles of different sizes, so a region's rows are a multiple of the largest.
+static int scatter_cols_tile(int nc, int bins) { return sc_smem_bytes<4096>(nc, bins) <= 220 * 1024 ? 4096 : 2048; }
+// Segmented regions are read in whole scatter tiles, so a region's rows are a multiple of the largest.
 static constexpr int POS_SEG_ROWS_ALIGN = 4096;
-static constexpr int PC_TILE = 2048;  // rows per tile of k_pos_count
+static constexpr int PP_TILE_ROWS = 12 * 32 * 2;  // rows per tile of k_probe_pos (probe_pos_variant)
 
-// count -> bases -> column-wise scatter of one positional batch into the result columns q.sp.out[c] (every slot of
-// [0, S) belongs to exactly one partition run or pad).  q describes the input as for k_scatter_aos (columns, key, key_mode,
-// selected, pbits, n, segments of seg_rows rows each, a multiple of POS_SEG_ROWS_ALIGN); m's words are reserved by the caller.
-static int32_t launch_pos_scatter(ScatterAosParams &q, int64_t seg_rows, const PosMeta &m, int probe_tile, unsigned long long *span, cudaStream_t s) {
+// Rows per page of the positional result.  Whole probe tiles, so ballot words and the probe's bulk copies stay inside a page;
+// at least one scatter tile, so a run a tile claims crosses at most one page boundary; past that, the most tiles that keep
+// P * page_rows -- the rows the partitions' last pages can leave unfilled, hence the room the result needs beyond n and the
+// holes to fill -- within 1 % of the batch.  At C3 (1e8 rows, 128 partitions) that is 10 tiles = 7,680 rows; a batch of 8M
+// rows gets the 6-tile minimum.
+static uint32_t pos_page_rows(int64_t n, int P, int nc) {
+  const int64_t min_tiles = (scatter_cols_tile(nc, P + 1) + PP_TILE_ROWS - 1) / PP_TILE_ROWS;
+  const int64_t tiles = n / (100ll * P * PP_TILE_ROWS);
+  return (uint32_t)((tiles > min_tiles ? tiles : min_tiles) * PP_TILE_ROWS);
+}
+
+// reset -> column-wise scatter -> page bases of one positional batch into the result columns q.sp.out[c] (every slot of
+// [0, S) belongs to exactly one page).  q describes the input as for k_scatter_aos (columns, key, key_mode, selected, pbits,
+// n, segments of seg_rows rows each, a multiple of POS_SEG_ROWS_ALIGN); m's words are reserved by the caller.
+static int32_t launch_pos_scatter(ScatterAosParams &q, int64_t seg_rows, const PosPages &m, unsigned long long *span, cudaStream_t s) {
   const int nc = q.sp.n_cols, P = 1 << q.sp.pbits;
   const bool plain = !q.sp.selected && q.sp.key_mode == KEYMODE_RAW;
-  auto n_tiles = [&](int T) { return q.n_segs ? (int64_t)q.n_segs * (seg_rows / T) : (q.sp.n + T - 1) / T; };
-  // counts
-  TQ_CUDA(cudaMemsetAsync(m.cnt, 0, (size_t)P * 4, s));
-  q.seg_tiles = (int)(seg_rows / PC_TILE);
-  const int cnt_smem = (PC_THREADS / 32) * P * 4;
-  const int64_t cnt_tiles = n_tiles(PC_TILE), cnt_cap = (int64_t)rt().sm_count * 8;
-  const int cnt_grid = (int)(cnt_tiles < cnt_cap ? (cnt_tiles < 1 ? 1 : cnt_tiles) : cnt_cap);
-  (plain ? k_pos_count<PC_TILE, true> : k_pos_count<PC_TILE, false>)<<<cnt_grid, PC_THREADS, cnt_smem, s>>>(q, m.cnt);
-  TQ_TRY(check_launch("k_pos_count"));
-  k_pos_bases<<<1, POS_BASES_THREADS, 0, s>>>(m, P, probe_tile, span);
-  TQ_TRY(check_launch("k_pos_bases"));
-  // scatter
   const int T = scatter_cols_tile(nc, P + 1);
   ScatterColsKernel k = T == 4096 ? (plain ? scatter_cols_kernel_t<4096, true>(nc) : scatter_cols_kernel_t<4096, false>(nc))
                                   : (plain ? scatter_cols_kernel_t<2048, true>(nc) : scatter_cols_kernel_t<2048, false>(nc));
-  const int smem = T == 4096 ? sa_smem_bytes<4096>(nc, P + 1) : sa_smem_bytes<2048>(nc, P + 1);
+  const int smem = T == 4096 ? sc_smem_bytes<4096>(nc, P + 1) : sc_smem_bytes<2048>(nc, P + 1);
   int per_sm = T == 4096 ? sa_occ<4096>(nc) : sa_occ<2048>(nc);
   if (!k || smem > 227 * 1024) { set_error("internal: column scatter of %d columns into %d partitions does not fit shared memory", nc, P); return TQ_ERR_INVALID_ARG; }
   TQ_CUDA(cudaFuncSetAttribute(k, cudaFuncAttributeMaxDynamicSharedMemorySize, smem));
   while (per_sm > 1 && (int64_t)smem * per_sm > 224 * 1024) per_sm--;
-  const int64_t tiles = n_tiles(T), cap = (int64_t)rt().sm_count * per_sm;
+  // (launched after the host-side set-up above, so that the scatter follows the tiny reset without a gap)
+  k_pos_reset<<<1, POS_BASES_THREADS, 0, s>>>(m.cursor, P + 1);
+  TQ_TRY(check_launch("k_pos_reset"));
+  const int64_t tiles = q.n_segs ? (int64_t)q.n_segs * (seg_rows / T) : (q.sp.n + T - 1) / T, cap = (int64_t)rt().sm_count * per_sm;
   q.seg_tiles = (int)(seg_rows / T);
-  q.sp.part_cursor = m.cursor;
   auto aligned = [](const void *ptr) { return (reinterpret_cast<uintptr_t>(ptr) & 15) == 0; };
   q.use_tma = 1;
   for (int c = 0; c < nc; c++) {
@@ -621,16 +648,20 @@ static int32_t launch_pos_scatter(ScatterAosParams &q, int64_t seg_rows, const P
     for (int g = 0; g < q.n_segs; g++)
       if (!aligned(q.seg_in[g][c])) q.use_tma = 0;
   }
-  k<<<(int)(tiles < cap ? (tiles < 1 ? 1 : tiles) : cap), SA_THREADS, smem, s>>>(q);
+  k<<<(int)(tiles < cap ? (tiles < 1 ? 1 : tiles) : cap), SA_THREADS, smem, s>>>(q, m);
+  TQ_TRY(check_launch("k_scatter_cols"));
+  k_pos_pages<<<1, POS_BASES_THREADS, 0, s>>>(m, P, PP_TILE_ROWS, span);
   count_launch(3);
-  return check_launch("k_scatter_cols");
+  return check_launch("k_pos_pages");
 }
 
 static constexpr int PP_STAGES = 4;
 
 struct ProbePosParams {
-  const uint64_t *keys;              // the result's probe key column: partition q = slots [base[q], base[q] + cnt[q])
-  const uint32_t *cnt, *base, *chunk;  // PosMeta
+  const uint64_t *keys;              // the result's probe key column
+  const uint32_t *cnt, *chunk;       // PosPages: rows per partition (the final cursors), the work list
+  const unsigned long long *pt;      // PosPages: the page table, kmax entries per partition
+  uint32_t page_rows, kmax;
   int n_parts;
   uint64_t *out_build[4];
   int build_word[4];                 // word of build column c inside a table entry
@@ -673,8 +704,9 @@ __device__ __forceinline__ bool probe_find(const uint64_t *words, uint32_t cap, 
 }
 
 // R rows per lane per step, CW consumer warps (+ 1 producer warp), OCC resident CTAs per SM asked of the compiler.
-// One tile = CW * 32 * R rows.  The probe columns are already in their result slots (k_scatter_cols): this kernel reads the
-// key column back and writes the build columns and the validity ballots.
+// One tile = CW * 32 * R rows, and a page is whole tiles: the producer maps each tile of the partition to its physical slots
+// through the page table and hands that slot to the consumers with the stage.  The probe columns are already in their result
+// slots (k_scatter_cols): this kernel reads the key column back and writes the build columns and the validity ballots.
 template <int NB, int R, int CW, int OCC>
 __global__ void __launch_bounds__((CW + 1) * 32, OCC) k_probe_pos(const ProbePosParams p, const JoinTable t) {
   constexpr int PP_TILE = CW * 32 * R;
@@ -684,8 +716,9 @@ __global__ void __launch_bounds__((CW + 1) * 32, OCC) k_probe_pos(const ProbePos
   uint64_t *s_tile = reinterpret_cast<uint64_t *>(s_raw);  // [PP_STAGES][PP_TILE] probe keys
   __shared__ __align__(8) uint64_t s_full[PP_STAGES], s_empty[PP_STAGES];
   __shared__ uint64_t s_sink[CW];
+  __shared__ uint32_t s_slot[PP_STAGES];  // physical slot of the first row of the tile in each stage
   const int tid = threadIdx.x, lane = tid & 31, warp = tid >> 5;
-  // this CTA's partition and tiles, from the work list of k_pos_bases: chunk[part] <= blockIdx.x < chunk[part + 1]
+  // this CTA's partition and tiles, from the work list of k_pos_pages: chunk[part] <= blockIdx.x < chunk[part + 1]
   const uint32_t cta = blockIdx.x;
   if (cta >= p.chunk[p.n_parts]) return;  // (the grid is sized for the worst case)
   uint32_t part = 0, hi = (uint32_t)p.n_parts;
@@ -698,8 +731,12 @@ __global__ void __launch_bounds__((CW + 1) * 32, OCC) k_probe_pos(const ProbePos
   const int64_t p_tiles = (p_rows + PP_TILE - 1) / PP_TILE;
   const int64_t t_lo = (int64_t)(cta - p.chunk[part]) * PP_CHUNK_TILES;
   const int64_t t_hi = t_lo + PP_CHUNK_TILES < p_tiles ? t_lo + PP_CHUNK_TILES : p_tiles;
-  const uint64_t p_base = p.base[part];
-  const uint64_t *keys = p.keys + p_base;  // 256-byte aligned: the bases are multiples of 32 slots
+  const unsigned long long *pages = p.pt + (uint64_t)part * p.kmax;
+  const uint32_t PG = p.page_rows;
+  auto tile_slot = [&](int64_t tile) {  // physical slot of the tile's first row: a multiple of 32 (256-byte aligned keys)
+    const uint32_t r0 = (uint32_t)(tile * PP_TILE), k = r0 / PG;
+    return (uint32_t)pages[k] * PG + (r0 - k * PG);
+  };
   if (tid == 0) {
     for (int s = 0; s < PP_STAGES; s++) { mbar_init(&s_full[s], 1); mbar_init(&s_empty[s], PP_CONSUMER_WARPS); }
     asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
@@ -712,16 +749,20 @@ __global__ void __launch_bounds__((CW + 1) * 32, OCC) k_probe_pos(const ProbePos
       if (it >= PP_STAGES) mbar_spin(&s_empty[s], (uint32_t)(((it / PP_STAGES) - 1) & 1));
       const int64_t r0 = tile * PP_TILE;
       const int64_t rows = (p_rows - r0) < PP_TILE ? (p_rows - r0) : PP_TILE;
+      const uint32_t slot = tile_slot(tile);
       uint64_t *dst = s_tile + (size_t)s * PP_TILE;
-      for (int64_t i = lane; i < rows; i += 32) dst[i] = keys[r0 + i];
+      for (int64_t i = lane; i < rows; i += 32) dst[i] = p.keys[slot + i];
       __syncwarp();
-      if (lane == 0) mbar_arrive(&s_full[s]);
+      if (lane == 0) {
+        s_slot[s] = slot;
+        mbar_arrive(&s_full[s]);
+      }
     }
     return;
   }
   if (warp == PP_CONSUMER_WARPS) {
     // ---- producer: keeps PP_STAGES key tiles in flight (TMA bulk copies; bytes rounded up to 16: an odd row count ends
-    // inside the partition's pad)
+    // inside the tile's page)
     if (lane == 0) {
       int it = 0;
       for (int64_t tile = t_lo; tile < t_hi; tile++, it++) {
@@ -730,8 +771,10 @@ __global__ void __launch_bounds__((CW + 1) * 32, OCC) k_probe_pos(const ProbePos
         const int64_t r0 = tile * PP_TILE;
         const int64_t rows = (p_rows - r0) < PP_TILE ? (p_rows - r0) : PP_TILE;
         const uint32_t bytes = (uint32_t)((rows * 8 + 15) & ~15ll);
+        const uint32_t slot = tile_slot(tile);
+        s_slot[s] = slot;  // (published to the consumers by the arrive below)
         mbar_expect_tx(&s_full[s], bytes);
-        tma_load_1d(s_tile + (size_t)s * PP_TILE, keys + r0, bytes, &s_full[s]);
+        tma_load_1d(s_tile + (size_t)s * PP_TILE, p.keys + slot, bytes, &s_full[s]);
       }
     }
     return;
@@ -740,12 +783,10 @@ __global__ void __launch_bounds__((CW + 1) * 32, OCC) k_probe_pos(const ProbePos
   // probe partitions (k_build_cluster's sub-tables), so a row's table comes from its own hash.
   const uint32_t cap = t.cap;
   const int woff = warp * (32 * R) + lane;                      // this lane's first row inside a tile
-  const uint64_t obase = p_base + woff;                         // ... and its output slot inside the partition's range
   uint64_t *ob[NB];
   int bw[NB];
 #pragma unroll
-  for (int c = 0; c < NB; c++) { ob[c] = p.out_build[c] + obase; bw[c] = p.build_word[c]; }
-  uint32_t *vword = p.valid + ((obase - lane) >> 5);
+  for (int c = 0; c < NB; c++) { ob[c] = p.out_build[c] + woff; bw[c] = p.build_word[c]; }
   unsigned matched = 0;
   int it = 0;
   for (int64_t tile = t_lo; tile < t_hi; tile++, it++) {
@@ -753,6 +794,7 @@ __global__ void __launch_bounds__((CW + 1) * 32, OCC) k_probe_pos(const ProbePos
     mbar_spin(&s_full[s], (uint32_t)((it / PP_STAGES) & 1));
     const int64_t t0 = tile * PP_TILE;                              // first row of the tile inside the partition
     const uint64_t *src = s_tile + (size_t)s * PP_TILE + woff;
+    const uint32_t oslot = s_slot[s];                               // ... and its physical slot
     uint64_t key[R];
 #pragma unroll
     for (int k = 0; k < R; k++) key[k] = src[k * 32];
@@ -760,7 +802,7 @@ __global__ void __launch_bounds__((CW + 1) * 32, OCC) k_probe_pos(const ProbePos
     // memory first.  An issued LDS is not a completed one: SASS showed LDS.128 x4, WARPSYNC, SYNCS.ARRIVE with no scoreboard
     // wait in between, and the refill then tore rows (first 16 bytes of one tile, last 16 of another).  The register scoreboard is per warp, so ONE instruction that reads every loaded
     // register waits for the whole warp's loads: lane 0 stores their XOR to a sink word before it arrives on the barrier.
-    uint64_t dep = 0;
+    uint64_t dep = oslot;
 #pragma unroll
     for (int k = 0; k < R; k++) dep ^= key[k];
     __syncwarp();
@@ -783,7 +825,7 @@ __global__ void __launch_bounds__((CW + 1) * 32, OCC) k_probe_pos(const ProbePos
         else ea[k] = ld_entry(t.words, loc[k], SHIFT);
       }
     }
-    const int64_t oslot = t0;  // output slot of this lane's k-th row = ob[c] + oslot + k * 32
+    uint32_t *vword = p.valid + ((oslot + warp * (32 * R)) >> 5);   // output slot of this lane's k-th row = ob[c] + oslot + k * 32
 #pragma unroll
     for (int k = 0; k < R; k++) {
       uint64_t w1 = 0;
@@ -797,9 +839,9 @@ __global__ void __launch_bounds__((CW + 1) * 32, OCC) k_probe_pos(const ProbePos
         }
       }
       const unsigned bal = __ballot_sync(0xffffffffu, hit);
-      // groups past the partition's padded end belong to the next partition: only groups that start inside it are recorded
+      // only groups that start inside the partition are recorded (the words past them in its last page are cleared below)
       if (lane == 0 && (t0 + woff + k * 32) < p_rows) {
-        vword[(oslot >> 5) + k] = bal;
+        vword[k] = bal;
         matched += __popc(bal);
       }
       if (hit) {
@@ -818,6 +860,13 @@ __global__ void __launch_bounds__((CW + 1) * 32, OCC) k_probe_pos(const ProbePos
       if (lane == 0) mbar_arrive(&s_empty[s]);
     }
   }
+  // the CTA with the partition's last tile clears the ballot words past it in its last page (no row ever lands there), so the
+  // validity bitmap is exact over the whole span
+  if (t_hi == p_tiles && p_rows > 0) {
+    const uint32_t kl = (uint32_t)((p_rows - 1) / PG), fill = (uint32_t)p_rows - kl * PG;
+    uint32_t *pw = p.valid + (((uint32_t)pages[kl] * PG) >> 5);
+    for (uint32_t w = (fill + 31) / 32 + warp * 32 + lane; w < PG / 32; w += CW * 32) pw[w] = 0;
+  }
   if (lane == 0 && matched) atomicAdd(p.cursor, (unsigned long long)matched);
 }
 
@@ -830,7 +879,8 @@ template <int NB>
 static ProbePosVariant probe_pos_variant() {
   // 2 rows per lane x 12 consumer warps x 3 CTAs per SM: more warps in flight hide the L2 latency of the table gathers better
   // than more loads per warp (4 rows per lane spills at 3 CTAs per SM).
-  return {k_probe_pos<NB, 2, 12, 3>, 12 * 32 * 2, 13 * 32};
+  static_assert(PP_TILE_ROWS == 12 * 32 * 2, "page sizes are whole probe tiles");
+  return {k_probe_pos<NB, 2, 12, 3>, PP_TILE_ROWS, 13 * 32};
 }
 static ProbePosVariant probe_pos_kernel(int nb) {
   switch (nb) {
