@@ -586,7 +586,10 @@ int32_t tq_mjoin_destroy(tq_mjoin *j);
  * All buffers are device memory.  out_cols must hold `n` rows each; rows of partition p
  * occupy [offsets[p], offsets[p+1]) of every output column, stable within a partition.
  * part_offsets is a HOST array of n_parts+1 entries.  Rows whose key is NULL go to
- * partition (row % n_parts): they never match but outer joins still emit them. */
+ * partition (row % n_parts): they never match but outer joins still emit them.
+ * Every column is moved as 8-byte words: types[c] & 0xFF must be TQ_TYPE_INT64, _UINT64 or
+ * _FLOAT64 and `offsets` NULL; a FLOAT32 or BYTES column is refused with
+ * TQ_ERR_UNSUPPORTED_TYPE before anything is written. */
 int32_t tq_partition_device(int32_t n_cols, const tq_column *cols, const int32_t *types,
                             int32_t key_col, int64_t n, int32_t n_parts, tq_column *out_cols,
                             int64_t *part_offsets);

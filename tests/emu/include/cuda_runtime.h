@@ -1,6 +1,6 @@
 // cuda_runtime.h of the CPU EMULATION build (tests/emu) — TEST INFRASTRUCTURE, never part of the product library.
 //
-// tests/emu compiles product sources (tinysql_b200/csrc/sort.cu, codec.cu, dict.cu, strdict.cu ...) unchanged with g++: this header stands in for the CUDA
+// tests/emu compiles product sources (tinysql_b200/csrc/sort.cu, codec.cu, dict.cu, strdict.cu, partition.cu ...) unchanged with g++: this header stands in for the CUDA
 // runtime and maps the handful of device primitives those kernels use onto host threads — ONE OS thread per CUDA thread of a
 // block, blocks run one after another, __syncthreads() and the warp collectives are pthread barriers.  Slow, but it executes
 // the real kernel code (indexing, ranking, masks, binary searches) so `-m "not gpu"` can check it against the oracle.
@@ -63,6 +63,7 @@ void warp_sync();
 #define TQ_LAUNCH(kernel, grid, block, smem, stream, ...) tq_emu::launch(dim3(grid), dim3(block), [&] { kernel(__VA_ARGS__); })
 
 static inline void __syncthreads() { tq_emu::block_sync(); }
+static inline void __syncwarp(unsigned = 0xffffffffu) { tq_emu::warp_sync(); }   // every lane of the warp arrives (see below)
 
 // warp collectives: every lane of the warp takes part (the kernels keep whole warps converged around them)
 template <typename T>
@@ -143,6 +144,7 @@ static inline unsigned long long atomicMax(unsigned long long *p, unsigned long 
   while (cur < v && !__atomic_compare_exchange_n(p, &cur, v, false, __ATOMIC_SEQ_CST, __ATOMIC_SEQ_CST)) {}
   return cur;
 }
+static inline unsigned atomicOr(unsigned *p, unsigned v) { return __atomic_fetch_or(p, v, __ATOMIC_SEQ_CST); }
 static inline unsigned long long atomicOr(unsigned long long *p, unsigned long long v) { return __atomic_fetch_or(p, v, __ATOMIC_SEQ_CST); }
 static inline unsigned long long atomicAnd(unsigned long long *p, unsigned long long v) { return __atomic_fetch_and(p, v, __ATOMIC_SEQ_CST); }
 

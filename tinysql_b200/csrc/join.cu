@@ -3741,8 +3741,14 @@ static int32_t partition_push(int32_t n_cols, const tq_column *cols, int32_t key
   DevBuf &cursor = cursors[async ? 1 : 0];
   TQ_TRY(cursor.reserve(64));
   static PinBuf h_cur_pin[2];
+  // staged_ev[i] marks the end of the last copy out of h_cur_pin[i]: an async push returns with that copy still queued
+  // behind whatever the push stream is running, so the next push may rewrite the staging only once the copy has read it
+  static cudaEvent_t staged_ev[2];
+  cudaEvent_t &staged = staged_ev[async ? 1 : 0];
+  if (!staged) TQ_CUDA(cudaEventCreateWithFlags(&staged, cudaEventDisableTiming));
   TQ_TRY(h_cur_pin[async ? 1 : 0].reserve(64));
   uint32_t *h_cur = h_cur_pin[async ? 1 : 0].as<uint32_t>();
+  TQ_CUDA(cudaEventSynchronize(staged));
   memset(h_cur, 0, 64);
   ScatterParams sp{};
   sp.n_cols = n_cols;
@@ -3758,6 +3764,7 @@ static int32_t partition_push(int32_t n_cols, const tq_column *cols, int32_t key
     for (int c = 0; c < n_cols; c++) sp.out_bin[q][c] = (uint64_t *)dest_data[q * n_cols + c];
   }
   TQ_CUDA(cudaMemcpyAsync(cursor.p, h_cur, 64, cudaMemcpyHostToDevice, s));
+  TQ_CUDA(cudaEventRecord(staged, s));
   sp.part_cursor = cursor.as<uint32_t>();
   sp.part_lim = nullptr;
   static DevBuf ovf;

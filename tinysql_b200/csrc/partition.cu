@@ -82,12 +82,20 @@ using namespace tq;
 
 extern "C" int32_t tq_partition_device(int32_t n_cols, const tq_column *cols, const int32_t *types, int32_t key_col, int64_t n, int32_t n_parts,
                                        tq_column *out_cols, int64_t *part_offsets) {
-  (void)types;
   TQ_TRY(ensure_init());
-  if (n_cols < 1 || n_cols > PART_MAXC || !cols || !out_cols || !part_offsets || key_col < 0 || key_col >= n_cols || n_parts < 1 || n_parts > PART_MAX ||
-      n < 0 || n > 0xFFFFFFF0ll) {
+  if (n_cols < 1 || n_cols > PART_MAXC || !cols || !types || !out_cols || !part_offsets || key_col < 0 || key_col >= n_cols || n_parts < 1 ||
+      n_parts > PART_MAX || n < 0 || n > 0xFFFFFFF0ll) {
     set_error("tq_partition_device: bad arguments");
     return TQ_ERR_INVALID_ARG;
+  }
+  // the kernels move every column as 8-byte words: FLOAT32 slots are 4 bytes and BYTES cells live behind offsets
+  for (int c = 0; c < n_cols; c++) {
+    const int t = types[c] & 0xFF;
+    if ((t != TQ_TYPE_INT64 && t != TQ_TYPE_UINT64 && t != TQ_TYPE_FLOAT64) || cols[c].offsets) {
+      set_error("tq_partition_device: column %d is not an 8-byte fixed-width column (type %d)", c, types[c]);
+      return TQ_ERR_UNSUPPORTED_TYPE;
+    }
+    if (cols[c].null_bitmap && !out_cols[c].null_bitmap) { set_error("output column %d needs a null bitmap", c); return TQ_ERR_INVALID_ARG; }
   }
   Runtime &r = rt();
   std::lock_guard<std::recursive_mutex> lk(r.mu);
@@ -109,7 +117,6 @@ extern "C" int32_t tq_partition_device(int32_t n_cols, const tq_column *cols, co
     p.in[c].bm = (const uint32_t *)cols[c].null_bitmap;
     p.out[c].data = (uint64_t *)out_cols[c].data;
     p.out[c].bm = cols[c].null_bitmap ? (uint32_t *)out_cols[c].null_bitmap : nullptr;
-    if (cols[c].null_bitmap && !out_cols[c].null_bitmap) { set_error("output column %d needs a null bitmap", c); return TQ_ERR_INVALID_ARG; }
     if (p.out[c].bm) TQ_CUDA(cudaMemsetAsync(p.out[c].bm, 0, bitmap_alloc_bytes(n) - 8, s));
     out_cols[c].length = n;
   }
@@ -119,12 +126,12 @@ extern "C" int32_t tq_partition_device(int32_t n_cols, const tq_column *cols, co
   TQ_TRY(h_off.reserve((size_t)(n_parts + 1) * 8));
   p.counts = counts.as<uint32_t>();
   const unsigned blocks = (unsigned)((p.n_chunks + 7) / 8);
-  k_part_hist<<<blocks, 256, 0, s>>>(p);
+  TQ_LAUNCH(k_part_hist, blocks, 256, 0, s, p);
   count_launch();
   TQ_TRY(check_launch("k_part_hist"));
   TQ_TRY(exclusive_scan_u32(p.counts, 1, p.counts, 1, n_counts, nullptr, scan_scratch, s));
-  k_part_offsets<<<(n_parts + 1 + 255) / 256, 256, 0, s>>>(p.counts, p.n_chunks, n_parts, n, d_off.as<int64_t>());
-  k_part_scatter<<<blocks, 256, 0, s>>>(p);
+  TQ_LAUNCH(k_part_offsets, (n_parts + 1 + 255) / 256, 256, 0, s, p.counts, p.n_chunks, n_parts, n, d_off.as<int64_t>());
+  TQ_LAUNCH(k_part_scatter, blocks, 256, 0, s, p);
   count_launch(2);
   TQ_TRY(check_launch("k_part_scatter"));
   TQ_CUDA(cudaMemcpyAsync(h_off.p, d_off.p, (size_t)(n_parts + 1) * 8, cudaMemcpyDeviceToHost, s));
