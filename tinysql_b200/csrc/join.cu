@@ -687,6 +687,94 @@ __global__ void __launch_bounds__(SCAT_THREADS) k_probe_part_hist(const ScatterP
     if (s_hist[b]) atomicAdd(&p.part_cnt[b], s_hist[b]);
 }
 
+// Exclusive scan of one value per thread over a CTA of THREADS threads (s_warp: THREADS / 32 + 1 words): returns the
+// thread's prefix, and s_warp[THREADS / 32] holds the CTA's sum.  Two barriers; a caller that writes s_warp again needs one
+// more between.
+template <int THREADS>
+__device__ __forceinline__ uint32_t block_excl_scan(uint32_t v, uint32_t *s_warp) {
+  static_assert(THREADS % 32 == 0 && THREADS <= 1024, "whole warps, at most 32 of them");
+  constexpr int NW = THREADS / 32;
+  const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
+  uint32_t inc = v;
+#pragma unroll
+  for (int d = 1; d < 32; d <<= 1) { const uint32_t x = __shfl_up_sync(0xffffffffu, inc, d); if (lane >= d) inc += x; }
+  if (lane == 31) s_warp[warp] = inc;
+  __syncthreads();
+  if (warp == 0) {
+    const uint32_t w = lane < NW ? s_warp[lane] : 0u;
+    uint32_t winc = w;
+#pragma unroll
+    for (int d = 1; d < 32; d <<= 1) { const uint32_t x = __shfl_up_sync(0xffffffffu, winc, d); if (lane >= d) winc += x; }
+    if (lane < NW) s_warp[lane] = winc - w;
+    if (lane == NW - 1) s_warp[NW] = winc;
+  }
+  __syncthreads();
+  return inc - v + s_warp[warp];
+}
+
+// Shared-memory image of k_probe_scatter and k_probe_scatter_fast (the fast kernel leaves `nn` unused).
+struct ScatterSmem {
+  uint64_t *stage;  // [SCAT_TILE] one column of the tile, sorted
+  uint32_t *bins;   // [n_bins] tile counts, then local exclusive offsets
+  uint32_t *gdelta; // [n_bins] (claimed global run start) - (local offset)
+  uint32_t *imax;   // [n_bins] first sorted position of the tile that no longer fits the slab
+  uint16_t *spid;   // [SCAT_TILE] sorted position -> partition
+  uint8_t *nn;      // [SCAT_TILE] sorted position -> NOT NULL flag
+};
+__host__ __device__ constexpr int scatter_smem_bytes(int n_bins) { return SCAT_TILE * (8 + 2 + 1) + n_bins * 4 * 3; }  // stage, spid, nn; 3 bin tables
+__device__ __forceinline__ ScatterSmem scatter_smem(unsigned char *raw, int n_bins) {
+  ScatterSmem m;
+  m.stage = reinterpret_cast<uint64_t *>(raw);
+  m.bins = reinterpret_cast<uint32_t *>(raw + SCAT_TILE * 8);
+  m.gdelta = m.bins + n_bins;
+  m.imax = m.gdelta + n_bins;
+  m.spid = reinterpret_cast<uint16_t *>(m.imax + n_bins);
+  m.nn = reinterpret_cast<uint8_t *>(m.spid + SCAT_TILE);
+  return m;
+}
+
+// From the partition pid[k] and the rank spos[k] of each of a thread's ROWS rows (sm.bins holds the tile's counts): scans the
+// bins, lets every non-empty bin claim its run with ONE global atomicAdd on part_cursor (clipped at part_lim, which raises the
+// overflow flag), turns each rank into the row's sorted position in the tile and records its partition in sm.spid.  Returns
+// the rows of the tile that go somewhere.
+template <int THREADS, int ROWS>
+__device__ __forceinline__ uint32_t scatter_claim(const ScatterParams &p, const ScatterSmem &sm, int n_bins, const uint32_t (&pid)[ROWS],
+                                                  uint32_t (&spos)[ROWS], uint32_t *s_warp) {
+  const int tid = threadIdx.x;
+  const int bpt = (n_bins + THREADS - 1) / THREADS;  // thread t owns bins [t*bpt, (t+1)*bpt)
+  __syncthreads();
+  uint32_t tsum = 0;
+  for (int q = 0; q < bpt; q++) { const int b = tid * bpt + q; if (b < n_bins) tsum += sm.bins[b]; }
+  uint32_t run = block_excl_scan<THREADS>(tsum, s_warp);
+  for (int q = 0; q < bpt; q++) {
+    const int b = tid * bpt + q;
+    if (b < n_bins) {
+      const uint32_t c = sm.bins[b];
+      sm.bins[b] = run;
+      if (c) {
+        const uint32_t g = atomicAdd(&p.part_cursor[b], c);
+        sm.gdelta[b] = g - run;
+        uint32_t imax = 0xFFFFFFFFu;
+        if (p.part_lim) {
+          const uint32_t lim = p.part_lim[b];
+          if (g + c > lim) { imax = (g < lim) ? run + (lim - g) : run; atomicOr(p.overflow, 1ull); }
+        }
+        sm.imax[b] = imax;
+      }
+      run += c;
+    }
+  }
+  const uint32_t total = s_warp[THREADS / 32];
+  __syncthreads();
+#pragma unroll
+  for (int k = 0; k < ROWS; k++) {
+    if (pid[k] == PID_DROP) continue;
+    spos[k] += sm.bins[pid[k]];
+    sm.spid[spos[k]] = (uint16_t)pid[k];
+  }
+  return total;
+}
+
 // One tile = SCAT_TILE (4096) rows.  The tile is counting-sorted by partition in shared memory (histogram -> local
 // exclusive scan -> sorted position per row), each non-empty partition claims its run with ONE global
 // atomicAdd, and every column then goes global -> shared (coalesced, at the row's sorted position) ->
@@ -694,20 +782,14 @@ __global__ void __launch_bounds__(SCAT_THREADS) k_probe_part_hist(const ScatterP
 __global__ void __launch_bounds__(SCAT_THREADS, 4) k_probe_scatter(const ScatterParams p) {
   extern __shared__ __align__(16) unsigned char s_scat[];
   const int n_bins = scatter_bins(p);
-  uint64_t *s_stage = reinterpret_cast<uint64_t *>(s_scat);                       // [SCAT_TILE] one column of the tile, sorted
-  uint32_t *s_bins = reinterpret_cast<uint32_t *>(s_scat + SCAT_TILE * 8);        // [n_bins] tile counts, then local exclusive offsets
-  uint32_t *s_gdelta = s_bins + n_bins;                                           // [n_bins] (claimed global run start) - (local offset)
-  uint32_t *s_imax = s_gdelta + n_bins;                                           // [n_bins] first sorted position of the tile that no longer fits the slab
-  uint16_t *s_spid = reinterpret_cast<uint16_t *>(s_imax + n_bins);               // [SCAT_TILE] sorted position -> partition
-  uint8_t *s_nn = reinterpret_cast<uint8_t *>(s_spid + SCAT_TILE);                // [SCAT_TILE] sorted position -> NOT NULL flag
+  const ScatterSmem sm = scatter_smem(s_scat, n_bins);
   __shared__ uint32_t s_warp[SCAT_THREADS / 32 + 1];
-  const int tid = threadIdx.x, lane = tid & 31, warp = tid >> 5;
-  const int bpt = (n_bins + SCAT_THREADS - 1) / SCAT_THREADS;  // bins per thread in the scan
+  const int tid = threadIdx.x;
   const uint64_t *keys = p.in[p.key_col].data;
   const int64_t n_tiles = (p.n + SCAT_TILE - 1) / SCAT_TILE;
   for (int64_t tile = blockIdx.x; tile < n_tiles; tile += gridDim.x) {
     const int64_t tile_base = tile * SCAT_TILE;
-    for (int b = tid; b < n_bins; b += SCAT_THREADS) s_bins[b] = 0;
+    for (int b = tid; b < n_bins; b += SCAT_THREADS) sm.bins[b] = 0;
     __syncthreads();
     uint32_t pid[SCAT_ROWS_PER_THREAD], spos[SCAT_ROWS_PER_THREAD];
 #pragma unroll
@@ -715,68 +797,25 @@ __global__ void __launch_bounds__(SCAT_THREADS, 4) k_probe_scatter(const Scatter
       const int64_t r = tile_base + k * SCAT_THREADS + tid;
       pid[k] = PID_DROP;
       if (r < p.n) pid[k] = probe_pid(p, r, keys[r]);
-      spos[k] = (pid[k] != PID_DROP) ? atomicAdd(&s_bins[pid[k]], 1u) : 0u;  // rank inside the partition
+      spos[k] = (pid[k] != PID_DROP) ? atomicAdd(&sm.bins[pid[k]], 1u) : 0u;  // rank inside the partition
     }
-    __syncthreads();
-    // exclusive scan over the bins (thread t owns bins [t*bpt, (t+1)*bpt))
-    uint32_t tsum = 0;
-    for (int q = 0; q < bpt; q++) { const int b = tid * bpt + q; if (b < n_bins) tsum += s_bins[b]; }
-    uint32_t inc = tsum;
-#pragma unroll
-    for (int d = 1; d < 32; d <<= 1) { const uint32_t v = __shfl_up_sync(0xffffffffu, inc, d); if (lane >= d) inc += v; }
-    if (lane == 31) s_warp[warp] = inc;
-    __syncthreads();
-    if (warp == 0) {
-      uint32_t w = (lane < SCAT_THREADS / 32) ? s_warp[lane] : 0, winc = w;
-#pragma unroll
-      for (int d = 1; d < 32; d <<= 1) { const uint32_t v = __shfl_up_sync(0xffffffffu, winc, d); if (lane >= d) winc += v; }
-      if (lane < SCAT_THREADS / 32) s_warp[lane] = winc - w;
-      if (lane == SCAT_THREADS / 32 - 1) s_warp[SCAT_THREADS / 32] = winc;
-    }
-    __syncthreads();
-    uint32_t run = inc - tsum + s_warp[warp];
-    for (int q = 0; q < bpt; q++) {
-      const int b = tid * bpt + q;
-      if (b < n_bins) {
-        const uint32_t c = s_bins[b];
-        s_bins[b] = run;
-        if (c) {
-          const uint32_t g = atomicAdd(&p.part_cursor[b], c);
-          s_gdelta[b] = g - run;
-          uint32_t imax = 0xFFFFFFFFu;
-          if (p.part_lim) {
-            const uint32_t lim = p.part_lim[b];
-            if (g + c > lim) { imax = (g < lim) ? run + (lim - g) : run; atomicOr(p.overflow, 1ull); }
-          }
-          s_imax[b] = imax;
-        }
-        run += c;
-      }
-    }
-    const uint32_t total = s_warp[SCAT_THREADS / 32];
-    __syncthreads();
-#pragma unroll
-    for (int k = 0; k < SCAT_ROWS_PER_THREAD; k++) {
-      if (pid[k] == PID_DROP) continue;
-      spos[k] += s_bins[pid[k]];
-      s_spid[spos[k]] = (uint16_t)pid[k];
-    }
+    const uint32_t total = scatter_claim<SCAT_THREADS>(p, sm, n_bins, pid, spos, s_warp);
     for (int c = 0; c < p.n_cols; c++) {
       const bool has_bm = p.out[c].bm != nullptr;
 #pragma unroll
       for (int k = 0; k < SCAT_ROWS_PER_THREAD; k++) {
         if (pid[k] == PID_DROP) continue;
         const int64_t r = tile_base + k * SCAT_THREADS + tid;
-        s_stage[spos[k]] = p.in[c].data[r];
-        if (has_bm) s_nn[spos[k]] = (uint8_t)tqd::bm_not_null(p.in[c].bm, r);
+        sm.stage[spos[k]] = p.in[c].data[r];
+        if (has_bm) sm.nn[spos[k]] = (uint8_t)tqd::bm_not_null(p.in[c].bm, r);
       }
       __syncthreads();
       for (uint32_t i = tid; i < total; i += SCAT_THREADS) {
-        const uint32_t bin = s_spid[i];
-        if (i >= s_imax[bin]) continue;  // slab full (optimistic path only)
-        const uint32_t dst = s_gdelta[bin] + i;
-        tqd::st_stream_u64(p.out[c].data + dst, s_stage[i]);
-        if (has_bm && s_nn[i]) atomicOr(&p.out[c].bm[dst >> 5], 1u << (dst & 31));
+        const uint32_t bin = sm.spid[i];
+        if (i >= sm.imax[bin]) continue;  // slab full (optimistic path only)
+        const uint32_t dst = sm.gdelta[bin] + i;
+        tqd::st_stream_u64(p.out[c].data + dst, sm.stage[i]);
+        if (has_bm && sm.nn[i]) atomicOr(&p.out[c].bm[dst >> 5], 1u << (dst & 31));
       }
       __syncthreads();
     }
@@ -792,14 +831,9 @@ template <int NP>
 __global__ void __launch_bounds__(SCATF_THREADS, (NP <= 2 ? 2 : 1)) k_probe_scatter_fast(const ScatterParams p) {
   extern __shared__ __align__(16) unsigned char s_scat[];
   const int n_bins = scatter_bins(p);
-  uint64_t *s_stage = reinterpret_cast<uint64_t *>(s_scat);
-  uint32_t *s_bins = reinterpret_cast<uint32_t *>(s_scat + SCAT_TILE * 8);
-  uint32_t *s_gdelta = s_bins + n_bins;
-  uint32_t *s_imax = s_gdelta + n_bins;
-  uint16_t *s_spid = reinterpret_cast<uint16_t *>(s_imax + n_bins);
+  const ScatterSmem sm = scatter_smem(s_scat, n_bins);
   __shared__ uint32_t s_warp[SCATF_THREADS / 32 + 1];
-  const int tid = threadIdx.x, lane = tid & 31, warp = tid >> 5;
-  const int bpt = (n_bins + SCATF_THREADS - 1) / SCATF_THREADS;
+  const int tid = threadIdx.x;
   const uint64_t *in[NP];
   uint64_t *out[NP];
 #pragma unroll
@@ -808,7 +842,7 @@ __global__ void __launch_bounds__(SCATF_THREADS, (NP <= 2 ? 2 : 1)) k_probe_scat
   const int64_t n_tiles = (p.n + SCAT_TILE - 1) / SCAT_TILE;
   for (int64_t tile = blockIdx.x; tile < n_tiles; tile += gridDim.x) {
     const int64_t tile_base = tile * SCAT_TILE;
-    for (int b = tid; b < n_bins; b += SCATF_THREADS) s_bins[b] = 0;
+    for (int b = tid; b < n_bins; b += SCATF_THREADS) sm.bins[b] = 0;
     uint64_t v[NP][SCATF_ROWS];
 #pragma unroll
     for (int k = 0; k < SCATF_ROWS; k++) {
@@ -830,84 +864,49 @@ __global__ void __launch_bounds__(SCATF_THREADS, (NP <= 2 ? 2 : 1)) k_probe_scat
         if (sel && key_valid(key, true, p.key_mode)) pid[k] = scatter_pid(p, key);
         else if (p.is_outer) pid[k] = (uint32_t)(n_bins - 1);
       }
-      spos[k] = (pid[k] != PID_DROP) ? atomicAdd(&s_bins[pid[k]], 1u) : 0u;
+      spos[k] = (pid[k] != PID_DROP) ? atomicAdd(&sm.bins[pid[k]], 1u) : 0u;
     }
-    __syncthreads();
-    uint32_t tsum = 0;
-    for (int q = 0; q < bpt; q++) { const int b = tid * bpt + q; if (b < n_bins) tsum += s_bins[b]; }
-    uint32_t inc = tsum;
-#pragma unroll
-    for (int d = 1; d < 32; d <<= 1) { const uint32_t x = __shfl_up_sync(0xffffffffu, inc, d); if (lane >= d) inc += x; }
-    if (lane == 31) s_warp[warp] = inc;
-    __syncthreads();
-    if (warp == 0) {
-      uint32_t w = (lane < SCATF_THREADS / 32) ? s_warp[lane] : 0, winc = w;
-#pragma unroll
-      for (int d = 1; d < 32; d <<= 1) { const uint32_t x = __shfl_up_sync(0xffffffffu, winc, d); if (lane >= d) winc += x; }
-      if (lane < SCATF_THREADS / 32) s_warp[lane] = winc - w;
-      if (lane == SCATF_THREADS / 32 - 1) s_warp[SCATF_THREADS / 32] = winc;
-    }
-    __syncthreads();
-    uint32_t run = inc - tsum + s_warp[warp];
-    for (int q = 0; q < bpt; q++) {
-      const int b = tid * bpt + q;
-      if (b < n_bins) {
-        const uint32_t c = s_bins[b];
-        s_bins[b] = run;
-        if (c) {
-          const uint32_t g = atomicAdd(&p.part_cursor[b], c);
-          s_gdelta[b] = g - run;
-          uint32_t imax = 0xFFFFFFFFu;
-          if (p.part_lim) {
-            const uint32_t lim = p.part_lim[b];
-            if (g + c > lim) { imax = (g < lim) ? run + (lim - g) : run; atomicOr(p.overflow, 1ull); }
-          }
-          s_imax[b] = imax;
-        }
-        run += c;
-      }
-    }
-    const uint32_t total = s_warp[SCATF_THREADS / 32];
-    __syncthreads();
-#pragma unroll
-    for (int k = 0; k < SCATF_ROWS; k++) {
-      if (pid[k] == PID_DROP) continue;
-      spos[k] += s_bins[pid[k]];
-      s_spid[spos[k]] = (uint16_t)pid[k];
-    }
+    const uint32_t total = scatter_claim<SCATF_THREADS>(p, sm, n_bins, pid, spos, s_warp);
 #pragma unroll
     for (int c = 0; c < NP; c++) {
 #pragma unroll
       for (int k = 0; k < SCATF_ROWS; k++)
-        if (pid[k] != PID_DROP) s_stage[spos[k]] = v[c][k];
+        if (pid[k] != PID_DROP) sm.stage[spos[k]] = v[c][k];
       __syncthreads();
       for (uint32_t i = tid; i < total; i += SCATF_THREADS) {
-        const uint32_t bin = s_spid[i];
-        if (i >= s_imax[bin]) continue;
+        const uint32_t bin = sm.spid[i];
+        if (i >= sm.imax[bin]) continue;
         uint64_t *dst = p.n_parts_mod ? p.out_bin[bin & 7][c] : out[c];
-        const uint32_t d32 = s_gdelta[bin] + i;  // 32-bit wrap-around arithmetic: (run start - local offset) + sorted position
-        tqd::st_stream_u64(dst + d32, s_stage[i]);
+        const uint32_t d32 = sm.gdelta[bin] + i;  // 32-bit wrap-around arithmetic: (run start - local offset) + sorted position
+        tqd::st_stream_u64(dst + d32, sm.stage[i]);
       }
       __syncthreads();
     }
   }
 }
-typedef void (*ScatterKernel)(const ScatterParams);
-static ScatterKernel scatter_fast_kernel(int np) {
-  switch (np) {
-    case 1: return k_probe_scatter_fast<1>;
-    case 2: return k_probe_scatter_fast<2>;
-    case 3: return k_probe_scatter_fast<3>;
-    case 4: return k_probe_scatter_fast<4>;
+
+// Launches k_probe_scatter_fast for sp.n_cols (1..4) NULL-free columns on stream s; `what` names the launch in errors.
+static int32_t launch_scatter_fast(const ScatterParams &sp, cudaStream_t s, const char *what) {
+  typedef void (*ScatterKernel)(const ScatterParams);
+  static const ScatterKernel kernels[5] = {nullptr, k_probe_scatter_fast<1>, k_probe_scatter_fast<2>, k_probe_scatter_fast<3>, k_probe_scatter_fast<4>};
+  static bool attr_set[5] = {};
+  const int np = sp.n_cols;
+  if (np < 1 || np > 4) { set_error("internal: %s of %d columns", what, np); return TQ_ERR_INVALID_ARG; }
+  if (!attr_set[np]) {
+    TQ_CUDA(cudaFuncSetAttribute(kernels[np], cudaFuncAttributeMaxDynamicSharedMemorySize, scatter_smem_bytes((1 << PART_MAX_BITS) + 1)));
+    attr_set[np] = true;
   }
-  return nullptr;
+  const int64_t tiles = (sp.n + SCAT_TILE - 1) / SCAT_TILE;
+  const int64_t cap = (int64_t)rt().sm_count * (np <= 2 ? 2 : 1);
+  kernels[np]<<<(int)(tiles < cap ? tiles : cap), SCATF_THREADS, scatter_smem_bytes(scatter_bins(sp)), s>>>(sp);
+  count_launch();
+  return check_launch(what);
 }
 
 // scatter.cuh: the same scatter for other operators (HashAgg pre-aggregation)
 int32_t scatter_rows_by_hash(const DCol *cols, int n_cols, int key_col, int64_t n, int pbits, std::vector<DevBuf> &out, DevBuf &lo, DevBuf &hi, DevBuf &lim,
                              unsigned long long *d_overflow, cudaStream_t s) {
-  ScatterKernel kern = scatter_fast_kernel(n_cols);
-  if (!kern || pbits < 1 || pbits > PART_MAX_BITS || n <= 0 || n > 0xFFFFFFF0ll) { set_error("internal: scatter_rows_by_hash arguments"); return TQ_ERR_INVALID_ARG; }
+  if (n_cols < 1 || n_cols > 4 || pbits < 1 || pbits > PART_MAX_BITS || n <= 0 || n > 0xFFFFFFF0ll) { set_error("internal: scatter_rows_by_hash arguments"); return TQ_ERR_INVALID_ARG; }
   const int P = 1 << pbits, n_bins = P + 1;
   const uint64_t slab = slab_rows(n, P, false);
   if (slab * P > 0xFFFFFFF0ull) { set_error("batch too large for 32-bit partition offsets"); return TQ_ERR_INVALID_ARG; }
@@ -935,17 +934,7 @@ int32_t scatter_rows_by_hash(const DCol *cols, int n_cols, int key_col, int64_t 
   sp.part_cursor = hi.as<uint32_t>();
   sp.part_lim = lim.as<uint32_t>();
   sp.overflow = d_overflow;
-  const int smem_scat = SCAT_TILE * 8 + n_bins * 12 + SCAT_TILE * 2 + SCAT_TILE;
-  static bool attr_set[5] = {};
-  if (!attr_set[n_cols]) {
-    TQ_CUDA(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)(SCAT_TILE * 11 + ((1 << PART_MAX_BITS) + 1) * 12)));
-    attr_set[n_cols] = true;
-  }
-  const int64_t tiles = (n + SCAT_TILE - 1) / SCAT_TILE;
-  const int64_t cap = (int64_t)rt().sm_count * (n_cols <= 2 ? 2 : 1);
-  kern<<<(int)(tiles < cap ? tiles : cap), SCATF_THREADS, smem_scat, s>>>(sp);
-  count_launch();
-  return check_launch("k_probe_scatter_fast");
+  return launch_scatter_fast(sp, s, "k_probe_scatter_fast");
 }
 
 // ---- partitioned probe: the partition's table image lives in shared memory ------------------------------
@@ -1377,13 +1366,7 @@ static int32_t scatter_aos(ScatterAosParams &q, DevBuf &aos, DevBuf &lo, DevBuf 
   TQ_TRY(lim.reserve((size_t)(P + 3) * 4));
   k_init_slabs<<<(P + 1 + 255) / 256, 256, 0, s>>>(lo.as<uint32_t>(), hi.as<uint32_t>(), lim.as<uint32_t>(), P, (uint32_t)slab, 0u);
   count_launch();
-  auto aligned = [](const void *ptr) { return (reinterpret_cast<uintptr_t>(ptr) & 15) == 0; };
-  q.use_tma = 1;
-  for (int c = 0; c < nc; c++) {
-    if (!aligned(q.sp.in[c].data)) q.use_tma = 0;
-    for (int g = 0; g < q.n_segs; g++)
-      if (!aligned(q.seg_in[g][c])) q.use_tma = 0;
-  }
+  set_use_tma(q);
   q.sp.part_cursor = hi.as<uint32_t>();
   q.sp.part_lim = lim.as<uint32_t>();
   q.out = aos.as<uint64_t>();
@@ -2063,7 +2046,7 @@ struct HoleRuns {
   uint32_t *t_start, *t_off;   // [n_parts], [n_parts + 1]: the i-th page at or above M: its real rows there, likewise
 };
 __global__ void __launch_bounds__(HOLE_PAD_THREADS) k_hole_pages(const PosPages m, int n_parts, unsigned long long *cur, const HoleRuns h) {
-  __shared__ uint32_t s_warp[33];
+  __shared__ uint32_t s_warp[HOLE_PAD_THREADS / 32 + 1];
   __shared__ uint32_t s_fill[HOLE_PAD_THREADS];
   const int q = threadIdx.x;
   const uint64_t M = cur[0], PG = m.page_rows;
@@ -2078,9 +2061,11 @@ __global__ void __launch_bounds__(HOLE_PAD_THREADS) k_hole_pages(const PosPages 
     const uint64_t h_hi = (last + 1) * PG < M ? (last + 1) * PG : M;
     n_h = h_hi > h_lo ? (uint32_t)(h_hi - h_lo) : 0u;
   }
-  uint32_t rows, n_holes;
-  block_excl_scan(c, s_warp, &rows);
-  const uint32_t h_off = block_excl_scan(n_h, s_warp, &n_holes);
+  block_excl_scan<HOLE_PAD_THREADS>(c, s_warp);
+  const uint32_t rows = s_warp[HOLE_PAD_THREADS / 32];
+  __syncthreads();   // s_warp is scanned again
+  const uint32_t h_off = block_excl_scan<HOLE_PAD_THREADS>(n_h, s_warp);
+  const uint32_t n_holes = s_warp[HOLE_PAD_THREADS / 32];
   if (q == 0) {
     cur[6] = rows;                    // rows the scatter placed: == M iff no probe row missed
     cur[5] = n_holes;                 // holes to fill
@@ -2103,8 +2088,8 @@ __global__ void __launch_bounds__(HOLE_PAD_THREADS) k_hole_pages(const PosPages 
     t_lo = pb > M ? pb : M;
     n_t = pb + s_fill[q] > t_lo ? (uint32_t)(pb + s_fill[q] - t_lo) : 0u;
   }
-  uint32_t n_tail_rows;
-  const uint32_t t_off = block_excl_scan(n_t, s_warp, &n_tail_rows);   // == n_holes
+  const uint32_t t_off = block_excl_scan<HOLE_PAD_THREADS>(n_t, s_warp);
+  const uint32_t n_tail_rows = s_warp[HOLE_PAD_THREADS / 32];   // == n_holes
   if (q < n_parts) {
     h.t_start[q] = (uint32_t)t_lo;
     h.t_off[q] = (uint64_t)q < n_tail ? t_off : n_tail_rows;   // (past the tail pages: no row, never found)
@@ -2368,7 +2353,7 @@ static int32_t launch_probe(tq_join *j, const std::vector<DCol> &probe, const ui
     if (!attr_done) {
       TQ_CUDA(cudaFuncSetAttribute(k_probe_part, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)PART_MAX_SMEM_BYTES));
       TQ_CUDA(cudaFuncSetAttribute(k_probe_part_uniq, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)PART_MAX_SMEM_BYTES));
-      TQ_CUDA(cudaFuncSetAttribute(k_probe_scatter, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)(SCAT_TILE * 11 + ((1 << PART_MAX_BITS) + 1) * 12)));
+      TQ_CUDA(cudaFuncSetAttribute(k_probe_scatter, cudaFuncAttributeMaxDynamicSharedMemorySize, scatter_smem_bytes((1 << PART_MAX_BITS) + 1)));
       TQ_CUDA(cudaFuncSetAttribute(k_probe_part_hist, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)(((1 << PART_MAX_BITS) + 1) * 4)));
       attr_done = true;
     }
@@ -2409,7 +2394,6 @@ static int32_t launch_probe(tq_join *j, const std::vector<DCol> &probe, const ui
       p.probe[c].bm = sp.out[c].bm;
     }
     const int smem_bins = n_bins * 4;
-    const int smem_scat = SCAT_TILE * 8 + n_bins * 12 + SCAT_TILE * 2 + SCAT_TILE;
     if (optimistic) {
       DevBuf &lim = j->part_lim[cursor_slot];
       TQ_TRY(lim.reserve((size_t)(n_bins + 1) * 4));
@@ -2434,22 +2418,15 @@ static int32_t launch_probe(tq_join *j, const std::vector<DCol> &probe, const ui
       p.part_hi = off.as<uint32_t>() + 1;
       p.part_lim = nullptr;
     }
-    const int64_t scat_tiles = (n + SCAT_TILE - 1) / SCAT_TILE;
-    const int64_t scat_cap = (int64_t)rt().sm_count * 4;
-    ScatterKernel sfast = (!any_in_bm && !g_no_fast_kernel) ? scatter_fast_kernel(j->n_probe_cols) : nullptr;
-    if (sfast) {
-      static bool sattr[5] = {};
-      if (!sattr[j->n_probe_cols]) {
-        TQ_CUDA(cudaFuncSetAttribute(sfast, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)(SCAT_TILE * 11 + ((1 << PART_MAX_BITS) + 1) * 12)));
-        sattr[j->n_probe_cols] = true;
-      }
-      const int64_t fcap = (int64_t)rt().sm_count * (j->n_probe_cols <= 2 ? 2 : 1);
-      sfast<<<(int)(scat_tiles < fcap ? scat_tiles : fcap), SCATF_THREADS, smem_scat, s>>>(sp);
+    if (!any_in_bm && !g_no_fast_kernel && j->n_probe_cols <= 4) {
+      TQ_TRY(launch_scatter_fast(sp, s, "k_probe_scatter_fast"));
     } else {
-      k_probe_scatter<<<(int)(scat_tiles < scat_cap ? scat_tiles : scat_cap), SCAT_THREADS, smem_scat, s>>>(sp);
+      const int64_t scat_tiles = (n + SCAT_TILE - 1) / SCAT_TILE;
+      const int64_t scat_cap = (int64_t)rt().sm_count * 4;
+      k_probe_scatter<<<(int)(scat_tiles < scat_cap ? scat_tiles : scat_cap), SCAT_THREADS, scatter_smem_bytes(n_bins), s>>>(sp);
+      count_launch();
+      TQ_TRY(check_launch("k_probe_scatter"));
     }
-    count_launch();
-    TQ_TRY(check_launch("k_probe_scatter"));
     p.selected = nullptr;
     const int work_parts = p.is_outer ? n_bins : P;
     // ~g_tiles_per_cta tiles per CTA: enough CTAs per partition that only a handful of partitions are live at once
@@ -3722,16 +3699,33 @@ int32_t tq_partition_count_device(const tq_column *key, int64_t n, int32_t n_par
   return TQ_OK;
 }
 
+// The push scatter of n rows of n_cols NOT NULL columns by column key_col into n_parts destinations: checks the arguments
+// the pushes share and fills sp up to the cursors, limits and overflow flag, which each push sets up itself.
+// dest_data[q * n_cols + c] = column c of destination q.  `fn` names the entry point in errors.
+static int32_t push_scatter_params(const char *fn, int32_t n_cols, const tq_column *cols, int32_t key_col, int64_t n, int32_t n_parts,
+                                   void *const *dest_data, ScatterParams &sp) {
+  if (!cols || !dest_data || n_cols < 1 || n_cols > 4 || key_col < 0 || key_col >= n_cols) { set_error("%s: 1..4 columns", fn); return TQ_ERR_INVALID_ARG; }
+  TQ_TRY(part_common_check(n_parts, n));
+  for (int c = 0; c < n_cols; c++)
+    if (cols[c].null_bitmap) { set_error("%s: columns with NULL bitmaps are not supported (use tq_partition_device)", fn); return TQ_ERR_UNSUPPORTED_TYPE; }
+  sp = ScatterParams{};
+  sp.n_cols = n_cols;
+  sp.key_col = key_col;
+  sp.key_mode = KEYMODE_RAW;
+  sp.n = n;
+  sp.n_parts_mod = n_parts;
+  for (int c = 0; c < n_cols; c++) sp.in[c].data = (const uint64_t *)cols[c].data;
+  for (int q = 0; q < n_parts; q++)
+    for (int c = 0; c < n_cols; c++) sp.out_bin[q][c] = (uint64_t *)dest_data[q * n_cols + c];
+  return TQ_OK;
+}
+
 static int32_t partition_push(int32_t n_cols, const tq_column *cols, int32_t key_col, int64_t n, int32_t n_parts, void *const *dest_data,
                               const int64_t *dest_row_offsets, bool async) {
   TQ_TRY(ensure_init());
-  if (!cols || !dest_data || !dest_row_offsets || n_cols < 1 || n_cols > 4 || key_col < 0 || key_col >= n_cols) {
-    set_error("tq_partition_push_device: 1..4 columns");
-    return TQ_ERR_INVALID_ARG;
-  }
-  TQ_TRY(part_common_check(n_parts, n));
-  for (int c = 0; c < n_cols; c++)
-    if (cols[c].null_bitmap) { set_error("tq_partition_push_device: columns with NULL bitmaps are not supported (use tq_partition_device)"); return TQ_ERR_UNSUPPORTED_TYPE; }
+  if (!dest_row_offsets) { set_error("tq_partition_push_device: 1..4 columns"); return TQ_ERR_INVALID_ARG; }
+  ScatterParams sp;
+  TQ_TRY(push_scatter_params("tq_partition_push_device", n_cols, cols, key_col, n, n_parts, dest_data, sp));
   if (n == 0) return TQ_OK;
   Runtime &r = rt();
   std::lock_guard<std::recursive_mutex> lk(r.mu);
@@ -3750,18 +3744,9 @@ static int32_t partition_push(int32_t n_cols, const tq_column *cols, int32_t key
   uint32_t *h_cur = h_cur_pin[async ? 1 : 0].as<uint32_t>();
   TQ_CUDA(cudaEventSynchronize(staged));
   memset(h_cur, 0, 64);
-  ScatterParams sp{};
-  sp.n_cols = n_cols;
-  sp.key_col = key_col;
-  sp.key_mode = KEYMODE_RAW;
-  sp.is_outer = 0;
-  sp.n = n;
-  sp.n_parts_mod = n_parts;
-  for (int c = 0; c < n_cols; c++) { sp.in[c].data = (const uint64_t *)cols[c].data; sp.in[c].bm = nullptr; sp.out[c].data = nullptr; sp.out[c].bm = nullptr; }
   for (int q = 0; q < n_parts; q++) {
     if (dest_row_offsets[q] < 0 || dest_row_offsets[q] > 0xFFFFFFF0ll) { set_error("destination offset out of range"); return TQ_ERR_INVALID_ARG; }
     h_cur[q] = (uint32_t)dest_row_offsets[q];
-    for (int c = 0; c < n_cols; c++) sp.out_bin[q][c] = (uint64_t *)dest_data[q * n_cols + c];
   }
   TQ_CUDA(cudaMemcpyAsync(cursor.p, h_cur, 64, cudaMemcpyHostToDevice, s));
   TQ_CUDA(cudaEventRecord(staged, s));
@@ -3770,19 +3755,7 @@ static int32_t partition_push(int32_t n_cols, const tq_column *cols, int32_t key
   static DevBuf ovf;
   TQ_TRY(ovf.reserve(8));
   sp.overflow = ovf.as<unsigned long long>();
-  ScatterKernel k = scatter_fast_kernel(n_cols);
-  static bool attr[5] = {};
-  if (!attr[n_cols]) {
-    TQ_CUDA(cudaFuncSetAttribute(k, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)(SCAT_TILE * 11 + ((1 << PART_MAX_BITS) + 1) * 12)));
-    attr[n_cols] = true;
-  }
-  const int n_bins = n_parts + 1;
-  const int smem = SCAT_TILE * 8 + n_bins * 12 + SCAT_TILE * 2 + SCAT_TILE;
-  const int64_t tiles = (n + SCAT_TILE - 1) / SCAT_TILE;
-  const int64_t cap = (int64_t)r.sm_count * (n_cols <= 2 ? 2 : 1);
-  k<<<(int)(tiles < cap ? tiles : cap), SCATF_THREADS, smem, s>>>(sp);
-  count_launch();
-  TQ_TRY(check_launch("k_probe_scatter_fast(push)"));
+  TQ_TRY(launch_scatter_fast(sp, s, "k_probe_scatter_fast(push)"));
   if (!async) TQ_CUDA(cudaStreamSynchronize(s));
   return TQ_OK;
 }
@@ -3846,14 +3819,12 @@ static PushSlot g_push_slot[PUSH_SLOTS];
 int32_t tq_partition_push_regions(int32_t n_cols, const tq_column *cols, int32_t key_col, int64_t n, int32_t n_parts, void *const *dest_data,
                                   void *const *dest_counts, int64_t region_cap, int32_t slot, uint64_t epoch) {
   TQ_TRY(ensure_init());
-  if (!cols || !dest_data || !dest_counts || n_cols < 1 || n_cols > 4 || key_col < 0 || key_col >= n_cols || slot < 0 || slot >= PUSH_SLOTS || region_cap < 1 ||
-      region_cap > 0xFFFFFFF0ll) {
+  if (!dest_counts || slot < 0 || slot >= PUSH_SLOTS || region_cap < 1 || region_cap > 0xFFFFFFF0ll) {
     set_error("tq_partition_push_regions: 1..4 columns, slot 0..%d", PUSH_SLOTS - 1);
     return TQ_ERR_INVALID_ARG;
   }
-  TQ_TRY(part_common_check(n_parts, n));
-  for (int c = 0; c < n_cols; c++)
-    if (cols[c].null_bitmap) { set_error("tq_partition_push_regions: columns with NULL bitmaps are not supported"); return TQ_ERR_UNSUPPORTED_TYPE; }
+  ScatterParams sp;
+  TQ_TRY(push_scatter_params("tq_partition_push_regions", n_cols, cols, key_col, n, n_parts, dest_data, sp));
   Runtime &r = rt();
   std::lock_guard<std::recursive_mutex> lk(r.mu);
   cudaStream_t s = r.h2d;  // the push stream: rows cross NVLink while the compute stream joins what has already arrived
@@ -3873,31 +3844,10 @@ int32_t tq_partition_push_regions(int32_t n_cols, const tq_column *cols, int32_t
   TQ_CUDA(cudaMemcpyAsync(ps.lim.p, ps.h_lim.p, 64, cudaMemcpyHostToDevice, s));
   TQ_CUDA(cudaMemcpyAsync(ps.counts_ptrs.p, ps.h_ptrs.p, 64, cudaMemcpyHostToDevice, s));
   if (n > 0) {
-    ScatterParams sp{};
-    sp.n_cols = n_cols;
-    sp.key_col = key_col;
-    sp.key_mode = KEYMODE_RAW;
-    sp.n = n;
-    sp.n_parts_mod = n_parts;
-    for (int c = 0; c < n_cols; c++) { sp.in[c].data = (const uint64_t *)cols[c].data; sp.in[c].bm = nullptr; }
-    for (int q = 0; q < n_parts; q++)
-      for (int c = 0; c < n_cols; c++) sp.out_bin[q][c] = (uint64_t *)dest_data[q * n_cols + c];
     sp.part_cursor = ps.cursor.as<uint32_t>();
     sp.part_lim = ps.lim.as<uint32_t>();
     sp.overflow = ps.ovf.as<unsigned long long>();
-    ScatterKernel k = scatter_fast_kernel(n_cols);
-    static bool attr[5] = {};
-    if (!attr[n_cols]) {
-      TQ_CUDA(cudaFuncSetAttribute(k, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)(SCAT_TILE * 11 + ((1 << PART_MAX_BITS) + 1) * 12)));
-      attr[n_cols] = true;
-    }
-    const int n_bins = n_parts + 1;
-    const int smem = SCAT_TILE * 8 + n_bins * 12 + SCAT_TILE * 2 + SCAT_TILE;
-    const int64_t tiles = (n + SCAT_TILE - 1) / SCAT_TILE;
-    const int64_t cap = (int64_t)r.sm_count * (n_cols <= 2 ? 2 : 1);
-    k<<<(int)(tiles < cap ? tiles : cap), SCATF_THREADS, smem, s>>>(sp);
-    count_launch();
-    TQ_TRY(check_launch("k_probe_scatter_fast(push regions)"));
+    TQ_TRY(launch_scatter_fast(sp, s, "k_probe_scatter_fast(push regions)"));
   }
   k_publish_counts<<<1, 32, 0, s>>>(ps.cursor.as<uint32_t>(), ps.ovf.as<unsigned long long>(), n_parts, ps.counts_ptrs.as<unsigned long long *>(), epoch);
   count_launch();

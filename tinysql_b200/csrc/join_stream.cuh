@@ -69,6 +69,17 @@ struct ScatterAosParams {
   const uint64_t *seg_in[SA_MAX_SEGS][4];
 };
 
+// q.use_tma: whether every input column (of every segment) is 16-byte aligned, as the TMA bulk copies of whole tiles require.
+static void set_use_tma(ScatterAosParams &q) {
+  auto aligned = [](const void *ptr) { return (reinterpret_cast<uintptr_t>(ptr) & 15) == 0; };
+  q.use_tma = 1;
+  for (int c = 0; c < q.sp.n_cols; c++) {
+    if (!aligned(q.sp.in[c].data)) q.use_tma = 0;
+    for (int g = 0; g < q.n_segs; g++)
+      if (!aligned(q.seg_in[g][c])) q.use_tma = 0;
+  }
+}
+
 template <int T>
 __host__ __device__ constexpr int sa_smem_bytes(int nc, int bins) {
   // 2 input stages + AoS staging + destination row per sorted position + 4 bin tables (4 bytes per bin each) + 2 mbarriers
@@ -103,7 +114,7 @@ __global__ void __launch_bounds__(SA_THREADS, sa_occ<T>(NC)) k_scatter_aos(const
   __shared__ uint32_t s_warp[SA_WARPS + 1];
   __shared__ uint32_t s_ovf;                                                   // some bin of this tile overflowed its slab
 
-  const int tid = threadIdx.x, lane = tid & 31, warp = tid >> 5;
+  const int tid = threadIdx.x;
   const int kc = p.key_col;
   const int64_t n_tiles = q.n_segs ? (int64_t)q.n_segs * q.seg_tiles : (p.n + T - 1) / T;
   const int bpt = (n_bins + SA_THREADS - 1) / SA_THREADS;
@@ -193,19 +204,7 @@ __global__ void __launch_bounds__(SA_THREADS, sa_occ<T>(NC)) k_scatter_aos(const
       const int b = tid * bpt + j;
       if (b < n_bins) tsum += s_hist[b];
     }
-    uint32_t inc = tsum;
-#pragma unroll
-    for (int d = 1; d < 32; d <<= 1) { const uint32_t x = __shfl_up_sync(0xffffffffu, inc, d); if (lane >= d) inc += x; }
-    if (lane == 31) s_warp[warp] = inc;
-    __syncthreads();
-    if (warp == 0) {
-      uint32_t w = (lane < SA_WARPS) ? s_warp[lane] : 0, winc = w;
-#pragma unroll
-      for (int d = 1; d < 32; d <<= 1) { const uint32_t x = __shfl_up_sync(0xffffffffu, winc, d); if (lane >= d) winc += x; }
-      if (lane < SA_WARPS) s_warp[lane] = winc - w;
-    }
-    __syncthreads();
-    uint32_t run = inc - tsum + s_warp[warp];
+    uint32_t run = block_excl_scan<SA_THREADS>(tsum, s_warp);
     for (int j = 0; j < bpt; j++) {
       const int b = tid * bpt + j;
       if (b < n_bins) {
@@ -305,29 +304,6 @@ static int32_t launch_scatter_aos(const ScatterAosParams &q, int nc, cudaStream_
 }
 
 // ------------------------------------------------------------------------------------------------ positional probe
-// exclusive scan of one value per thread over a CTA of up to 1024 threads (s_warp: 33 words); returns the prefix, *total = the sum
-__device__ __forceinline__ uint32_t block_excl_scan(uint32_t v, uint32_t *s_warp, uint32_t *total) {
-  const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5, n_warps = (blockDim.x + 31) >> 5;
-  uint32_t inc = v;
-#pragma unroll
-  for (int d = 1; d < 32; d <<= 1) { const uint32_t x = __shfl_up_sync(0xffffffffu, inc, d); if (lane >= d) inc += x; }
-  if (lane == 31) s_warp[warp] = inc;
-  __syncthreads();
-  if (warp == 0) {
-    const uint32_t w = lane < n_warps ? s_warp[lane] : 0u;
-    uint32_t winc = w;
-#pragma unroll
-    for (int d = 1; d < 32; d <<= 1) { const uint32_t x = __shfl_up_sync(0xffffffffu, winc, d); if (lane >= d) winc += x; }
-    if (lane < n_warps) s_warp[lane] = winc - w;
-    if (lane == 31) s_warp[32] = winc;
-  }
-  __syncthreads();
-  const uint32_t res = inc - v + s_warp[warp];
-  *total = s_warp[32];
-  __syncthreads();
-  return res;
-}
-
 // The paged result of a positional batch.  The result's slots are cut into pages of page_rows slots (whole probe tiles); a
 // page belongs to one partition.  Partition q's rows take VIRTUAL slots 0, 1, ... (cursor[q] counts them); its virtual page k
 // is physical page pt[q * kmax + k], and physical page i holds result slots [i * page_rows, (i + 1) * page_rows).
@@ -391,15 +367,14 @@ __global__ void __launch_bounds__(POS_BASES_THREADS) k_pos_reset(uint32_t *curso
 // partition (so its table stays in L2 while they run).
 static constexpr int PP_CHUNK_TILES = 11;       // probe tiles per CTA (~8K rows): enough CTAs per partition that only a handful of partitions are live at once
 __global__ void __launch_bounds__(POS_BASES_THREADS) k_pos_pages(const PosPages m, int n_parts, int tile_rows, unsigned long long *span) {
-  __shared__ uint32_t s_warp[33];
+  __shared__ uint32_t s_warp[POS_BASES_THREADS / 32 + 1];
   const int q = threadIdx.x;
   const uint32_t c = q < n_parts ? m.cursor[q] : 0u;
   const uint32_t tiles = (c + (uint32_t)tile_rows - 1) / (uint32_t)tile_rows;
-  uint32_t ctas;
-  const uint32_t first = block_excl_scan((tiles + PP_CHUNK_TILES - 1) / PP_CHUNK_TILES, s_warp, &ctas);
+  const uint32_t first = block_excl_scan<POS_BASES_THREADS>((tiles + PP_CHUNK_TILES - 1) / PP_CHUNK_TILES, s_warp);
   if (q < n_parts) m.chunk[q] = first;
   if (q == 0) {
-    m.chunk[n_parts] = ctas;
+    m.chunk[n_parts] = s_warp[POS_BASES_THREADS / 32];
     *span = (unsigned long long)m.cursor[n_parts] * m.page_rows;
   }
 }
@@ -439,7 +414,7 @@ __global__ void __launch_bounds__(SA_THREADS, sa_occ<T>(NC)) k_scatter_cols(cons
   uint64_t *s_mbar = reinterpret_cast<uint64_t *>(s_map + bstride);            // [2]
   __shared__ uint32_t s_warp[SA_WARPS + 1];
 
-  const int tid = threadIdx.x, lane = tid & 31, warp = tid >> 5;
+  const int tid = threadIdx.x;
   const int kc = p.key_col;
   const int64_t n_tiles = q.n_segs ? (int64_t)q.n_segs * q.seg_tiles : (p.n + T - 1) / T;
   const int bpt = (n_bins + SA_THREADS - 1) / SA_THREADS;
@@ -505,19 +480,7 @@ __global__ void __launch_bounds__(SA_THREADS, sa_occ<T>(NC)) k_scatter_cols(cons
       const int b = tid * bpt + j;
       if (b < n_bins) tsum += s_hist[b];
     }
-    uint32_t inc = tsum;
-#pragma unroll
-    for (int d = 1; d < 32; d <<= 1) { const uint32_t x = __shfl_up_sync(0xffffffffu, inc, d); if (lane >= d) inc += x; }
-    if (lane == 31) s_warp[warp] = inc;
-    __syncthreads();
-    if (warp == 0) {
-      uint32_t w = (lane < SA_WARPS) ? s_warp[lane] : 0, winc = w;
-#pragma unroll
-      for (int d = 1; d < 32; d <<= 1) { const uint32_t x = __shfl_up_sync(0xffffffffu, winc, d); if (lane >= d) winc += x; }
-      if (lane < SA_WARPS) s_warp[lane] = winc - w;
-    }
-    __syncthreads();
-    uint32_t run = inc - tsum + s_warp[warp];
+    uint32_t run = block_excl_scan<SA_THREADS>(tsum, s_warp);
     // a run that starts inside a page an earlier claim opened: that page's table entry (loaded now, awaited after placement)
     const unsigned long long *wait_e[BPT];
     unsigned long long wait_v[BPT];
@@ -641,13 +604,7 @@ static int32_t launch_pos_scatter(ScatterAosParams &q, int64_t seg_rows, const P
   TQ_TRY(check_launch("k_pos_reset"));
   const int64_t tiles = q.n_segs ? (int64_t)q.n_segs * (seg_rows / T) : (q.sp.n + T - 1) / T, cap = (int64_t)rt().sm_count * per_sm;
   q.seg_tiles = (int)(seg_rows / T);
-  auto aligned = [](const void *ptr) { return (reinterpret_cast<uintptr_t>(ptr) & 15) == 0; };
-  q.use_tma = 1;
-  for (int c = 0; c < nc; c++) {
-    if (!aligned(q.sp.in[c].data)) q.use_tma = 0;
-    for (int g = 0; g < q.n_segs; g++)
-      if (!aligned(q.seg_in[g][c])) q.use_tma = 0;
-  }
+  set_use_tma(q);
   k<<<(int)(tiles < cap ? (tiles < 1 ? 1 : tiles) : cap), SA_THREADS, smem, s>>>(q, m);
   TQ_TRY(check_launch("k_scatter_cols"));
   k_pos_pages<<<1, POS_BASES_THREADS, 0, s>>>(m, P, PP_TILE_ROWS, span);
