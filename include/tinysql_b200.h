@@ -370,7 +370,8 @@ int32_t tq_join_probe_eof(tq_join *j);
  * peers' tq_partition_push_regions kernels).  cols[g * n_probe_cols + c] = column c of region g (NOT NULL 8-byte columns,
  * `length` ignored); *seg_counts[g] = the rows region g holds — a DEVICE value, read by the kernels, never by the host, so no
  * host synchronisation sits between the exchange and the join; seg_cap = rows a region can hold.  Inner PK-FK joins on the
- * streaming path only (TQ_ERR_UNSUPPORTED_TYPE otherwise: read the counts and use tq_join_put_probe per region).
+ * streaming path only (TQ_ERR_UNSUPPORTED_TYPE otherwise: read the regions with tq_region_gather and use tq_join_put_probe,
+ * which is also how outer joins and nullable columns pushed by tq_partition_push_regions_masked are joined).
  * The call only enqueues the batch: the regions and their counts must stay unchanged until the batch is finalised, i.e.
  * until the next tq_join_put_probe / _put_probe_segments, tq_join_probe_eof, or the tq_join_next* call that returns its
  * rows.  Skewed probe keys that overflow a partition slab are still joined: the batch is then re-run on the exact
@@ -596,7 +597,8 @@ int32_t tq_partition_device(int32_t n_cols, const tq_column *cols, const int32_t
 
 /* Fused scatter + exchange over NVLink peer memory (one process per GPU, buffers shared through CUDA IPC):
  *   tq_partition_count_device  rows of `key` per destination partition (hash >> 40) % n_parts, n_parts <= 8; rows whose
- *                              key is NULL are not counted / exchanged (they cannot match in an inner join);
+ *                              key is NULL are not counted / exchanged (they cannot match in an inner join; outer joins and
+ *                              nullable columns go through tq_partition_push_regions_masked below);
  *   tq_partition_push_device   scatters every row straight into partition q's destination columns
  *                              dest_data[q * n_cols + c] (device pointers, local or PEER-mapped) starting at row
  *                              dest_row_offsets[q]; the offsets come from an all-gather of the counts.
@@ -630,6 +632,34 @@ int32_t tq_partition_push_sync(int32_t slot);
  * `slots` (this rank's own table) carry `epoch` — the device-side barrier between the peers' pushes and the kernels that read
  * the regions; no host synchronisation, no NCCL call on the data path. */
 int32_t tq_region_wait(const void *slots, int32_t n_sources, uint64_t epoch);
+/* The push of an outer join's probe side and of nullable columns (SURVEY §8(e): NULL-key rows never match; an inner join
+ * drops them before the exchange, an outer join emits their miss rows on the rank that holds them).  Same regions, slots,
+ * slot numbers and epochs as tq_partition_push_regions, plus:
+ *  - cols may carry NULL bitmaps.  If any does, the side travels with one more column, the mask word: bit c of a row's
+ *    word = column c is NOT NULL.  Wire columns per row = n_cols (+ 1 with the mask, which comes last):
+ *    dest_data[q * n_wire + c].  At most 4 wire columns: 3 nullable or 4 NOT NULL columns; a wider side is refused with
+ *    TQ_ERR_UNSUPPORTED_TYPE before anything is pushed.
+ *  - selected: n DEVICE bytes of 0/1 (the outer-side filter) or NULL = all selected.
+ *  - A row can match when its key is NOT NULL and it is selected; it goes to rank (mix64(key) >> 40) % n_parts.  Any other
+ *    row is dropped, or with keep_misses != 0 (the probe side of an outer join) written to this rank's miss_data[c]
+ *    (n_wire local device columns of miss_cap rows), whose count is published at the 16-byte slot miss_count like a
+ *    peer's; such a row never crosses a link.
+ *  - Overflow of any region or of the miss columns makes every slot this push publishes read ~0.
+ * The receiver reads them with tq_region_gather and joins them with tq_join_put_build / tq_join_put_probe (TQ_MEM_DEVICE):
+ * the kept miss rows as one more probe batch whose host `selected` is all zeros. */
+int32_t tq_partition_push_regions_masked(int32_t n_cols, const tq_column *cols, int32_t key_col, int64_t n, int32_t n_parts,
+                                         const uint8_t *selected, int32_t keep_misses, void *const *dest_data, void *const *dest_counts,
+                                         int64_t region_cap, void *const *miss_data, void *miss_count, int64_t miss_cap, int32_t slot,
+                                         uint64_t epoch);
+/* Receives n_regions (1..8) regions into one set of contiguous DEVICE columns, on the compute stream (queue tq_region_wait
+ * first).  slots: the n_regions consecutive published {u64 rows, u64 epoch} slots, read on the device; regions[g * n_wire + c]
+ * = wire column c of region g (n_wire = n_cols + has_mask; the mask word, when has_mask, is the last).  out_cols[c].data
+ * holds out_cap rows; out_cols[c].null_bitmap, when not NULL, is a device bitmap for out_cap rows and receives the mask's bit
+ * c (whole 64-row groups, bits past the last row 0), or all ones without a mask.  Rows keep region order.  Returns the rows in
+ * *n_rows and every out_cols[c].length (one host read).  A slot reading more than region_cap (~0: an overflowed push) is
+ * TQ_ERR_OOM, more rows than out_cap TQ_ERR_INVALID_ARG; either way nothing is written to the outputs. */
+int32_t tq_region_gather(int32_t n_regions, const void *slots, int64_t region_cap, int32_t n_cols, int32_t has_mask, const tq_column *regions,
+                         tq_column *out_cols, int64_t out_cap, int64_t *n_rows);
 
 #ifdef __cplusplus
 }

@@ -654,9 +654,10 @@ struct ScatterParams {
   const uint32_t *part_lim;  // optimistic slabs: one past the last row a partition may hold (nullptr: exact offsets, cannot overflow)
   unsigned long long *overflow;  // set when a slab was too small
   // multi-GPU push scatter: partition = (hash >> 40) % n_parts_mod and partition q's rows go to out_bin[q][c] — the
-  // receive buffer of rank q, a PEER pointer mapped through CUDA IPC: the stores travel over NVLink
+  // receive buffer of rank q, a PEER pointer mapped through CUDA IPC: the stores travel over NVLink.  With is_outer the rows
+  // that cannot match go to out_bin[n_parts_mod][c], local columns of this rank.
   int n_parts_mod;
-  uint64_t *out_bin[8][4];
+  uint64_t *out_bin[9][4];
 };
 __host__ __device__ __forceinline__ int scatter_bins(const ScatterParams &p) { return (p.n_parts_mod ? p.n_parts_mod : (1 << p.pbits)) + 1; }
 __device__ __forceinline__ uint32_t scatter_pid(const ScatterParams &p, uint64_t key) {
@@ -876,7 +877,7 @@ __global__ void __launch_bounds__(SCATF_THREADS, (NP <= 2 ? 2 : 1)) k_probe_scat
       for (uint32_t i = tid; i < total; i += SCATF_THREADS) {
         const uint32_t bin = sm.spid[i];
         if (i >= sm.imax[bin]) continue;
-        uint64_t *dst = p.n_parts_mod ? p.out_bin[bin & 7][c] : out[c];
+        uint64_t *dst = p.n_parts_mod ? p.out_bin[bin][c] : out[c];
         const uint32_t d32 = sm.gdelta[bin] + i;  // 32-bit wrap-around arithmetic: (run start - local offset) + sorted position
         tqd::st_stream_u64(dst + d32, sm.stage[i]);
       }
@@ -3699,24 +3700,34 @@ int32_t tq_partition_count_device(const tq_column *key, int64_t n, int32_t n_par
   return TQ_OK;
 }
 
-// The push scatter of n rows of n_cols NOT NULL columns by column key_col into n_parts destinations: checks the arguments
-// the pushes share and fills sp up to the cursors, limits and overflow flag, which each push sets up itself.
-// dest_data[q * n_cols + c] = column c of destination q.  `fn` names the entry point in errors.
+// The push scatter of n rows of n_cols columns by column key_col into n_parts destinations: checks the arguments the pushes
+// share and fills sp up to the cursors, limits and overflow flag, which each push sets up itself.  dest_data[q * n_wire + c] =
+// column c of destination q.  `fn` names the entry point in errors.  Unless `masked`, the columns must be NOT NULL and
+// n_wire = n_cols; masked, NULL bitmaps are accepted (sp.in[c].bm, for pack_null_mask) and n_wire = n_cols + 1 when one is
+// present: the mask word is wire column n_cols, its source is set by the push.
 static int32_t push_scatter_params(const char *fn, int32_t n_cols, const tq_column *cols, int32_t key_col, int64_t n, int32_t n_parts,
-                                   void *const *dest_data, ScatterParams &sp) {
-  if (!cols || !dest_data || n_cols < 1 || n_cols > 4 || key_col < 0 || key_col >= n_cols) { set_error("%s: 1..4 columns", fn); return TQ_ERR_INVALID_ARG; }
+                                   void *const *dest_data, ScatterParams &sp, bool masked = false) {
+  if (!cols || !dest_data || n_cols < 1 || (!masked && n_cols > 4) || key_col < 0 || key_col >= n_cols) { set_error("%s: 1..4 columns", fn); return TQ_ERR_INVALID_ARG; }
   TQ_TRY(part_common_check(n_parts, n));
-  for (int c = 0; c < n_cols; c++)
-    if (cols[c].null_bitmap) { set_error("%s: columns with NULL bitmaps are not supported (use tq_partition_device)", fn); return TQ_ERR_UNSUPPORTED_TYPE; }
+  bool any_bm = false;
+  for (int c = 0; c < n_cols; c++) {
+    if (cols[c].null_bitmap && !masked) { set_error("%s: columns with NULL bitmaps are not supported (use tq_partition_device)", fn); return TQ_ERR_UNSUPPORTED_TYPE; }
+    any_bm = any_bm || cols[c].null_bitmap;
+  }
+  const int n_wire = n_cols + (any_bm ? 1 : 0);
+  if (n_wire > 4) { set_error("%s: %d columns%s: the push moves at most 4 words per row", fn, n_cols, any_bm ? " and the NULL mask word" : ""); return TQ_ERR_UNSUPPORTED_TYPE; }
   sp = ScatterParams{};
-  sp.n_cols = n_cols;
+  sp.n_cols = n_wire;
   sp.key_col = key_col;
   sp.key_mode = KEYMODE_RAW;
   sp.n = n;
   sp.n_parts_mod = n_parts;
-  for (int c = 0; c < n_cols; c++) sp.in[c].data = (const uint64_t *)cols[c].data;
+  for (int c = 0; c < n_cols; c++) {
+    sp.in[c].data = (const uint64_t *)cols[c].data;
+    sp.in[c].bm = (const uint32_t *)cols[c].null_bitmap;
+  }
   for (int q = 0; q < n_parts; q++)
-    for (int c = 0; c < n_cols; c++) sp.out_bin[q][c] = (uint64_t *)dest_data[q * n_cols + c];
+    for (int c = 0; c < n_wire; c++) sp.out_bin[q][c] = (uint64_t *)dest_data[q * n_wire + c];
   return TQ_OK;
 }
 
@@ -3810,21 +3821,26 @@ __global__ void k_region_wait(const unsigned long long *slots, int n, unsigned l
   }
 }
 struct PushSlot {
-  DevBuf cursor, lim, ovf, counts_ptrs;
+  DevBuf cursor, lim, ovf, counts_ptrs, mask, sel;
   PinBuf h_lim, h_ptrs;
   cudaEvent_t ev = nullptr;
 };
 static PushSlot g_push_slot[PUSH_SLOTS];
 
-int32_t tq_partition_push_regions(int32_t n_cols, const tq_column *cols, int32_t key_col, int64_t n, int32_t n_parts, void *const *dest_data,
-                                  void *const *dest_counts, int64_t region_cap, int32_t slot, uint64_t epoch) {
-  TQ_TRY(ensure_init());
+static int32_t push_slot_check(const char *fn, void *const *dest_counts, int64_t region_cap, int32_t slot) {
   if (!dest_counts || slot < 0 || slot >= PUSH_SLOTS || region_cap < 1 || region_cap > 0xFFFFFFF0ll) {
-    set_error("tq_partition_push_regions: 1..4 columns, slot 0..%d", PUSH_SLOTS - 1);
+    set_error("%s: 1..4 columns, slot 0..%d", fn, PUSH_SLOTS - 1);
     return TQ_ERR_INVALID_ARG;
   }
-  ScatterParams sp;
-  TQ_TRY(push_scatter_params("tq_partition_push_regions", n_cols, cols, key_col, n, n_parts, dest_data, sp));
+  return TQ_OK;
+}
+
+// Enqueues one region push of sp (filled by push_scatter_params, arguments checked by push_slot_check) on the push stream and publishes its counts: n_parts slots
+// at dest_counts, and with keep_misses the miss bin's count at miss_count.  n_cols user columns; with `pack` the mask word and
+// the effective selection are made first (pack_null_mask), otherwise `selected` is used as it is.
+static int32_t push_regions(const char *fn, ScatterParams &sp, const tq_column *cols, int32_t n_cols, bool pack, const uint8_t *selected,
+                            int32_t n_parts, void *const *dest_counts, int64_t region_cap, bool keep_misses, void *miss_count, int64_t miss_cap,
+                            int32_t slot, uint64_t epoch) {
   Runtime &r = rt();
   std::lock_guard<std::recursive_mutex> lk(r.mu);
   cudaStream_t s = r.h2d;  // the push stream: rows cross NVLink while the compute stream joins what has already arrived
@@ -3833,27 +3849,70 @@ int32_t tq_partition_push_regions(int32_t n_cols, const tq_column *cols, int32_t
   TQ_TRY(ps.cursor.reserve(64));
   TQ_TRY(ps.lim.reserve(64));
   TQ_TRY(ps.ovf.reserve(8));
-  TQ_TRY(ps.counts_ptrs.reserve(64));
+  TQ_TRY(ps.counts_ptrs.reserve(128));
   TQ_TRY(ps.h_lim.reserve(64));
-  TQ_TRY(ps.h_ptrs.reserve(64));
-  TQ_CUDA(cudaEventSynchronize(ps.ev));  // the previous push of this slot no longer reads the pinned tables below
+  TQ_TRY(ps.h_ptrs.reserve(128));
+  TQ_CUDA(cudaEventSynchronize(ps.ev));  // the previous push of this slot no longer reads the pinned tables or the mask below
+  const int n_pub = n_parts + (keep_misses ? 1 : 0);
   for (int q = 0; q < 16; q++) ps.h_lim.as<uint32_t>()[q] = (uint32_t)region_cap;
   for (int q = 0; q < n_parts; q++) ps.h_ptrs.as<void *>()[q] = dest_counts[q];
+  if (keep_misses) {
+    ps.h_lim.as<uint32_t>()[n_parts] = (uint32_t)miss_cap;
+    ps.h_ptrs.as<void *>()[n_parts] = miss_count;
+    sp.is_outer = 1;
+  }
   TQ_CUDA(cudaMemsetAsync(ps.cursor.p, 0, 64, s));
   TQ_CUDA(cudaMemsetAsync(ps.ovf.p, 0, 8, s));
   TQ_CUDA(cudaMemcpyAsync(ps.lim.p, ps.h_lim.p, 64, cudaMemcpyHostToDevice, s));
-  TQ_CUDA(cudaMemcpyAsync(ps.counts_ptrs.p, ps.h_ptrs.p, 64, cudaMemcpyHostToDevice, s));
-  if (n > 0) {
+  TQ_CUDA(cudaMemcpyAsync(ps.counts_ptrs.p, ps.h_ptrs.p, 128, cudaMemcpyHostToDevice, s));
+  sp.selected = selected;
+  if (sp.n > 0) {
+    if (pack) {
+      TQ_TRY(ps.mask.reserve((size_t)sp.n * 8));
+      TQ_TRY(ps.sel.reserve((size_t)sp.n));
+      TQ_TRY(pack_null_mask(sp.in, n_cols, sp.key_col, selected, sp.n, ps.mask.as<uint64_t>(), ps.sel.as<uint8_t>(), s));
+      sp.selected = ps.sel.as<uint8_t>();
+      if (sp.n_cols > n_cols) sp.in[n_cols] = DCol{ps.mask.as<uint64_t>(), nullptr};
+    }
     sp.part_cursor = ps.cursor.as<uint32_t>();
     sp.part_lim = ps.lim.as<uint32_t>();
     sp.overflow = ps.ovf.as<unsigned long long>();
     TQ_TRY(launch_scatter_fast(sp, s, "k_probe_scatter_fast(push regions)"));
   }
-  k_publish_counts<<<1, 32, 0, s>>>(ps.cursor.as<uint32_t>(), ps.ovf.as<unsigned long long>(), n_parts, ps.counts_ptrs.as<unsigned long long *>(), epoch);
+  k_publish_counts<<<1, 32, 0, s>>>(ps.cursor.as<uint32_t>(), ps.ovf.as<unsigned long long>(), n_pub, ps.counts_ptrs.as<unsigned long long *>(), epoch);
   count_launch();
   TQ_TRY(check_launch("k_publish_counts"));
   TQ_CUDA(cudaEventRecord(ps.ev, s));
   return TQ_OK;
+}
+
+int32_t tq_partition_push_regions(int32_t n_cols, const tq_column *cols, int32_t key_col, int64_t n, int32_t n_parts, void *const *dest_data,
+                                  void *const *dest_counts, int64_t region_cap, int32_t slot, uint64_t epoch) {
+  TQ_TRY(ensure_init());
+  TQ_TRY(push_slot_check("tq_partition_push_regions", dest_counts, region_cap, slot));
+  ScatterParams sp;
+  TQ_TRY(push_scatter_params("tq_partition_push_regions", n_cols, cols, key_col, n, n_parts, dest_data, sp));
+  return push_regions("tq_partition_push_regions", sp, cols, n_cols, false, nullptr, n_parts, dest_counts, region_cap, false, nullptr, 0, slot, epoch);
+}
+
+int32_t tq_partition_push_regions_masked(int32_t n_cols, const tq_column *cols, int32_t key_col, int64_t n, int32_t n_parts,
+                                         const uint8_t *selected, int32_t keep_misses, void *const *dest_data, void *const *dest_counts,
+                                         int64_t region_cap, void *const *miss_data, void *miss_count, int64_t miss_cap, int32_t slot,
+                                         uint64_t epoch) {
+  TQ_TRY(ensure_init());
+  const char *fn = "tq_partition_push_regions_masked";
+  TQ_TRY(push_slot_check(fn, dest_counts, region_cap, slot));
+  if (keep_misses && (!miss_data || !miss_count || miss_cap < 0 || miss_cap > 0xFFFFFFF0ll)) {
+    set_error("%s: keep_misses needs miss columns, a miss slot and 0 <= miss_cap < 2^32", fn);
+    return TQ_ERR_INVALID_ARG;
+  }
+  ScatterParams sp;
+  TQ_TRY(push_scatter_params(fn, n_cols, cols, key_col, n, n_parts, dest_data, sp, true));
+  if (keep_misses) {
+    for (int c = 0; c < sp.n_cols; c++) sp.out_bin[n_parts][c] = (uint64_t *)miss_data[c];
+  }
+  const bool pack = sp.n_cols > n_cols;  // a NULL bitmap somewhere: the mask word travels, and a NULL key routes like an unselected row
+  return push_regions(fn, sp, cols, n_cols, pack, selected, n_parts, dest_counts, region_cap, keep_misses != 0, miss_count, miss_cap, slot, epoch);
 }
 
 int32_t tq_region_wait(const void *slots, int32_t n_sources, uint64_t epoch) {

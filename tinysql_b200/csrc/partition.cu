@@ -2,7 +2,9 @@
 // executor/aggregate.go:352-356): rows are split into n_parts partitions by the high bits of the key
 // hash, stable within a partition.  Three launches: per-chunk histogram, exclusive scan over
 // (partition-major, chunk-minor) counts, ordered scatter of every column.
-#include "common.cuh"
+// Also both ends of the nullable region exchange: the mask word a pushing rank packs (k_pack_null_mask) and the receiver's
+// tq_region_gather, which copies the arrived regions into contiguous columns and expands the mask word into NULL bitmaps.
+#include "scatter.cuh"
 
 namespace tq {
 
@@ -76,6 +78,98 @@ __global__ void k_part_offsets(const uint32_t *scanned, int64_t n_chunks, int n_
   if (i == n_parts) offsets[i] = n;
 }
 
+// ---- the nullable wire format of the region exchange (scatter.cuh): mask word out at the source, bitmaps back at the receiver
+static constexpr int MASK_MAXC = 4;  // the push scatter moves at most 4 words per row, the mask word included
+static constexpr int GATHER_MAX_REGIONS = 8;
+
+struct PackParams {
+  int n_cols, key_col;
+  DCol in[MASK_MAXC];
+  const uint8_t *selected;
+  int64_t n;
+  uint64_t *mask;
+  uint8_t *sel_out;
+};
+
+__global__ void __launch_bounds__(256) k_pack_null_mask(const PackParams p) {
+  for (int64_t r = (int64_t)blockIdx.x * blockDim.x + threadIdx.x; r < p.n; r += (int64_t)gridDim.x * blockDim.x) {
+    uint64_t m = 0;
+    for (int c = 0; c < p.n_cols; c++) m |= (uint64_t)tqd::bm_not_null(p.in[c].bm, r) << c;
+    p.mask[r] = m;
+    const bool sel = p.selected ? p.selected[r] != 0 : true;
+    p.sel_out[r] = (uint8_t)(sel && ((m >> p.key_col) & 1));
+  }
+}
+
+int32_t pack_null_mask(const DCol *cols, int n_cols, int key_col, const uint8_t *selected, int64_t n, uint64_t *mask, uint8_t *sel_out,
+                       cudaStream_t s) {
+  if (n_cols < 1 || n_cols > MASK_MAXC || key_col < 0 || key_col >= n_cols || n < 1) { set_error("internal: pack_null_mask arguments"); return TQ_ERR_INVALID_ARG; }
+  PackParams p{};
+  p.n_cols = n_cols;
+  p.key_col = key_col;
+  for (int c = 0; c < n_cols; c++) p.in[c] = cols[c];
+  p.selected = selected;
+  p.n = n;
+  p.mask = mask;
+  p.sel_out = sel_out;
+  const int64_t blocks = (n + 255) / 256, cap = (int64_t)rt().sm_count * 8;
+  TQ_LAUNCH(k_pack_null_mask, (unsigned)(blocks < cap ? blocks : cap), 256, 0, s, p);
+  count_launch();
+  return check_launch("k_pack_null_mask");
+}
+
+struct GatherParams {
+  int n_regions, n_cols, has_mask;  // region g holds n_cols (+ the mask word) columns
+  const unsigned long long *slots;  // n_regions x {u64 rows, u64 epoch}
+  unsigned long long region_cap, out_cap;
+  const uint64_t *src[GATHER_MAX_REGIONS][MASK_MAXC];
+  uint64_t *out[MASK_MAXC];
+  uint32_t *out_bm[MASK_MAXC];
+  unsigned long long *total;  // rows of all regions, ~0 when a slot reads more than region_cap (a region overflowed)
+};
+
+// Every thread reads the slots (through shared memory, once per CTA), so the kernel knows the row count before it writes:
+// when a region overflowed or the rows exceed out_cap it writes nothing but *total.  Rows [0, rows) are the regions in order;
+// bitmap words are written for the whole 64-row groups that hold them, with 0 for the rows past the end, so every output
+// bitmap is a complete device bitmap of `rows` rows.  A warp covers 32 consecutive rows: one ballot = one bitmap word.
+__global__ void __launch_bounds__(256) k_region_gather(const GatherParams p) {
+  __shared__ unsigned long long s_off[GATHER_MAX_REGIONS + 1];
+  __shared__ int s_ok;
+  if (threadIdx.x == 0) {
+    unsigned long long off = 0;
+    bool ok = true;
+    for (int g = 0; g < p.n_regions; g++) {
+      const unsigned long long rows = p.slots[2 * g];
+      s_off[g] = off;
+      if (rows > p.region_cap) ok = false;
+      else off += rows;
+    }
+    s_off[p.n_regions] = off;
+    if (blockIdx.x == 0) *p.total = ok ? off : ~0ull;
+    s_ok = ok && off <= p.out_cap;
+  }
+  __syncthreads();
+  if (!s_ok) return;
+  const unsigned long long rows = s_off[p.n_regions], padded = (rows + 63) & ~63ull;
+  const int lane = threadIdx.x & 31;
+  for (unsigned long long base = (unsigned long long)blockIdx.x * blockDim.x; base < padded; base += (unsigned long long)gridDim.x * blockDim.x) {
+    const unsigned long long r = base + threadIdx.x;
+    const bool live = r < rows;
+    int g = 0;
+    if (live)
+      while (r >= s_off[g + 1]) g++;
+    const unsigned long long i = live ? r - s_off[g] : 0;
+    const uint64_t m = (live && p.has_mask) ? p.src[g][p.n_cols][i] : ~0ull;
+    for (int c = 0; c < p.n_cols; c++) {
+      if (live) p.out[c][r] = p.src[g][c][i];
+      if (p.out_bm[c]) {
+        const unsigned w = __ballot_sync(0xffffffffu, live && ((m >> c) & 1));
+        if (lane == 0 && r < padded) p.out_bm[c][r >> 5] = w;
+      }
+    }
+  }
+}
+
 }  // namespace tq
 
 using namespace tq;
@@ -137,5 +231,56 @@ extern "C" int32_t tq_partition_device(int32_t n_cols, const tq_column *cols, co
   TQ_CUDA(cudaMemcpyAsync(h_off.p, d_off.p, (size_t)(n_parts + 1) * 8, cudaMemcpyDeviceToHost, s));
   TQ_CUDA(cudaStreamSynchronize(s));
   memcpy(part_offsets, h_off.p, (size_t)(n_parts + 1) * 8);
+  return TQ_OK;
+}
+
+extern "C" int32_t tq_region_gather(int32_t n_regions, const void *slots, int64_t region_cap, int32_t n_cols, int32_t has_mask,
+                                    const tq_column *regions, tq_column *out_cols, int64_t out_cap, int64_t *n_rows) {
+  TQ_TRY(ensure_init());
+  if (n_regions < 1 || n_regions > GATHER_MAX_REGIONS || !slots || region_cap < 1 || n_cols < 1 || (has_mask != 0 && has_mask != 1) ||
+      n_cols + has_mask > MASK_MAXC || !regions || !out_cols || out_cap < 0 || !n_rows) {
+    set_error("tq_region_gather: 1..%d regions, 1..%d columns with the mask word, region_cap >= 1", GATHER_MAX_REGIONS, MASK_MAXC);
+    return TQ_ERR_INVALID_ARG;
+  }
+  const int nw = n_cols + has_mask;
+  GatherParams p{};
+  p.n_regions = n_regions;
+  p.n_cols = n_cols;
+  p.has_mask = has_mask;
+  p.slots = static_cast<const unsigned long long *>(slots);
+  p.region_cap = (unsigned long long)region_cap;
+  p.out_cap = (unsigned long long)out_cap;
+  for (int g = 0; g < n_regions; g++)
+    for (int c = 0; c < nw; c++) {
+      p.src[g][c] = (const uint64_t *)regions[g * nw + c].data;
+      if (!p.src[g][c]) { set_error("tq_region_gather: region %d column %d has no data", g, c); return TQ_ERR_INVALID_ARG; }
+    }
+  for (int c = 0; c < n_cols; c++) {
+    p.out[c] = (uint64_t *)out_cols[c].data;
+    p.out_bm[c] = (uint32_t *)out_cols[c].null_bitmap;
+    if (!p.out[c]) { set_error("tq_region_gather: output column %d has no data", c); return TQ_ERR_INVALID_ARG; }
+  }
+  Runtime &r = rt();
+  std::lock_guard<std::recursive_mutex> lk(r.mu);
+  cudaStream_t s = r.compute;
+  static DevBuf d_total;
+  static PinBuf h_total;
+  TQ_TRY(d_total.reserve(8));
+  TQ_TRY(h_total.reserve(8));
+  p.total = d_total.as<unsigned long long>();
+  const int64_t blocks = (out_cap + 255) / 256, cap = (int64_t)r.sm_count * 8;
+  TQ_LAUNCH(k_region_gather, (unsigned)(blocks < 1 ? 1 : (blocks < cap ? blocks : cap)), 256, 0, s, p);
+  count_launch();
+  TQ_TRY(check_launch("k_region_gather"));
+  TQ_CUDA(cudaMemcpyAsync(h_total.p, d_total.p, 8, cudaMemcpyDeviceToHost, s));
+  TQ_CUDA(cudaStreamSynchronize(s));
+  const unsigned long long total = *h_total.as<unsigned long long>();
+  if (total == ~0ull) { set_error("tq_region_gather: a region overflowed (its slot reads more than %lld rows)", (long long)region_cap); return TQ_ERR_OOM; }
+  if (total > (unsigned long long)out_cap) {
+    set_error("tq_region_gather: %llu rows arrived, the output holds %lld", total, (long long)out_cap);
+    return TQ_ERR_INVALID_ARG;
+  }
+  for (int c = 0; c < n_cols; c++) out_cols[c].length = (int64_t)total;
+  *n_rows = (int64_t)total;
   return TQ_OK;
 }

@@ -20,4 +20,11 @@ int32_t scatter_rows_by_hash_aos(const DCol *cols, int n_cols, int key_col, int6
                                  unsigned long long *d_overflow, cudaStream_t s);
 static constexpr int SCATTER_AOS_MAX_PBITS = 9;
 
+// The wire format of a nullable side of the multi-GPU push (partition.cu, k_pack_null_mask): the push scatter moves 8-byte
+// words only, so the NULL bitmaps of a row travel as one more column, mask[r] bit c = "column c of row r is NOT NULL".
+// sel_out[r] = selected[r] (all 1 when selected is null) AND the key column of row r is NOT NULL: the push routes on it, so a
+// row with a NULL key takes the path of an unselected row.  Enqueued on s; n >= 1.
+int32_t pack_null_mask(const DCol *cols, int n_cols, int key_col, const uint8_t *selected, int64_t n, uint64_t *mask, uint8_t *sel_out,
+                       cudaStream_t s);
+
 }  // namespace tq

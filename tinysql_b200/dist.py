@@ -372,50 +372,142 @@ class RegionJoin:
 
     wait(t) is the device-side tq_region_wait; the chunk-c join overlaps the chunk-(c+1) push.  Host synchronisation: one count
     read for the build side (tq_join_put_build takes host lengths), the result drain, and ONE barrier at the end of the step
-    (nobody may overwrite a region a peer is still joining)."""
+    (nobody may overwrite a region a peer is still joining).
 
-    def __init__(self, lib, L, world, rank, n_build_max, n_probe_max, n_chunks, slack=1.25):
-        """n_build_max / n_probe_max: the largest per-rank shard (every rank must pass the same numbers: the layout is shared)"""
+    The join is an ordinary tq_join_desc with the key in column 0 of both sides: join_type / outer_is_right as on one GPU,
+    INT64 / UINT64 / FLOAT64 columns, optional defaultInner.  An inner join of NOT NULL columns reads the regions in place
+    (tq_join_put_probe_segments).  Otherwise (an outer join, or a side declared nullable) the pushes are
+    tq_partition_push_regions_masked: a nullable side carries the mask word, the probe rows of an outer join that cannot
+    match (NULL key, selected == 0) stay on this rank, and the receiver copies each table's regions into contiguous columns
+    with tq_region_gather before tq_join_put_build / tq_join_put_probe; the kept rows are one more probe batch, unselected."""
+
+    def __init__(self, lib, L, world, rank, n_build_max, n_probe_max, n_chunks, slack=1.25, join_type=0, outer_is_right=True,
+                 build_types=None, probe_types=None, build_nullable=False, probe_nullable=False, default_inner=None):
+        """n_build_max / n_probe_max: the largest per-rank shard (every rank must pass the same numbers: the layout is shared).
+        build_types / probe_types: TQ_TYPE_* per column (default two INT64 columns).  *_nullable: that side may carry NULL
+        bitmaps.  default_inner: the inner side of a miss row, one value (int or float) or None per build column."""
         self.lib, self.L, self.world, self.rank, self.n_chunks = lib, L, world, rank, n_chunks
+        self.join_type, self.outer_is_right = join_type, bool(outer_is_right)
+        self.build_types = list(build_types or (L.TQ_TYPE_INT64, L.TQ_TYPE_INT64))
+        self.probe_types = list(probe_types or (L.TQ_TYPE_INT64, L.TQ_TYPE_INT64))
+        self.default_inner = default_inner
+        self.bmask, self.pmask = int(bool(build_nullable)), int(bool(probe_nullable))
+        self.segmented = join_type == 0 and not build_nullable and not probe_nullable
+        nb, npc = len(self.build_types), len(self.probe_types)
         cap = lambda n: int(n / world * slack) + (1 << 14)   # keys are hash-spread: +25 % covers the imbalance between (source, destination) pairs
-        chunk_max = (n_probe_max + n_chunks - 1) // n_chunks
-        tables = [(2, cap(n_build_max))] + [(2, cap(chunk_max)) for c in range(n_chunks)]
+        # the gather path cuts a nullable probe side at whole 64-row bitmap groups: a chunk may be up to 63 rows longer
+        self.chunk_max = (n_probe_max + n_chunks - 1) // n_chunks + (0 if self.segmented else 64)
+        tables = [(nb + self.bmask, cap(n_build_max))] + [(npc + self.pmask, cap(self.chunk_max)) for c in range(n_chunks)]
         self.rx = RegionExchange(lib, L, world, rank, tables)
+        self._bufs = []
+        if not self.segmented:
+            rx = self.rx
+            # receive side: the build table and one probe chunk as contiguous columns (+ bitmaps), and the kept miss rows
+            self.g_build = self._cols(nb, world * rx.cap[0], self.bmask)
+            self.g_probe = self._cols(npc, world * rx.cap[1], self.pmask)
+            self.outer = join_type != 0
+            if self.outer:
+                self.g_miss = self._cols(npc, self.chunk_max, self.pmask)
+                # this rank's miss rows of chunk c: wire columns of chunk_max rows and a 16-byte {rows, epoch} slot
+                nw = npc + self.pmask
+                self.miss_data = [[self._alloc(max(self.chunk_max, 1) * 8) for _ in range(nw)] for _ in range(n_chunks)]
+                self.miss_slot = [self._alloc(16, zero=True) for _ in range(n_chunks)]
+
+    def _alloc(self, nbytes, zero=False):
+        p = C.c_void_p()
+        self.L.check(self.lib.tq_device_alloc(nbytes, C.byref(p)))
+        self._bufs.append(p.value)
+        if zero:
+            self.L.check(self.lib.tq_memset_device(p, 0, nbytes))
+            self.L.check(self.lib.tq_device_synchronize())
+        return p.value
+
+    def _ones(self, n):
+        """a device NOT-NULL-everywhere bitmap of at least n rows"""
+        if getattr(self, "_ones_rows", 0) < n:
+            nbytes = ((n + 63) // 64) * 8 + 8
+            self._ones_ptr, self._ones_rows = self._alloc(nbytes), n
+            self.L.check(self.lib.tq_memset_device(C.c_void_p(self._ones_ptr), 0xFF, nbytes))
+            self.L.check(self.lib.tq_device_synchronize())
+        return self._ones_ptr
+
+    def _cols(self, ncols, rows, nullable):
+        """ncols device columns of `rows` rows for tq_region_gather, with device bitmaps when nullable"""
+        arr = (self.L.TQColumn * ncols)()
+        for c in range(ncols):
+            arr[c].data = self._alloc(max(rows, 1) * 8)
+            arr[c].null_bitmap = self._alloc(((rows + 63) // 64) * 8 + 8) if nullable else None
+        return arr, rows
 
     def close(self):
         self.rx.close()
+        for p in self._bufs:
+            self.lib.tq_device_free(C.c_void_p(p))
+        self._bufs = []
+
+    def _desc(self):
+        L = self.L
+        tb = (C.c_int32 * len(self.build_types))(*self.build_types)
+        tp = (C.c_int32 * len(self.probe_types))(*self.probe_types)
+        k = (C.c_int32 * 1)(0)
+        dbits = dnn = None
+        if self.default_inner is not None:
+            vals = [0 if v is None else int(np.array([v], dtype=np.float64 if t == L.TQ_TYPE_FLOAT64 else (np.uint64 if t == L.TQ_TYPE_UINT64 else np.int64)).view(np.uint64)[0])
+                    for v, t in zip(self.default_inner, self.build_types)]
+            dbits = (C.c_uint64 * len(vals))(*vals)
+            dnn = (C.c_uint8 * len(vals))(*[0 if v is None else 1 for v in self.default_inner])
+        d = L.TQJoinDesc(self.join_type, 1 if self.outer_is_right else 0, len(self.build_types), tb, len(self.probe_types), tp, 1, k, k, 0, 0,
+                         C.cast(dbits, C.POINTER(C.c_uint64)) if dbits is not None else None, C.cast(dnn, C.POINTER(C.c_uint8)) if dnn is not None else None)
+        return d, (tb, tp, k, dbits, dnn)
 
     def step(self, bk, bv, pk, pv, keep_result=False):
         """bk / bv / pk / pv: this rank's row shards as (device pointer, rows)-like objects.  Returns (rows, stats, result)."""
+        return self.step_cols([bk, bv], [pk, pv], keep_result=keep_result)
+
+    def step_cols(self, build, probe, build_bitmaps=None, probe_bitmaps=None, selected=None, keep_result=False):
+        """build / probe: this rank's shard of every column ((device pointer, rows)-like objects, key = column 0).
+        *_bitmaps: a device NULL bitmap pointer (or None) per column, on a side declared nullable.  selected: device bytes
+        (0/1, one per probe row: the outer-side filter) or None.  Returns (rows, stats, result); result (keep_result) is a
+        list of numpy value arrays on the segmented path, of host chunk Columns (with their NULLs) otherwise."""
         lib, L, rx, w = self.lib, self.L, self.rx, self.world
+        if self.segmented and (build_bitmaps or probe_bitmaps or selected is not None):
+            raise ValueError("RegionJoin: NULL bitmaps need build_nullable / probe_nullable, selected[] an outer join")
         t_start = time.perf_counter()
         trace = []
         mark = lambda name: trace.append((name, (time.perf_counter() - t_start) * 1e3))   # host-side timeline: where the host blocks
-        n_probe = int(pk.numel())
+        n_build, n_probe = int(build[0].numel()), int(probe[0].numel())
         bounds = [n_probe * i // self.n_chunks for i in range(self.n_chunks + 1)]
+        if not self.segmented:
+            bounds = [min(n_probe, (b + 63) // 64 * 64) for b in bounds]
         rx.next_epoch()
-        rx.push(0, [bk, bv], int(bk.numel()), 0)
+        self._push(0, build, build_bitmaps, None, n_build, 0, 0)
         for c in range(self.n_chunks):
             lo, hi = bounds[c], bounds[c + 1]
-            rx.push(1 + c, [RawCol(pk.data_ptr() + lo * 8, hi - lo), RawCol(pv.data_ptr() + lo * 8, hi - lo)], hi - lo, 1 + c)
+            self._push(1 + c, [RawCol(x.data_ptr() + lo * 8, hi - lo) for x in probe], probe_bitmaps, selected, hi - lo, 1 + c, lo, chunk=c)
         mark("pushes enqueued")
-        # ---- build side: the only place the host needs row counts
-        cnt_b = rx.counts(0)
-        mark("build rows arrived (host read)")
-        t = (C.c_int32 * 2)(1, 1)
-        k = (C.c_int32 * 1)(0)
-        d = L.TQJoinDesc(0, 1, 2, t, 2, t, 1, k, k, 0, 0)
+        n_out = len(self.build_types) + len(self.probe_types)
+        d, keep = self._desc()
         h = C.c_void_p()
         L.check(lib.tq_join_create(C.byref(d), C.byref(h)))
         total, result, st = 0, None, (C.c_int64 * 8)()
+        out_types = (self.build_types + self.probe_types) if self.outer_is_right else (self.probe_types + self.build_types)
         try:
-            for g in range(w):
-                if cnt_b[g]:
-                    cols = [RawCol(rx.region_ptr(self.rank, 0, g, c), cnt_b[g]) for c in range(2)]
-                    L.check(lib.tq_join_put_build(h, _tq_cols(L, cols, cnt_b[g]), L.TQ_MEM_DEVICE))
+            if self.segmented:
+                # ---- build side: the only place the host needs row counts
+                cnt_b = rx.counts(0)
+                mark("build rows arrived (host read)")
+                for g in range(w):
+                    if cnt_b[g]:
+                        cols = [RawCol(rx.region_ptr(self.rank, 0, g, c), cnt_b[g]) for c in range(len(self.build_types))]
+                        L.check(lib.tq_join_put_build(h, _tq_cols(L, cols, cnt_b[g]), L.TQ_MEM_DEVICE))
+            else:
+                rows = self._gather(0, self.g_build, self.bmask)
+                if rows:
+                    L.check(lib.tq_join_put_build(h, self.g_build[0], L.TQ_MEM_DEVICE))
+                mark("build rows arrived (gathered)")
             L.check(lib.tq_join_finalize_build(h))
             mark("build done")
-            out = (L.TQColumn * 4)()
+            out = (L.TQColumn * n_out)()
             n, eof = C.c_int64(0), C.c_int32(0)
             chunks = []
 
@@ -428,24 +520,43 @@ class RegionJoin:
                     total += n.value
                     if keep_result:
                         from .chunk import device_to_host
-                        chunks.append([device_to_host(1, out[c].data, None, n.value).values for c in range(4)])
+                        if self.segmented:
+                            chunks.append([device_to_host(1, out[c].data, None, n.value).values for c in range(n_out)])
+                        else:
+                            chunks.append([device_to_host(out_types[c], out[c].data, out[c].null_bitmap, n.value) for c in range(n_out)])
                     if not final:
                         return
             for c in range(self.n_chunks):
-                rx.wait(1 + c)                                   # device-side: chunk c has landed from every source
-                cols, cnts = rx.segment_args(1 + c)
-                st_ = lib.tq_join_put_probe_segments(h, w, cols, cnts, rx.cap[1 + c])
-                L.check(st_)
-                mark(f"chunk {c} enqueued")
-                if c >= 1:
-                    drain(False)                                 # hand back the batch before last (keeps two result sets alive, not n_chunks)
-                    mark(f"chunk {c - 1} drained")
+                if self.segmented:
+                    rx.wait(1 + c)                                   # device-side: chunk c has landed from every source
+                    cols, cnts = rx.segment_args(1 + c)
+                    L.check(lib.tq_join_put_probe_segments(h, w, cols, cnts, rx.cap[1 + c]))
+                    mark(f"chunk {c} enqueued")
+                    if c >= 1:
+                        drain(False)                                 # hand back the batch before last (keeps two result sets alive, not n_chunks)
+                        mark(f"chunk {c - 1} drained")
+                    continue
+                # gather path: a put borrows its columns until its batch is finished, so the chunk is drained before the
+                # next one reuses the gather buffers
+                if self._gather(1 + c, self.g_probe, self.pmask):
+                    L.check(lib.tq_join_put_probe(h, self.g_probe[0], None, L.TQ_MEM_DEVICE))
+                if self.outer:
+                    m = self._gather_misses(c)
+                    if m:
+                        zeros = np.zeros(m, np.uint8)
+                        L.check(lib.tq_join_put_probe(h, self.g_miss[0], zeros.ctypes.data, L.TQ_MEM_DEVICE))
+                drain(True)
+                mark(f"chunk {c} joined")
             L.check(lib.tq_join_probe_eof(h))
             drain(True)
             mark("all drained")
             lib.tq_join_stats(h, st)
             if keep_result:
-                result = [np.concatenate([ch[c] for ch in chunks]) if chunks else np.zeros(0, np.int64) for c in range(4)]
+                if self.segmented:
+                    result = [np.concatenate([ch[c] for ch in chunks]) if chunks else np.zeros(0, np.int64) for c in range(n_out)]
+                else:
+                    from .chunk import Chunk, Column
+                    result = Chunk.concat([Chunk(ch) for ch in chunks], out_types).cols if chunks else [Column.empty(t, 0) for t in out_types]
         finally:
             lib.tq_join_destroy(h)
         rx.check_all_counts()                                    # a region overflow would have dropped rows: fail loudly
@@ -454,6 +565,57 @@ class RegionJoin:
         mark("barrier")
         self.last_trace = trace
         return total, list(st), result
+
+    def _push(self, t, cols, bitmaps, selected, n, slot, row0, chunk=None):
+        """push this rank's rows of table t; on the masked path bitmaps / selected are taken from row row0 on"""
+        rx = self.rx
+        if self.segmented:
+            rx.push(t, cols, n, slot)
+            return
+        L, w, nw = self.L, self.world, rx.ncols[t]
+        nc = nw - (self.bmask if t == 0 else self.pmask)
+        arr = _tq_cols(self.L, cols, n)
+        for c, b in enumerate(bitmaps or []):
+            arr[c].null_bitmap = None if b is None else b + row0 // 8
+        if nw > nc and n and not any(arr[c].null_bitmap for c in range(nc)):
+            arr[0].null_bitmap = self._ones(n)          # a side declared nullable always carries the mask word: the layout is shared
+        dest = (C.c_void_p * (w * nw))()
+        cnts = (C.c_void_p * w)()
+        for d in range(w):
+            for c in range(nw):
+                dest[d * nw + c] = rx.region_ptr(d, t, rx.rank, c)
+            cnts[d] = rx.slot_ptr(d, t, rx.rank)
+        keep = t > 0 and self.outer
+        miss = (C.c_void_p * nw)(*self.miss_data[chunk]) if keep else None
+        sel = None if (t == 0 or selected is None) else selected.data_ptr() + row0
+        L.check(self.lib.tq_partition_push_regions_masked(nc, arr, 0, n, w, sel, int(keep), dest, cnts, rx.cap[t], miss,
+                                                          self.miss_slot[chunk] if keep else None, self.chunk_max, slot, rx.epoch))
+
+    def _gather(self, t, target, has_mask):
+        """wait (device-side) for table t from every source and copy its regions into target; returns the rows"""
+        rx, L, w = self.rx, self.L, self.world
+        rx.wait(t)
+        nw = rx.ncols[t]
+        regs = (L.TQColumn * (w * nw))()
+        for g in range(w):
+            for c in range(nw):
+                regs[g * nw + c].data = rx.region_ptr(self.rank, t, g, c)
+        n = C.c_int64(0)
+        L.check(self.lib.tq_region_gather(w, C.c_void_p(rx.slot_ptr(self.rank, t, 0)), rx.cap[t], nw - has_mask, has_mask, regs, target[0], target[1], C.byref(n)))
+        return n.value
+
+    def _gather_misses(self, c):
+        """this rank's kept probe rows of chunk c (published by its own push) as contiguous columns; returns the rows"""
+        L = self.L
+        nw = len(self.probe_types) + self.pmask
+        L.check(self.lib.tq_region_wait(C.c_void_p(self.miss_slot[c]), 1, self.rx.epoch))
+        regs = (L.TQColumn * nw)()
+        for k in range(nw):
+            regs[k].data = self.miss_data[c][k]
+        n = C.c_int64(0)
+        L.check(self.lib.tq_region_gather(1, C.c_void_p(self.miss_slot[c]), max(self.chunk_max, 1), len(self.probe_types), self.pmask, regs,
+                                          self.g_miss[0], self.g_miss[1], C.byref(n)))
+        return n.value
 
 
 def gen_dist_tables(rank, world, n_b, n_p):
