@@ -371,7 +371,7 @@ int32_t tq_join_probe_eof(tq_join *j);
  * `length` ignored); *seg_counts[g] = the rows region g holds — a DEVICE value, read by the kernels, never by the host, so no
  * host synchronisation sits between the exchange and the join; seg_cap = rows a region can hold.  Inner PK-FK joins on the
  * streaming path only (TQ_ERR_UNSUPPORTED_TYPE otherwise: read the regions with tq_region_gather and use tq_join_put_probe,
- * which is also how outer joins and nullable columns pushed by tq_partition_push_regions_masked are joined).
+ * which is also how outer joins and nullable columns pushed by tq_partition_push_regions are joined).
  * The call only enqueues the batch: the regions and their counts must stay unchanged until the batch is finalised, i.e.
  * until the next tq_join_put_probe / _put_probe_segments, tq_join_probe_eof, or the tq_join_next* call that returns its
  * rows.  Skewed probe keys that overflow a partition slab are still joined: the batch is then re-run on the exact
@@ -595,62 +595,49 @@ int32_t tq_partition_device(int32_t n_cols, const tq_column *cols, const int32_t
                             int32_t key_col, int64_t n, int32_t n_parts, tq_column *out_cols,
                             int64_t *part_offsets);
 
-/* Fused scatter + exchange over NVLink peer memory (one process per GPU, buffers shared through CUDA IPC):
- *   tq_partition_count_device  rows of `key` per destination partition (hash >> 40) % n_parts, n_parts <= 8; rows whose
- *                              key is NULL are not counted / exchanged (they cannot match in an inner join; outer joins and
- *                              nullable columns go through tq_partition_push_regions_masked below);
- *   tq_partition_push_device   scatters every row straight into partition q's destination columns
- *                              dest_data[q * n_cols + c] (device pointers, local or PEER-mapped) starting at row
- *                              dest_row_offsets[q]; the offsets come from an all-gather of the counts.
- * Columns must be NOT NULL (no bitmaps), n_cols <= 4. */
 /* Kernel-level load/store access from this process's device to `peer_device` (cudaDeviceEnablePeerAccess): required
- * before tq_partition_push_device is handed PEER pointers. */
+ * before tq_partition_push_regions is handed PEER pointers. */
 int32_t tq_enable_peer_access(int32_t peer_device);
 /* CUDA IPC (cudaIpcGetMemHandle / OpenMemHandle / CloseMemHandle) for buffers from tq_device_alloc: a rank exports its
  * receive buffer as a 64-byte handle; peers open it under THEIR device and push rows into it over NVLink. */
 int32_t tq_ipc_get_handle(void *dev_ptr, void *handle64);
 int32_t tq_ipc_open_handle(const void *handle64, void **dev_ptr);
 int32_t tq_ipc_close_handle(void *dev_ptr);
-int32_t tq_partition_count_device(const tq_column *key, int64_t n, int32_t n_parts, int64_t *counts);
-int32_t tq_partition_push_device(int32_t n_cols, const tq_column *cols, int32_t key_col, int64_t n, int32_t n_parts,
-                                 void *const *dest_data, const int64_t *dest_row_offsets);
-/* Same, enqueued on the library's second stream and not waited for: lets the probe rows cross NVLink while the hash
- * table is being built on the compute stream; tq_partition_push_wait blocks until the push has completed. */
-int32_t tq_partition_push_device_async(int32_t n_cols, const tq_column *cols, int32_t key_col, int64_t n, int32_t n_parts,
-                                       void *const *dest_data, const int64_t *dest_row_offsets);
-int32_t tq_partition_push_wait(void);
-/* Push into per-source REGIONS (no count exchange before the push): destination q reserves `region_cap` rows per source rank and
- * column; dest_data[q * n_cols + c] = the start of THIS rank's region for column c on rank q (local or PEER pointer),
- * dest_counts[q] = where to publish (as one u64, ~0 = region overflow) how many rows this rank wrote there.  Enqueued on the
- * library's push stream; tq_partition_push_sync(slot) waits for that push (slots 0..15 may be in flight together).  The
- * receiver joins its regions with tq_join_put_probe_segments after a cross-rank barrier. */
-int32_t tq_partition_push_regions(int32_t n_cols, const tq_column *cols, int32_t key_col, int64_t n, int32_t n_parts, void *const *dest_data,
-                                  void *const *dest_counts, int64_t region_cap, int32_t slot, uint64_t epoch);
-int32_t tq_partition_push_sync(int32_t slot);
-/* dest_counts[q] points at a 16-byte slot {u64 rows, u64 epoch}: the count is published first, the epoch after a system-scope
- * fence.  tq_region_wait enqueues, on the compute stream, a kernel that waits (bounded) until the n_sources consecutive slots at
- * `slots` (this rank's own table) carry `epoch` — the device-side barrier between the peers' pushes and the kernels that read
- * the regions; no host synchronisation, no NCCL call on the data path. */
-int32_t tq_region_wait(const void *slots, int32_t n_sources, uint64_t epoch);
-/* The push of an outer join's probe side and of nullable columns (SURVEY §8(e): NULL-key rows never match; an inner join
- * drops them before the exchange, an outer join emits their miss rows on the rank that holds them).  Same regions, slots,
- * slot numbers and epochs as tq_partition_push_regions, plus:
- *  - cols may carry NULL bitmaps.  If any does, the side travels with one more column, the mask word: bit c of a row's
- *    word = column c is NOT NULL.  Wire columns per row = n_cols (+ 1 with the mask, which comes last):
- *    dest_data[q * n_wire + c].  At most 4 wire columns: 3 nullable or 4 NOT NULL columns; a wider side is refused with
- *    TQ_ERR_UNSUPPORTED_TYPE before anything is pushed.
+/* Fused scatter + exchange over NVLink peer memory (one process per GPU, buffers shared through CUDA IPC): the push into
+ * per-source REGIONS, with no count exchange before it.  Destination q reserves `region_cap` rows per source rank and wire
+ * column; this rank scatters each of its n rows straight into its region on rank (mix64(key) >> 40) % n_parts and then
+ * publishes, per destination, how many rows it wrote there.
+ *  - n_parts 1..8, n < 2^32, 0 <= key_col < n_cols, 1 <= region_cap < 2^32.
+ *  - cols may carry NULL bitmaps (SURVEY §8(e): NULL-key rows never match; an inner join drops them before the exchange,
+ *    an outer join emits their miss rows on the rank that holds them).  If any does, the side travels with one more column,
+ *    the mask word: bit c of a row's word = column c is NOT NULL.  Wire columns per row: n_wire = n_cols (+ 1 with the mask,
+ *    which comes last).  At most 4 wire columns: 3 nullable or 4 NOT NULL columns; a wider side is TQ_ERR_UNSUPPORTED_TYPE.
+ *  - dest_data[q * n_wire + c] = the start of THIS rank's region for wire column c on rank q (local or PEER pointer).
+ *  - dest_counts[q] points at a 16-byte slot {u64 rows, u64 epoch} on rank q: the count is published first (~0 = overflow),
+ *    the epoch after a system-scope fence.
  *  - selected: n DEVICE bytes of 0/1 (the outer-side filter) or NULL = all selected.
- *  - A row can match when its key is NOT NULL and it is selected; it goes to rank (mix64(key) >> 40) % n_parts.  Any other
- *    row is dropped, or with keep_misses != 0 (the probe side of an outer join) written to this rank's miss_data[c]
- *    (n_wire local device columns of miss_cap rows), whose count is published at the 16-byte slot miss_count like a
- *    peer's; such a row never crosses a link.
+ *  - A row can match when its key is NOT NULL and it is selected.  Any other row is dropped, or with keep_misses != 0 (the
+ *    probe side of an outer join) written to this rank's miss_data[c] (n_wire local device columns of miss_cap rows, 0 <=
+ *    miss_cap < 2^32), whose count is published at the 16-byte slot miss_count like a peer's; such a row never crosses a link.
  *  - Overflow of any region or of the miss columns makes every slot this push publishes read ~0.
- * The receiver reads them with tq_region_gather and joins them with tq_join_put_build / tq_join_put_probe (TQ_MEM_DEVICE):
- * the kept miss rows as one more probe batch whose host `selected` is all zeros. */
-int32_t tq_partition_push_regions_masked(int32_t n_cols, const tq_column *cols, int32_t key_col, int64_t n, int32_t n_parts,
-                                         const uint8_t *selected, int32_t keep_misses, void *const *dest_data, void *const *dest_counts,
-                                         int64_t region_cap, void *const *miss_data, void *miss_count, int64_t miss_cap, int32_t slot,
-                                         uint64_t epoch);
+ * A NOT NULL inner-join push passes selected = NULL, keep_misses = 0 and no miss buffers.  This signature replaced a
+ * 10-argument NOT NULL-only form; against it two refusals changed: NULL bitmaps are accepted (were TQ_ERR_UNSUPPORTED_TYPE),
+ * and more than 4 wire columns is TQ_ERR_UNSUPPORTED_TYPE (was TQ_ERR_INVALID_ARG).
+ * Every argument is checked before anything is enqueued: a refused push writes no region and publishes no slot.  The push is
+ * enqueued on the library's push stream; tq_partition_push_sync(slot) waits for it (slots 0..15 may be in flight together).
+ * The receiver waits with tq_region_wait, then joins an inner join of NOT NULL columns in place with
+ * tq_join_put_probe_segments, and everything else by copying the regions out with tq_region_gather and joining them with
+ * tq_join_put_build / tq_join_put_probe (TQ_MEM_DEVICE): the kept miss rows as one more probe batch whose host `selected` is
+ * all zeros. */
+int32_t tq_partition_push_regions(int32_t n_cols, const tq_column *cols, int32_t key_col, int64_t n, int32_t n_parts,
+                                  const uint8_t *selected, int32_t keep_misses, void *const *dest_data, void *const *dest_counts,
+                                  int64_t region_cap, void *const *miss_data, void *miss_count, int64_t miss_cap, int32_t slot,
+                                  uint64_t epoch);
+int32_t tq_partition_push_sync(int32_t slot);
+/* Enqueues, on the compute stream, a kernel that waits (bounded) until the n_sources consecutive slots at `slots` (this rank's
+ * own table) carry `epoch` — the device-side barrier between the peers' pushes and the kernels that read the regions; no host
+ * synchronisation, no NCCL call on the data path. */
+int32_t tq_region_wait(const void *slots, int32_t n_sources, uint64_t epoch);
 /* Receives n_regions (1..8) regions into one set of contiguous DEVICE columns, on the compute stream (queue tq_region_wait
  * first).  slots: the n_regions consecutive published {u64 rows, u64 epoch} slots, read on the device; regions[g * n_wire + c]
  * = wire column c of region g (n_wire = n_cols + has_mask; the mask word, when has_mask, is the last).  out_cols[c].data

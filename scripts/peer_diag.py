@@ -25,20 +25,26 @@ def step(name, f):
     except Exception as e:
         print(rank, name, "FAILED", str(e)[:200], flush=True); raise
 step("memset peer via lib", lambda: L.check(lib.tq_memset_device(C.c_void_p(pt.data_ptr()), 1, 64)))
-loc = torch.arange(4096, dtype=torch.int64, device=dev)
-# push with everything local first, then with the peer as partition 1
+dist.barrier()
+# one region push of 10000 rows into 2 destinations: this rank's own buffer (destination 0) and the peer's (destination 1).
+# Every buffer holds a {rows, epoch} slot per source at its start and, from byte 4096, 2 region columns of CAP rows per source.
+CAP = 20000
+slot_of = lambda base, src: base + 16 * src
+region_of = lambda base, src, c: base + 4096 + (src * 2 + c) * CAP * 8
 k = torch.arange(10000, dtype=torch.int64, device=dev); v = k * 2
-def push(dst_ptrs):
+def push():
     cols = (L.TQColumn * 2)()
     for i, t in enumerate((k, v)):
         cols[i].length, cols[i].data, cols[i].null_bitmap, cols[i].offsets = 10000, t.data_ptr(), None, None
-    dest = (C.c_void_p * 4)(*dst_ptrs)
-    offs = (C.c_int64 * 2)(0, 0)
-    L.check(lib.tq_partition_push_device(2, cols, 0, 10000, 2, dest, offs))
-l0, l1, l2, l3 = [torch.zeros(20000, dtype=torch.int64, device=dev) for _ in range(4)]
-step("push all-local", lambda: push([l0.data_ptr(), l1.data_ptr(), l2.data_ptr(), l3.data_ptr()]))
+    dest = (C.c_void_p * 4)(*[region_of(b, rank, c) for b in (own.value, pp.value) for c in range(2)])
+    cnts = (C.c_void_p * 2)(slot_of(own.value, rank), slot_of(pp.value, rank))
+    L.check(lib.tq_partition_push_regions(2, cols, 0, 10000, 2, None, 0, dest, cnts, CAP, None, None, 0, 0, 1))
+    L.check(lib.tq_partition_push_sync(0))
+step("region push, destination 1 = peer", push)
 dist.barrier()
-step("push part1->peer", lambda: push([l0.data_ptr(), l1.data_ptr(), pt.data_ptr(), pt.data_ptr() + 8 * 20000]))
-dist.barrier()
-hostbuf = np.zeros(40000, np.int64); L.check(lib.tq_memcpy_d2h(hostbuf.ctypes.data, own, 320000)); print(rank, "received sum", int(hostbuf.sum()), flush=True)
+src = (rank - 1) % world   # the rank whose destination 1 is this rank
+hostslot = np.zeros(2, np.uint64); L.check(lib.tq_memcpy_d2h(hostslot.ctypes.data, C.c_void_p(slot_of(own.value, src)), 16))
+rows = int(hostslot[0]); received = np.zeros(2 * CAP, np.int64)
+L.check(lib.tq_memcpy_d2h(received.ctypes.data, C.c_void_p(region_of(own.value, src, 0)), 2 * CAP * 8))
+print(rank, "received from", src, "rows", rows, "epoch", int(hostslot[1]), "sum", int(received[:rows].sum() + received[CAP:CAP + rows].sum()), flush=True)
 dist.destroy_process_group()

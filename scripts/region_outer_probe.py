@@ -1,9 +1,9 @@
 """Cost of the outer-join / nullable path of the region exchange on ONE GPU with W emulated ranks (all receive buffers in
 this GPU's memory), on the per-rank C5 shape (12.5M build / 125M probe rows per rank by default, uniform keys, every probe row
 matches once).  W sources push into one destination, which times, with CUDA events:
-  masked : tq_partition_push_regions_masked of every source (probe side: LEFT OUTER, keep_misses, a NULL bitmap on the
-           payload column so the mask word travels) -> tq_region_gather -> tq_join_put_probe of the gathered rows
-  inner  : tq_partition_push_regions (NOT NULL) -> tq_join_put_probe_segments over the regions in place
+  masked : tq_partition_push_regions of every source (probe side: LEFT OUTER, keep_misses, a NULL bitmap on the payload
+           column so the mask word travels) -> tq_region_gather -> tq_join_put_probe of the gathered rows
+  inner  : tq_partition_push_regions of NOT NULL columns -> tq_join_put_probe_segments over the regions in place
 on the same data and the same build table (every rank's build shard), and checks every output row of both (B.v = 7 B.k + 1,
 B.k = P.k = mix64(P.v) % N_build, as many rows as probe rows).  Prints one JSON line with the card name and power limit.
 
@@ -110,12 +110,11 @@ def main():
                 nw = 3 if masked else 2
                 dest = (C.c_void_p * nw)(*[reg_ptr(s, c) for c in range(nw)])
                 cnts = (C.c_void_p * 1)(ptr(slots) + s * 16)
+                md, ms = None, None
                 if masked:
                     cols[1].null_bitmap = ptr(pv_nn)
-                    md = (C.c_void_p * 3)(*[ptr(miss) + c * 64 * 8 for c in range(3)])
-                    L.check(lib.tq_partition_push_regions_masked(2, cols, 0, npr, 1, None, 1, dest, cnts, cap, md, C.c_void_p(ptr(miss_slot)), 64, s, 1))
-                else:
-                    L.check(lib.tq_partition_push_regions(2, cols, 0, npr, 1, dest, cnts, cap, s, 1))
+                    md, ms = (C.c_void_p * 3)(*[ptr(miss) + c * 64 * 8 for c in range(3)]), C.c_void_p(ptr(miss_slot))
+                L.check(lib.tq_partition_push_regions(2, cols, 0, npr, 1, None, int(masked), dest, cnts, cap, md, ms, 64 if masked else 0, s, 1))
             for s in range(W):
                 L.check(lib.tq_partition_push_sync(s))
             e[1].record()

@@ -7,14 +7,17 @@
         outer_fast      LEFT OUTER hash join, 1e7 unique build rows x 5e7 probe rows, 2 + 2 NOT NULL INT64 columns: the
                         general partitioned probe, scattered by k_probe_scatter_fast
         outer_nullable  the same join with nullable probe columns (no NULL in them): k_probe_scatter
-        push8           tq_partition_push_device of 2e7 rows x 4 columns into 8 destinations on this GPU: k_probe_scatter_fast<4>
+        push8           tq_partition_push_regions of 2e7 rows x 4 NOT NULL columns into 8 regions on this GPU, caps from the
+                        host-side destinations: k_probe_scatter_fast<4>
         agg_part        GROUP BY of 8e6 rows into ~1.5e6 groups (SUM, COUNT, FIRSTROW over INT64): the HashAgg pre-aggregation
                         at 2^10 partitions, scattered by scatter_rows_by_hash (k_probe_scatter_fast); time = tq_agg_stats[2]
         stream_build    inner PK-FK hash join, 1e7 unique build rows x 2e7 probe rows: the streaming build (k_scatter_aos)
                         and the positional probe (k_scatter_cols); time = the whole join
   python scripts/scatter_probe.py --compare PARENT_LIB [--reps 3]
       alternates a library built from the parent commit with this tree's library, one process per run, parent first, --reps
-      times each; prints every run, the medians per case and whether rows and checksums agree between the two libraries."""
+      times each; prints every run, the medians per case and whether rows and checksums agree between the two libraries.
+      A library from before the region push had one entry point exports it, with the same arguments, under its former
+      name: tq_partition_push_regions with the suffix _masked.  Such a library is called through that name."""
 import argparse
 import ctypes as C
 import json
@@ -40,6 +43,11 @@ def load(path):
         fn = getattr(lib, name, None)
         if fn is not None:
             fn.restype, fn.argtypes = res, args
+    push = "tq_partition_push_regions"
+    former = getattr(lib, f"{push}_masked", None)      # the same push of a library from before it had one entry point
+    if former is not None:
+        former.restype, former.argtypes = L.SYMBOLS[push]
+        setattr(lib, push, former)
     L._lib = lib
     L.check(lib.tq_init(0))
     return L, lib
@@ -108,6 +116,8 @@ def case_join(L, lib, reps, join_type, n_build, n_probe, nullable):
 
 
 def case_push8(L, lib, reps):
+    from tinysql_b200.chunk import INT64, DeviceColumn
+    from tinysql_b200.dist import dest_rank_np
     n, ncols, n_parts = 20_000_000, 4, 8
     rng = np.random.default_rng(7)
     cols = [rng.integers(-(1 << 63), (1 << 63) - 1, n, dtype=np.int64)] + [np.arange(n, dtype=np.int64) * (c + 3) + c for c in range(1, ncols)]
@@ -115,25 +125,30 @@ def case_push8(L, lib, reps):
     tq = (L.TQColumn * ncols)(*[d.tq() for d in d_in])
     for c in range(ncols):
         tq[c].null_bitmap = None
-    counts = (C.c_int64 * n_parts)()
-    L.check(lib.tq_partition_count_device(tq, n, n_parts, counts))
-    from tinysql_b200.chunk import INT64, DeviceColumn
-    dst = [[DeviceColumn(INT64, counts[q], with_bitmap=False) for _ in range(ncols)] for q in range(n_parts)]
+    counts = np.bincount(dest_rank_np(cols[0], n_parts), minlength=n_parts)
+    cap = int(counts.max())
+    dst = [[DeviceColumn(INT64, cap, with_bitmap=False) for _ in range(ncols)] for q in range(n_parts)]
+    slots = DeviceColumn(INT64, 2 * n_parts, with_bitmap=False)
     ptrs = (C.c_void_p * (n_parts * ncols))(*[d._data.value for dq in dst for d in dq])
-    offs = (C.c_int64 * n_parts)(*([0] * n_parts))
+    cnts = (C.c_void_p * n_parts)(*[slots._data.value + 16 * q for q in range(n_parts)])
 
     def once():
         t0 = time.perf_counter()
-        L.check(lib.tq_partition_push_device(ncols, tq, 0, n, n_parts, ptrs, offs))
-        L.check(lib.tq_device_synchronize())
+        L.check(lib.tq_partition_push_regions(ncols, tq, 0, n, n_parts, None, 0, ptrs, cnts, cap, None, None, 0, 0, 1))
+        L.check(lib.tq_partition_push_sync(0))
         return time.perf_counter() - t0
 
     once()
-    sums = [str(col_sum(L, lib, d._data, d.length)) for dq in dst for d in dq]
+    pub = np.zeros(2 * n_parts, np.uint64)
+    L.check(lib.tq_memcpy_d2h(pub.ctypes.data, slots._data, pub.nbytes))
+    rows = [int(r) for r in pub[0::2]]
+    if rows != [int(c) for c in counts]:
+        raise SystemExit(f"push8: published rows {rows}, host destinations {list(counts)}")
+    sums = [str(col_sum(L, lib, d._data, rows[q])) for q, dq in enumerate(dst) for d in dq]
     times = [once() for _ in range(reps)]
-    for d in d_in + [d for dq in dst for d in dq]:
+    for d in d_in + [d for dq in dst for d in dq] + [slots]:
         d.free()
-    return times, {"rows": int(sum(counts)), "counts": list(counts), "checksums": sums}
+    return times, {"rows": sum(rows), "counts": rows, "checksums": sums}
 
 
 def case_agg(L, lib, reps):

@@ -4,8 +4,8 @@ tq_partition_device: a row goes to dest_rank_np(key) (= (mix64(key) >> 40) % n_p
 row % n_parts; the rows of a partition keep their input order (a stable argsort by destination), so data, NOT-NULL bitmaps
 and part_offsets compare bit for bit.
 
-tq_partition_count_device / _push_device / _push_regions: a row whose key is NULL is neither counted nor sent; a destination
-receives a multiset of rows (runs of a destination are claimed with atomics: the order inside it is not promised).
+tq_partition_push_regions: a row whose key is NULL is neither counted nor sent; a destination receives a multiset of rows
+(runs of a destination are claimed with atomics: the order inside it is not promised).
 
 Regions: the exchange of dist.RegionExchange with all W ranks' receive buffers in this GPU's memory.  RegionExchange itself
 needs a process group and CUDA IPC (which cannot open a handle in the process that exported it), so its layout is restated
@@ -47,7 +47,7 @@ def partition_ref(cols, nns, key_col, n_parts):
 
 
 def push_dest(keys, key_nn, n_parts):
-    """destination of every row under the count / push rule; -1 = not sent (NULL key)"""
+    """destination of every row under the push rule; -1 = not sent (NULL key)"""
     d = dest_rank_np(keys, n_parts) if len(keys) else np.zeros(0, np.int64)
     if key_nn is not None:
         d = np.where(key_nn, d, -1)
@@ -146,19 +146,24 @@ class Regions:
     def slot_ptr(self, dst, src):
         return self.buf.addr((dst * self.world + src) * 16)
 
-    def push(self, src, cols, n, slot, epoch, key_col=0):
-        """source `src` scatters its n rows (device column pointers) into its region on every destination"""
-        w, nc = self.world, self.ncols
-        dest = (C.c_void_p * (w * nc))()
+    def push(self, src, cols, n, slot, epoch, key_col=0, bitmaps=None, selected=None, miss=None, miss_slot=None, miss_cap=0):
+        """source `src` scatters its n rows (device column pointers; bitmaps: a device NULL bitmap pointer or None per
+        column) into its region on every destination.  selected: device bytes or None.  miss (ncols wire column pointers),
+        miss_slot and miss_cap keep the rows that cannot match on the source (keep_misses); without miss they are dropped."""
+        w, nw = self.world, self.ncols
+        dest = (C.c_void_p * (w * nw))()
         cnts = (C.c_void_p * w)()
         for d in range(w):
-            for c in range(nc):
-                dest[d * nc + c] = self.region_ptr(d, src, c)
+            for c in range(nw):
+                dest[d * nw + c] = self.region_ptr(d, src, c)
             cnts[d] = self.slot_ptr(d, src)
-        tq = (L.TQColumn * nc)()
-        for c in range(nc):
+        tq = (L.TQColumn * len(cols))()
+        for c in range(len(cols)):
             tq[c].length, tq[c].data = n, cols[c]
-        return self.lib.tq_partition_push_regions(nc, tq, key_col, n, w, dest, cnts, self.cap, slot, epoch)
+            tq[c].null_bitmap = bitmaps[c] if bitmaps else None
+        md = (C.c_void_p * nw)(*miss) if miss is not None else None
+        return self.lib.tq_partition_push_regions(len(cols), tq, key_col, n, w, selected, int(miss is not None), dest, cnts, self.cap, md,
+                                                  miss_slot, miss_cap, slot, epoch)
 
     def wait(self, dst, epoch):
         return self.lib.tq_region_wait(C.c_void_p(self.slot_ptr(dst, 0)), self.world, epoch)

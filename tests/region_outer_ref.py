@@ -1,5 +1,5 @@
 """Outer joins and nullable columns over the region exchange with W ranks emulated in one process (tests/exchange_ref.py's
-Regions layout): each source pushes its shards with tq_partition_push_regions_masked, each destination copies its regions
+Regions layout): each source pushes its shards with tq_partition_push_regions, each destination copies its regions
 with tq_region_gather and joins them with an ordinary join handle, as dist.RegionJoin does across processes.
 
 A shard is (cols, nns): uint64 arrays and NOT-NULL bool arrays (None = no bitmap), key = column 0.  Every output buffer a
@@ -17,7 +17,7 @@ GUARD = 64
 
 
 def routed(keys, nn, sel, n_parts):
-    """destination of every row under the masked push's rule; -1 = cannot match (NULL key or selected == 0)"""
+    """destination of every row under the push's rule; -1 = cannot match (NULL key or selected == 0)"""
     d = dest_rank_np(np.asarray(keys).view(np.int64), n_parts) if len(keys) else np.zeros(0, np.int64)
     ok = np.ones(len(keys), bool)
     if nn is not None:
@@ -74,22 +74,23 @@ class GuardedCols:
 
 
 class Source:
-    """one emulated rank's shard in device memory: columns, bitmaps (padded to 64-row groups), selected bytes"""
+    """one emulated rank's shard in device memory: column pointers, bitmap pointers (padded to 64-row groups; None = no
+    bitmap), selected bytes"""
 
     def __init__(self, lib, cols, nns, sel=None):
         self.n = len(cols[0])
-        self.bufs = []
-        self.arr = (L.TQColumn * len(cols))()
-        for c, (v, nn) in enumerate(zip(cols, nns)):
+        self.bufs, self.ptrs, self.bms = [], [], []
+        for v, nn in zip(cols, nns):
             b = X.Buf(lib, max(self.n, 1) * 8, None)
             b.put(np.asarray(v).view(np.uint64))
             self.bufs.append(b)
-            self.arr[c].length, self.arr[c].data = self.n, b.addr()
+            self.ptrs.append(b.addr())
+            self.bms.append(None)
             if nn is not None:
                 m = X.Buf(lib, ((self.n + 63) // 64) * 8 + 8, None)
                 m.put(X.bitmap_words(nn))
                 self.bufs.append(m)
-                self.arr[c].null_bitmap = m.addr()
+                self.bms[-1] = m.addr()
         self.sel = None
         if sel is not None:
             s = X.Buf(lib, max(self.n, 1), None)
@@ -102,14 +103,10 @@ class Source:
             b.free()
 
 
-def push(lib, reg, src_idx, source, ncols, slot, epoch, keep_misses=False, miss=None, miss_slot=None, miss_cap=0):
+def push(reg, src_idx, source, slot, epoch, miss=None, miss_slot=None, miss_cap=0):
     """source src_idx pushes its rows into its region on every destination of `reg` (wire columns = reg.ncols)"""
-    w, nw = reg.world, reg.ncols
-    dest = (C.c_void_p * (w * nw))(*[reg.region_ptr(d, src_idx, c) for d in range(w) for c in range(nw)])
-    cnts = (C.c_void_p * w)(*[reg.slot_ptr(d, src_idx) for d in range(w)])
-    md = (C.c_void_p * nw)(*miss) if miss is not None else None
-    return lib.tq_partition_push_regions_masked(ncols, source.arr, 0, source.n, w, source.sel, int(keep_misses), dest, cnts, reg.cap, md,
-                                                miss_slot, miss_cap, slot, epoch)
+    return reg.push(src_idx, source.ptrs, source.n, slot, epoch, bitmaps=source.bms, selected=source.sel, miss=miss, miss_slot=miss_slot,
+                    miss_cap=miss_cap)
 
 
 def gather(lib, n_regions, slots_ptr, cap, ncols, has_mask, region_ptr, out, out_cap=None):
@@ -195,9 +192,9 @@ def run(lib, W, jt, oir, btypes, ptypes, bshards, pshards, psel=None, default_in
         mslot = [X.Buf(lib, 16, 0) for _ in range(W)] if outer else []
         keep += miss + mslot
         for s in range(W):
-            L.check(push(lib, breg, s, srcs[s], nb, s, epoch))
+            L.check(push(breg, s, srcs[s], s, epoch))
             mp = [miss[s].addr(c * (max(mcap, 1) + GUARD) * 8) for c in range(nwp)] if outer else None
-            L.check(push(lib, preg, s, srcs[W + s], npc, 8 + s, epoch, outer, mp, mslot[s].addr() if outer else None, mcap))
+            L.check(push(preg, s, srcs[W + s], 8 + s, epoch, mp, mslot[s].addr() if outer else None, mcap))
         for slot in list(range(W)) + list(range(8, 8 + W)):
             L.check(lib.tq_partition_push_sync(slot))
         for d in range(W):

@@ -42,7 +42,7 @@ def test_emu_pack_null_mask(emu, n):
         src = R.Source(emu, cols, nns, sel)
         mask, sel_out = X.Buf(emu, n * 8 + 64), X.Buf(emu, n + 64)
         try:
-            dcols = (_DCol * 3)(*[_DCol(src.arr[c].data, src.arr[c].null_bitmap) for c in range(3)])
+            dcols = (_DCol * 3)(*[_DCol(src.ptrs[c], src.bms[c]) for c in range(3)])
             st = _pack_null_mask(emu)(dcols, 3, key_col, src.sel, n, mask.addr(), sel_out.addr(), None)
             assert st == L.TQ_OK
             want = sum((nn if nn is not None else np.ones(n, bool)).astype(np.uint64) << np.uint64(c) for c, nn in enumerate(nns))

@@ -4,13 +4,12 @@ exact reference of tests/exchange_ref.py:
   A. tq_partition_device (the NCCL path's and the distributed GROUP BY's partitioner): stable, NULL keys to row % n_parts,
      bitmaps carried with their rows, bit for bit at the warp-chunk (2048 rows) and block (16384 rows) edges, 1..256
      partitions and 1..16 columns; nothing written outside the outputs; FLOAT32 / BYTES columns refused.
-  B. tq_partition_count_device + tq_partition_push_device / _async: count and push agree, every destination's rows land at
-     its own offset, the guard rows around them stay intact; two async pushes queued behind a busy push stream each keep
-     their own offsets.
-  C. tq_partition_push_regions -> the published {rows, epoch} slots -> tq_region_wait, for 1..8 emulated ranks, caps that
-     fit, fit exactly and overflow by one row.
-  D. tq_join_put_probe_segments over regions filled by real pushes, in the exchange's order (push, device-side wait, join).
-  E. dist.py's device GROUP BY and join with the NCCL exchange replaced by concatenating each destination's slices.
+  B. tq_partition_push_regions -> the published {rows, epoch} slots -> tq_region_wait: every destination's rows exact with
+     the guard rows after them intact, at 0..1,100,003 rows, 1..8 destinations and 1..4 columns; NULL keys neither counted
+     nor sent; 1..8 emulated ranks with caps that fit, fit exactly and overflow by one row; two pushes queued on one slot
+     behind a busy push stream each keep their own regions and slots; every bad argument refused before anything is written.
+  C. tq_join_put_probe_segments over regions filled by real pushes, in the exchange's order (push, device-side wait, join).
+  D. dist.py's device GROUP BY and join with the NCCL exchange replaced by concatenating each destination's slices.
 
 Every buffer a wrong offset or cap could reach is a sentinel-filled part of a larger allocation, so such a bug misplaces
 rows inside an allocation and shows up in a guard.  Every tq_region_wait is queued after the pushes that satisfy it.
@@ -200,7 +199,7 @@ def test_partition_refusals(lib):
         io.free()
 
 
-# ================================================================================================ B. count / push
+# ================================================================================================ B. push_regions / publish / wait
 def _dev_cols(lib, arrays, keep):
     ptrs = []
     for a in arrays:
@@ -218,25 +217,6 @@ def _tq(ptrs, n):
     return arr
 
 
-class _PushDest:
-    """destination buffers of a push: per destination q and column, a sentinel buffer of rows[q] rows"""
-
-    def __init__(self, lib, rows, ncols, keep):
-        self.rows, self.ncols = rows, ncols
-        self.bufs = [[X.Buf(lib, r * 8) for _ in range(ncols)] for r in rows]
-        for bq in self.bufs:
-            keep.extend(bq)
-        self.ptrs = (C.c_void_p * (len(rows) * ncols))(*[b.addr() for bq in self.bufs for b in bq])
-
-    def check(self, q, off, want_rows):
-        """rows [off, off + len(want_rows)) of destination q hold want_rows (a multiset); every other row the sentinel"""
-        got = np.stack([b.get() for b in self.bufs[q]], axis=1)
-        m = len(want_rows)
-        assert np.all(got[:off] == X.SENTINEL), f"destination {q}: a row before its offset {off}"
-        assert np.all(got[off + m:] == X.SENTINEL), f"destination {q}: a row past offset + count"
-        assert np.array_equal(X.sorted_rows(got[off:off + m]), want_rows), f"destination {q}: rows differ"
-
-
 def _push_data(rng, n, ncols, key_col, first_id):
     cols = [np.arange(first_id, first_id + n, dtype=np.int64) * (c + 3) + c for c in range(ncols)]
     k = rng.integers(-(1 << 63), (1 << 63) - 1, n, dtype=np.int64)
@@ -246,11 +226,41 @@ def _push_data(rng, n, ncols, key_col, first_id):
     return cols
 
 
-@pytest.mark.parametrize("n", [4095, 4096, 4097, 1_100_003])
-def test_count_and_push_agree(lib, n):
-    """1..8 destinations, 1..4 columns with the key first or last; counts with a nullable key skip the NULLs; every
-    destination gets its rows at its own nonzero offset with guards before and after (1,100,003 rows: more 4096-row tiles than the
-    capped grid of 2 x 132 CTAs, so the CTAs loop)"""
+def _check_source(reg, s, cols, dest, epoch):
+    """source s's slot and region on every destination after a push that did not overflow: dest[i] = where row i went
+    (-1 = not sent); each region holds exactly those rows (a multiset, whole rows) and the sentinel past them"""
+    for d in range(reg.world):
+        idx = np.flatnonzero(dest == d)
+        assert reg.slots(d)[s] == (len(idx), epoch), f"slot ({d}, {s})"
+        got = np.stack([reg.region(d, s, c) for c in range(reg.ncols)], axis=1)
+        assert np.all(got[len(idx):] == X.SENTINEL), f"region ({d}, {s}): a row past its count"
+        assert np.array_equal(X.sorted_rows(got[:len(idx)]), X.rows_of(cols, idx)), f"region ({d}, {s}) rows"
+
+
+def _push_one_source(lib, cols, ptrs, key_col, n_parts, key_nn=None, key_bm=None):
+    """one source pushes every row into n_parts destinations whose regions fit exactly; with key_bm (the device bitmap of
+    key_nn) on the key column the mask word travels as the last wire column and says NOT NULL for every sent row"""
+    n = len(cols[0])
+    dest = X.push_dest(cols[key_col], key_nn, n_parts)
+    cap = max(int(np.bincount(dest[dest >= 0], minlength=n_parts).max()) if n else 0, 1)
+    mask = [] if key_bm is None else [np.full(n, (1 << len(cols)) - 1, np.uint64)]
+    reg = X.Regions(lib, n_parts, len(cols) + len(mask), cap, guard=GUARD)
+    try:
+        bms = None if key_bm is None else [key_bm if c == key_col else None for c in range(len(cols))]
+        L.check(reg.push(0, ptrs, n, 0, 5, key_col, bms))
+        L.check(lib.tq_partition_push_sync(0))
+        _check_source(reg, 0, cols + mask, dest, 5)
+        assert all(reg.slots(d)[1:] == [(0, 0)] * (n_parts - 1) for d in range(n_parts)), "a slot of another source was written"
+    finally:
+        reg.free()
+
+
+@pytest.mark.parametrize("n", [0, 1, 4095, 4096, 4097, 1_100_003])
+def test_push_regions_rows_exact(lib, n):
+    """1..8 destinations, 1..4 columns with the key first or last: every destination's region holds exactly the rows (key
+    and payload together) whose key maps to it (1,100,003 rows: more 4096-row tiles than the capped grid of 2 x 132 CTAs,
+    so the CTAs loop).  Then the same rows with a bitmap on the key (at most 3 columns: the mask word is the 4th): a row
+    whose key is NULL is neither counted nor sent"""
     rng = np.random.default_rng(n)
     keep = []
     try:
@@ -259,29 +269,14 @@ def test_count_and_push_agree(lib, n):
             key_col = 0 if n_parts % 2 else ncols - 1
             cols = _push_data(rng, n, ncols, key_col, 0)
             ptrs = _dev_cols(lib, cols, keep)
+            _push_one_source(lib, cols, ptrs, key_col, n_parts)
             nn = rng.random(n) >= 0.25
             bm = X.Buf(lib, ((n + 63) // 64) * 8 + 8, None)
             keep.append(bm)
             bm.put(X.bitmap_words(nn))
-            key = _tq([ptrs[key_col]], n)
-            key[0].null_bitmap = bm.addr()
-            counts = (C.c_int64 * n_parts)()
-            L.check(lib.tq_partition_count_device(key, n, n_parts, counts))
-            d_nn = X.push_dest(cols[key_col], nn, n_parts)
-            assert list(counts) == list(np.bincount(d_nn[d_nn >= 0], minlength=n_parts)), "count with NULL keys"
-            key[0].null_bitmap = None
-            L.check(lib.tq_partition_count_device(key, n, n_parts, counts))
-            d = X.push_dest(cols[key_col], None, n_parts)
-            assert list(counts) == list(np.bincount(d, minlength=n_parts))
-            offs = [17 + 29 * q for q in range(n_parts)]
-            dst = _PushDest(lib, [offs[q] + counts[q] + GUARD for q in range(n_parts)], ncols, keep)
-            tq = _tq(ptrs, n)
-            L.check(lib.tq_partition_push_device(ncols, tq, key_col, n, n_parts, dst.ptrs, (C.c_int64 * n_parts)(*offs)))
-            for q in range(n_parts):
-                dst.check(q, offs[q], X.rows_of(cols, np.flatnonzero(d == q)))
-            tq[0].null_bitmap = bm.addr()
-            for push in (lib.tq_partition_push_device, lib.tq_partition_push_device_async):
-                assert push(ncols, tq, key_col, n, n_parts, dst.ptrs, (C.c_int64 * n_parts)(*offs)) == L.TQ_ERR_UNSUPPORTED_TYPE
+            m = min(ncols, 3)
+            sub = slice(0, m) if key_col == 0 else slice(ncols - m, ncols)
+            _push_one_source(lib, cols[sub], ptrs[sub], 0 if key_col == 0 else m - 1, n_parts, nn, bm.addr())
             for b in keep:
                 b.free()
             keep.clear()
@@ -290,42 +285,80 @@ def test_count_and_push_agree(lib, n):
             b.free()
 
 
-def test_back_to_back_async_pushes_keep_their_offsets(lib):
-    """two tq_partition_push_device_async calls with different offsets, queued behind pushes that keep the push stream busy:
-    the second call must not change the offsets the first one scatters at.  Each destination buffer has room for either
-    offset set and all n rows, so a push at the wrong offsets (or to the wrong destination) misplaces rows inside its buffer
-    and the sentinel check sees it."""
+def test_pushes_on_one_slot_keep_their_regions(lib):
+    """two pushes on the same slot, into different regions with different caps and epochs, queued behind pushes that keep
+    the push stream busy: the second call must not change where the first one scatters, its limits, or the slots it
+    publishes to (the slot's staging is rewritten only after the previous push of that slot has read it).  The first push
+    does not fit the second one's cap, so scattering under it would publish ~0."""
     rng = np.random.default_rng(8)
     keep, regs = [], []
-    n_busy, n, n_parts, ncols = 1 << 25, 200_003, 4, 2
+    n_busy, n_parts, ncols = 1 << 25, 4, 2
+    sizes = [200_003, 40_009]
     try:
         busy = rng.integers(-(1 << 63), (1 << 63) - 1, n_busy, dtype=np.int64)
         bptr = _dev_cols(lib, [busy], keep)
-        data = [_push_data(rng, n, ncols, 0, i * n) for i in range(2)]
+        data = [_push_data(rng, n, ncols, 0, i * sizes[0]) for i, n in enumerate(sizes)]
         ptrs = [_dev_cols(lib, d, keep) for d in data]
         dests = [X.push_dest(d[0], None, n_parts) for d in data]
-        offs = [[1000 + 5000 * q for q in range(n_parts)], [41 + 77 * q for q in range(n_parts)]]
-        rows = [max(offs[0][q], offs[1][q]) + n + GUARD for q in range(n_parts)]     # room for any split of the n rows
-        dst = [_PushDest(lib, rows, ncols, keep) for _ in range(2)]
+        caps = [int(np.bincount(d, minlength=n_parts).max()) for d in dests]
+        assert caps[0] > caps[1]
+        dst = [X.Regions(lib, n_parts, ncols, cap) for cap in caps]
+        regs += dst
         for s in range(4):                      # 1 GB of scatter stores queued on the push stream
             r = X.Regions(lib, 1, 1, n_busy, guard=8)
             regs.append(r)
             L.check(r.push(0, bptr, n_busy, s, 1))
         for i in range(2):
-            L.check(lib.tq_partition_push_device_async(ncols, _tq(ptrs[i], n), 0, n, n_parts, dst[i].ptrs, (C.c_int64 * n_parts)(*offs[i])))
-        L.check(lib.tq_partition_push_wait())
-        for s in range(4):
+            L.check(dst[i].push(0, ptrs[i], sizes[i], 5, 2 + i))
+        for s in (0, 1, 2, 3, 5):
             L.check(lib.tq_partition_push_sync(s))
         for i in range(2):
-            for q in range(n_parts):
-                dst[i].check(q, offs[i][q], X.rows_of(data[i], np.flatnonzero(dests[i] == q)))
-        assert regs[0].slots(0) == [(n_busy, 1)]
+            _check_source(dst[i], 0, data[i], dests[i], 2 + i)
+        assert regs[2].slots(0) == [(n_busy, 1)]
     finally:
         for b in keep + regs:
             b.free()
 
 
-# ================================================================================================ C. push_regions / publish / wait
+def test_push_regions_refusals(lib):
+    """every bad argument: TQ_ERR_INVALID_ARG (more than 4 wire columns: TQ_ERR_UNSUPPORTED_TYPE), and no region, slot,
+    miss column or miss slot is written; then the same buffers push correctly"""
+    rng = np.random.default_rng(12)
+    n, W, ncols = 5_000, 3, 2
+    keep = []
+    reg = X.Regions(lib, W, ncols, n)
+    miss = X.Buf(lib, ncols * (n + GUARD) * 8)
+    mslot = X.Buf(lib, 16, 0)
+    try:
+        cols = _push_data(rng, n, ncols, 0, 0)
+        tq = _tq(_dev_cols(lib, cols, keep), n)
+        args = dict(n_cols=ncols, cols=tq, key_col=0, n=n, n_parts=W, selected=None, keep_misses=1,
+                    dest_data=(C.c_void_p * (W * ncols))(*[reg.region_ptr(d, 0, c) for d in range(W) for c in range(ncols)]),
+                    dest_counts=(C.c_void_p * W)(*[reg.slot_ptr(d, 0) for d in range(W)]), region_cap=reg.cap,
+                    miss_data=(C.c_void_p * ncols)(*[miss.addr(c * (n + GUARD) * 8) for c in range(ncols)]), miss_count=mslot.addr(),
+                    miss_cap=n, slot=0, epoch=1)
+        push = lambda **bad: lib.tq_partition_push_regions(*{**args, **bad}.values())
+        for bad in (dict(n_parts=0), dict(n_parts=9), dict(n_parts=-1), dict(n=-1), dict(n=1 << 32), dict(key_col=-1),
+                    dict(key_col=ncols), dict(n_cols=0), dict(cols=None), dict(dest_data=None), dict(dest_counts=None),
+                    dict(slot=-1), dict(slot=16), dict(region_cap=0), dict(region_cap=1 << 32), dict(miss_data=None),
+                    dict(miss_count=None), dict(miss_cap=-1), dict(miss_cap=1 << 32)):
+            assert push(**bad) == L.TQ_ERR_INVALID_ARG, bad
+        assert push(n_cols=5, cols=(L.TQColumn * 5)(*([tq[0]] * 5))) == L.TQ_ERR_UNSUPPORTED_TYPE
+        for d in range(W):
+            assert reg.slots(d) == [(0, 0)] * W, "a refused push published a slot"
+            assert all(np.all(reg.region(d, 0, c) == X.SENTINEL) for c in range(ncols)), "a refused push wrote rows"
+        assert np.all(mslot.get() == 0), "a refused push published its miss slot"
+        L.check(push())
+        L.check(lib.tq_partition_push_sync(0))
+        _check_source(reg, 0, cols, X.push_dest(cols[0], None, W), 1)
+        assert list(mslot.get()) == [0, 1], "no row misses: the miss slot reads {0, epoch}"
+        assert np.all(miss.get() == X.SENTINEL), "a miss column was written"
+    finally:
+        reg.free()
+        for b in keep + [miss, mslot]:
+            b.free()
+
+
 def _shards(rng, sizes, ncols, first=0):
     out = []
     for n in sizes:
@@ -337,23 +370,14 @@ def _shards(rng, sizes, ncols, first=0):
 def _check_regions(reg, shards, epoch, overflowed=()):
     """slots and regions of every (destination, source) after the pushes of `shards` under `epoch`"""
     w = reg.world
-    for d in range(w):
-        assert [e for _, e in reg.slots(d)] == [epoch] * w, f"destination {d}: epochs"
     for s, cols in enumerate(shards):
-        dest = X.push_dest(cols[0], None, w)
+        if s not in overflowed:
+            _check_source(reg, s, cols, X.push_dest(cols[0], None, w), epoch)
+            continue
         for d in range(w):
-            rows, _ = reg.slots(d)[s]
-            idx = np.flatnonzero(dest == d)
-            if s in overflowed:
-                assert rows == (1 << 64) - 1, f"source {s} overflowed: destination {d} must read ~0, not {rows}"
-                m = reg.cap
-            else:
-                assert rows == len(idx), f"slot ({d}, {s})"
-                m = len(idx)
+            assert reg.slots(d)[s] == ((1 << 64) - 1, epoch), f"source {s} overflowed: destination {d} must read ~0"
             got = np.stack([reg.region(d, s, c) for c in range(reg.ncols)], axis=1)
-            assert np.all(got[m:] == X.SENTINEL), f"region ({d}, {s}): a row past its count / cap"
-            if s not in overflowed:
-                assert np.array_equal(X.sorted_rows(got[:m]), X.rows_of(cols, idx)), f"region ({d}, {s}) rows"
+            assert np.all(got[reg.cap:] == X.SENTINEL), f"region ({d}, {s}): a row past its cap"
 
 
 def _push_all(lib, reg, shards, epoch, keep, slot0=0, wait=True):
@@ -416,7 +440,7 @@ def test_sixteen_push_slots_in_flight(lib):
             b.free()
 
 
-# ================================================================================================ D. segmented join
+# ================================================================================================ C. segmented join
 POS_LAUNCHES = 6        # probe launches of one batch on the streaming join's positional path
 
 
@@ -513,7 +537,7 @@ def test_segmented_join_segment_limit(lib, _stream_partitions):
             ptrs = _dev_cols(lib, cols, keep)
             dest = (C.c_void_p * 2)(reg.region_ptr(0, s, 0), reg.region_ptr(0, s, 1))
             cnts = (C.c_void_p * 1)(reg.slot_ptr(0, s))
-            L.check(lib.tq_partition_push_regions(2, _tq(ptrs, 5_000), 0, 5_000, 1, dest, cnts, reg.cap, s, 1))
+            L.check(lib.tq_partition_push_regions(2, _tq(ptrs, 5_000), 0, 5_000, 1, None, 0, dest, cnts, reg.cap, None, None, 0, s, 1))
         for s in range(8):
             L.check(lib.tq_partition_push_sync(s))
         cols, cnts = reg.segment_args(0)
@@ -528,7 +552,7 @@ def test_segmented_join_segment_limit(lib, _stream_partitions):
             b.free()
 
 
-# ================================================================================================ E. dist.py on the device
+# ================================================================================================ D. dist.py on the device
 def _exchange_in_process(parts, world):
     """what the NCCL all-to-all delivers: destination d receives every source's slice [off[d], off[d + 1]) per column"""
     import torch

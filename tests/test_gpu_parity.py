@@ -541,47 +541,6 @@ def test_agg_table_growth(lib):
         assert_col_equal(a, b)
 
 
-# ------------------------------------------------------------------ multi-GPU shard boundary, exercised on ONE GPU
-def test_partition_count_and_push_local(lib):
-    """tq_partition_count_device + tq_partition_push_device with all destination buffers on this GPU: every row lands in
-    the partition (mix64(key) >> 40) % n_parts, at the offsets the count pass implies, nothing lost or duplicated"""
-    from tinysql_b200 import dist as D
-    from tinysql_b200.chunk import DeviceColumn
-    rng = np.random.default_rng(31)
-    for n, n_parts in ((0, 2), (1, 2), (5000, 3), (300001, 4), (1200000, 8)):
-        k = rng.integers(-(1 << 40), 1 << 40, n).astype(np.int64)
-        v = np.arange(n, dtype=np.int64)
-        dk, dv = DeviceColumn.from_host(Column(INT64, k)), DeviceColumn.from_host(Column(INT64, v))
-        tk = dk.tq(); tk.null_bitmap = None
-        counts = (C.c_int64 * n_parts)()
-        L.check(lib.tq_partition_count_device(C.byref(tk), n, n_parts, counts))
-        want_dest = D.dest_rank_np(k, n_parts) if n else np.zeros(0, np.int64)
-        assert list(counts) == list(np.bincount(want_dest, minlength=n_parts))
-        # destination q gets its own pair of buffers, with a 7-row offset to prove offsets are honoured
-        bufs = [[DeviceColumn(INT64, int(counts[q]) + 7, with_bitmap=False) for _ in range(2)] for q in range(n_parts)]
-        dest = (C.c_void_p * (n_parts * 2))()
-        for q in range(n_parts):
-            for c in range(2):
-                dest[q * 2 + c] = bufs[q][c]._data.value
-        offs = (C.c_int64 * n_parts)(*([7] * n_parts))
-        cols = (L.TQColumn * 2)(dk.tq(), dv.tq())
-        cols[0].null_bitmap = None
-        cols[1].null_bitmap = None
-        L.check(lib.tq_partition_push_device(2, cols, 0, n, n_parts, dest, offs))
-        seen = []
-        for q in range(n_parts):
-            kq = bufs[q][0].to_host().values[7:]
-            vq = bufs[q][1].to_host().values[7:]
-            assert np.all(D.dest_rank_np(kq, n_parts) == q)
-            assert np.array_equal(k[vq], kq)  # the payload still travels with its key
-            seen.append(vq)
-            for b in bufs[q]:
-                b.free()
-        allv = np.sort(np.concatenate(seen)) if seen else np.zeros(0, np.int64)
-        assert np.array_equal(allv, np.arange(n))
-        dk.free(); dv.free()
-
-
 # ------------------------------------------------------------------ partial -> final aggregation (the multi-GPU agg shape)
 def test_agg_partial_export_and_final_merge(lib):
     """two Partial1 handles over disjoint halves -> tq_agg_export_partial -> one Final handle via tq_agg_merge_partial

@@ -1,12 +1,10 @@
 """Outer joins and nullable columns across GPUs on one GPU, every rank emulated in this process (tests/region_outer_ref.py):
-tq_partition_push_regions_masked -> published slots -> tq_region_gather -> an ordinary join handle per destination.
+tq_partition_push_regions -> published slots -> tq_region_gather -> an ordinary join handle per destination.
 
 Per destination: every matched row's probe key has dest_rank_np(key) == destination; a probe row that cannot match (NULL key
 or selected == 0) of an outer join comes out once, as its miss row, on the rank that held it.  Over all destinations the rows
 are exactly oracle_py.hash_join over every shard.  A cap one row short fails the receiving gather, which writes nothing;
 a side wider than the push's 4 words is refused before anything is pushed."""
-import ctypes as C
-
 import numpy as np
 import pytest
 
@@ -181,11 +179,9 @@ def test_push_word_limit_refused_before_any_push(lib):
             src = R.Source(lib, cols[:ncols], nns)
             keep.append(src)
             nw = ncols + (bm_col is not None)
-            reg = X.Regions(lib, W, min(nw, 4), n)
+            reg = X.Regions(lib, W, nw, n)
             keep.append(reg)
-            dest = (C.c_void_p * (W * nw))(*[reg.region_ptr(d, 0, min(c, 3)) for d in range(W) for c in range(nw)])
-            cnts = (C.c_void_p * W)(*[reg.slot_ptr(d, 0) for d in range(W)])
-            st = lib.tq_partition_push_regions_masked(ncols, src.arr, 0, n, W, None, 0, dest, cnts, reg.cap, None, None, 0, 0, 1)
+            st = R.push(reg, 0, src, 0, 1)
             if st == L.TQ_OK:
                 L.check(lib.tq_partition_push_sync(0))
             if ok:

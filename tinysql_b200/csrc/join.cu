@@ -3661,131 +3661,7 @@ int32_t tq_join_build_path(tq_join *j, int32_t *path) {
   return TQ_OK;
 }
 
-// ---- multi-GPU shard boundary: count, then push-scatter straight into the peers' receive buffers ---------------
-static int32_t part_common_check(int32_t n_parts, int64_t n) {
-  if (n_parts < 1 || n_parts > 8 || n < 0 || n > 0xFFFFFFF0ll) { set_error("push partitioning supports 1..8 partitions and < 2^32 rows"); return TQ_ERR_INVALID_ARG; }
-  return TQ_OK;
-}
-
-int32_t tq_partition_count_device(const tq_column *key, int64_t n, int32_t n_parts, int64_t *counts) {
-  TQ_TRY(ensure_init());
-  if (!key || !counts) return TQ_ERR_INVALID_ARG;
-  TQ_TRY(part_common_check(n_parts, n));
-  Runtime &r = rt();
-  std::lock_guard<std::recursive_mutex> lk(r.mu);
-  cudaStream_t s = r.compute;
-  static DevBuf cnt;
-  static PinBuf h_cnt;
-  TQ_TRY(cnt.reserve(64));
-  TQ_TRY(h_cnt.reserve(64));
-  TQ_CUDA(cudaMemsetAsync(cnt.p, 0, 64, s));
-  if (n > 0) {
-    ScatterParams sp{};
-    sp.n_cols = 1;
-    sp.in[0].data = (const uint64_t *)key->data;
-    sp.in[0].bm = (const uint32_t *)key->null_bitmap;
-    sp.key_col = 0;
-    sp.key_mode = KEYMODE_RAW;
-    sp.is_outer = 0;  // rows with a NULL key cannot match in an inner join: they are not exchanged
-    sp.n = n;
-    sp.part_cnt = cnt.as<uint32_t>();
-    sp.n_parts_mod = n_parts;
-    k_probe_part_hist<<<r.sm_count * 4, SCAT_THREADS, (n_parts + 1) * 4, s>>>(sp);
-    count_launch();
-    TQ_TRY(check_launch("k_probe_part_hist"));
-  }
-  TQ_CUDA(cudaMemcpyAsync(h_cnt.p, cnt.p, 64, cudaMemcpyDeviceToHost, s));
-  TQ_CUDA(cudaStreamSynchronize(s));
-  for (int i = 0; i < n_parts; i++) counts[i] = h_cnt.as<uint32_t>()[i];
-  return TQ_OK;
-}
-
-// The push scatter of n rows of n_cols columns by column key_col into n_parts destinations: checks the arguments the pushes
-// share and fills sp up to the cursors, limits and overflow flag, which each push sets up itself.  dest_data[q * n_wire + c] =
-// column c of destination q.  `fn` names the entry point in errors.  Unless `masked`, the columns must be NOT NULL and
-// n_wire = n_cols; masked, NULL bitmaps are accepted (sp.in[c].bm, for pack_null_mask) and n_wire = n_cols + 1 when one is
-// present: the mask word is wire column n_cols, its source is set by the push.
-static int32_t push_scatter_params(const char *fn, int32_t n_cols, const tq_column *cols, int32_t key_col, int64_t n, int32_t n_parts,
-                                   void *const *dest_data, ScatterParams &sp, bool masked = false) {
-  if (!cols || !dest_data || n_cols < 1 || (!masked && n_cols > 4) || key_col < 0 || key_col >= n_cols) { set_error("%s: 1..4 columns", fn); return TQ_ERR_INVALID_ARG; }
-  TQ_TRY(part_common_check(n_parts, n));
-  bool any_bm = false;
-  for (int c = 0; c < n_cols; c++) {
-    if (cols[c].null_bitmap && !masked) { set_error("%s: columns with NULL bitmaps are not supported (use tq_partition_device)", fn); return TQ_ERR_UNSUPPORTED_TYPE; }
-    any_bm = any_bm || cols[c].null_bitmap;
-  }
-  const int n_wire = n_cols + (any_bm ? 1 : 0);
-  if (n_wire > 4) { set_error("%s: %d columns%s: the push moves at most 4 words per row", fn, n_cols, any_bm ? " and the NULL mask word" : ""); return TQ_ERR_UNSUPPORTED_TYPE; }
-  sp = ScatterParams{};
-  sp.n_cols = n_wire;
-  sp.key_col = key_col;
-  sp.key_mode = KEYMODE_RAW;
-  sp.n = n;
-  sp.n_parts_mod = n_parts;
-  for (int c = 0; c < n_cols; c++) {
-    sp.in[c].data = (const uint64_t *)cols[c].data;
-    sp.in[c].bm = (const uint32_t *)cols[c].null_bitmap;
-  }
-  for (int q = 0; q < n_parts; q++)
-    for (int c = 0; c < n_wire; c++) sp.out_bin[q][c] = (uint64_t *)dest_data[q * n_wire + c];
-  return TQ_OK;
-}
-
-static int32_t partition_push(int32_t n_cols, const tq_column *cols, int32_t key_col, int64_t n, int32_t n_parts, void *const *dest_data,
-                              const int64_t *dest_row_offsets, bool async) {
-  TQ_TRY(ensure_init());
-  if (!dest_row_offsets) { set_error("tq_partition_push_device: 1..4 columns"); return TQ_ERR_INVALID_ARG; }
-  ScatterParams sp;
-  TQ_TRY(push_scatter_params("tq_partition_push_device", n_cols, cols, key_col, n, n_parts, dest_data, sp));
-  if (n == 0) return TQ_OK;
-  Runtime &r = rt();
-  std::lock_guard<std::recursive_mutex> lk(r.mu);
-  // async pushes run on the library's second stream so the probe rows can cross NVLink while the hash table is built
-  cudaStream_t s = async ? r.h2d : r.compute;
-  static DevBuf cursors[2];
-  DevBuf &cursor = cursors[async ? 1 : 0];
-  TQ_TRY(cursor.reserve(64));
-  static PinBuf h_cur_pin[2];
-  // staged_ev[i] marks the end of the last copy out of h_cur_pin[i]: an async push returns with that copy still queued
-  // behind whatever the push stream is running, so the next push may rewrite the staging only once the copy has read it
-  static cudaEvent_t staged_ev[2];
-  cudaEvent_t &staged = staged_ev[async ? 1 : 0];
-  if (!staged) TQ_CUDA(cudaEventCreateWithFlags(&staged, cudaEventDisableTiming));
-  TQ_TRY(h_cur_pin[async ? 1 : 0].reserve(64));
-  uint32_t *h_cur = h_cur_pin[async ? 1 : 0].as<uint32_t>();
-  TQ_CUDA(cudaEventSynchronize(staged));
-  memset(h_cur, 0, 64);
-  for (int q = 0; q < n_parts; q++) {
-    if (dest_row_offsets[q] < 0 || dest_row_offsets[q] > 0xFFFFFFF0ll) { set_error("destination offset out of range"); return TQ_ERR_INVALID_ARG; }
-    h_cur[q] = (uint32_t)dest_row_offsets[q];
-  }
-  TQ_CUDA(cudaMemcpyAsync(cursor.p, h_cur, 64, cudaMemcpyHostToDevice, s));
-  TQ_CUDA(cudaEventRecord(staged, s));
-  sp.part_cursor = cursor.as<uint32_t>();
-  sp.part_lim = nullptr;
-  static DevBuf ovf;
-  TQ_TRY(ovf.reserve(8));
-  sp.overflow = ovf.as<unsigned long long>();
-  TQ_TRY(launch_scatter_fast(sp, s, "k_probe_scatter_fast(push)"));
-  if (!async) TQ_CUDA(cudaStreamSynchronize(s));
-  return TQ_OK;
-}
-
-int32_t tq_partition_push_device(int32_t n_cols, const tq_column *cols, int32_t key_col, int64_t n, int32_t n_parts, void *const *dest_data,
-                                 const int64_t *dest_row_offsets) {
-  return partition_push(n_cols, cols, key_col, n, n_parts, dest_data, dest_row_offsets, false);
-}
-int32_t tq_partition_push_device_async(int32_t n_cols, const tq_column *cols, int32_t key_col, int64_t n, int32_t n_parts, void *const *dest_data,
-                                       const int64_t *dest_row_offsets) {
-  return partition_push(n_cols, cols, key_col, n, n_parts, dest_data, dest_row_offsets, true);
-}
-int32_t tq_partition_push_wait(void) {
-  TQ_TRY(ensure_init());
-  TQ_CUDA(cudaStreamSynchronize(rt().h2d));
-  return TQ_OK;
-}
-
-// ---- push into per-source REGIONS of the peers' receive buffers: no count exchange before the push -----------------------
+// ---- multi-GPU shard boundary: push into per-source REGIONS of the peers' receive buffers, no count exchange first --------
 // Every destination rank reserves one region of `region_cap` rows per source rank and per column; this rank scatters its rows
 // straight into "its" region on every peer (stores over NVLink) and then publishes how many rows it wrote to each peer in
 // that peer's count table (one 8-byte peer store per destination).  The receiver joins the regions as ONE segmented batch
@@ -3827,20 +3703,50 @@ struct PushSlot {
 };
 static PushSlot g_push_slot[PUSH_SLOTS];
 
-static int32_t push_slot_check(const char *fn, void *const *dest_counts, int64_t region_cap, int32_t slot) {
-  if (!dest_counts || slot < 0 || slot >= PUSH_SLOTS || region_cap < 1 || region_cap > 0xFFFFFFF0ll) {
-    set_error("%s: 1..4 columns, slot 0..%d", fn, PUSH_SLOTS - 1);
+// One region push (include/tinysql_b200.h): every argument is checked before anything is enqueued, so a refused push writes
+// no region and publishes no slot.  Then the scatter of n rows into n_parts destinations (+ the miss bin with keep_misses)
+// runs on the push stream, followed by k_publish_counts.
+int32_t tq_partition_push_regions(int32_t n_cols, const tq_column *cols, int32_t key_col, int64_t n, int32_t n_parts,
+                                  const uint8_t *selected, int32_t keep_misses, void *const *dest_data, void *const *dest_counts,
+                                  int64_t region_cap, void *const *miss_data, void *miss_count, int64_t miss_cap, int32_t slot,
+                                  uint64_t epoch) {
+  TQ_TRY(ensure_init());
+  const char *fn = "tq_partition_push_regions";
+  if (!cols || !dest_data || !dest_counts || n_cols < 1 || key_col < 0 || key_col >= n_cols) {
+    set_error("%s: needs columns, destinations, count slots and 0 <= key_col < n_cols", fn);
     return TQ_ERR_INVALID_ARG;
   }
-  return TQ_OK;
-}
+  if (n_parts < 1 || n_parts > 8 || n < 0 || n > 0xFFFFFFF0ll) { set_error("%s: 1..8 destinations and < 2^32 rows", fn); return TQ_ERR_INVALID_ARG; }
+  if (slot < 0 || slot >= PUSH_SLOTS || region_cap < 1 || region_cap > 0xFFFFFFF0ll) {
+    set_error("%s: slot 0..%d and 1 <= region_cap < 2^32", fn, PUSH_SLOTS - 1);
+    return TQ_ERR_INVALID_ARG;
+  }
+  if (keep_misses && (!miss_data || !miss_count || miss_cap < 0 || miss_cap > 0xFFFFFFF0ll)) {
+    set_error("%s: keep_misses needs miss columns, a miss slot and 0 <= miss_cap < 2^32", fn);
+    return TQ_ERR_INVALID_ARG;
+  }
+  // a NULL bitmap anywhere: the mask word travels as wire column n_cols, and a NULL key routes like an unselected row
+  bool pack = false;
+  for (int c = 0; c < n_cols; c++) pack = pack || cols[c].null_bitmap;
+  const int n_wire = n_cols + (pack ? 1 : 0);
+  if (n_wire > 4) { set_error("%s: %d columns%s: the push moves at most 4 words per row", fn, n_cols, pack ? " and the NULL mask word" : ""); return TQ_ERR_UNSUPPORTED_TYPE; }
+  ScatterParams sp{};
+  sp.n_cols = n_wire;
+  sp.key_col = key_col;
+  sp.key_mode = KEYMODE_RAW;
+  sp.n = n;
+  sp.n_parts_mod = n_parts;
+  sp.is_outer = keep_misses ? 1 : 0;
+  sp.selected = selected;
+  for (int c = 0; c < n_cols; c++) {
+    sp.in[c].data = (const uint64_t *)cols[c].data;
+    sp.in[c].bm = (const uint32_t *)cols[c].null_bitmap;
+  }
+  for (int q = 0; q < n_parts; q++)
+    for (int c = 0; c < n_wire; c++) sp.out_bin[q][c] = (uint64_t *)dest_data[q * n_wire + c];
+  if (keep_misses)
+    for (int c = 0; c < n_wire; c++) sp.out_bin[n_parts][c] = (uint64_t *)miss_data[c];
 
-// Enqueues one region push of sp (filled by push_scatter_params, arguments checked by push_slot_check) on the push stream and publishes its counts: n_parts slots
-// at dest_counts, and with keep_misses the miss bin's count at miss_count.  n_cols user columns; with `pack` the mask word and
-// the effective selection are made first (pack_null_mask), otherwise `selected` is used as it is.
-static int32_t push_regions(const char *fn, ScatterParams &sp, const tq_column *cols, int32_t n_cols, bool pack, const uint8_t *selected,
-                            int32_t n_parts, void *const *dest_counts, int64_t region_cap, bool keep_misses, void *miss_count, int64_t miss_cap,
-                            int32_t slot, uint64_t epoch) {
   Runtime &r = rt();
   std::lock_guard<std::recursive_mutex> lk(r.mu);
   cudaStream_t s = r.h2d;  // the push stream: rows cross NVLink while the compute stream joins what has already arrived
@@ -3859,20 +3765,18 @@ static int32_t push_regions(const char *fn, ScatterParams &sp, const tq_column *
   if (keep_misses) {
     ps.h_lim.as<uint32_t>()[n_parts] = (uint32_t)miss_cap;
     ps.h_ptrs.as<void *>()[n_parts] = miss_count;
-    sp.is_outer = 1;
   }
   TQ_CUDA(cudaMemsetAsync(ps.cursor.p, 0, 64, s));
   TQ_CUDA(cudaMemsetAsync(ps.ovf.p, 0, 8, s));
   TQ_CUDA(cudaMemcpyAsync(ps.lim.p, ps.h_lim.p, 64, cudaMemcpyHostToDevice, s));
   TQ_CUDA(cudaMemcpyAsync(ps.counts_ptrs.p, ps.h_ptrs.p, 128, cudaMemcpyHostToDevice, s));
-  sp.selected = selected;
-  if (sp.n > 0) {
-    if (pack) {
-      TQ_TRY(ps.mask.reserve((size_t)sp.n * 8));
-      TQ_TRY(ps.sel.reserve((size_t)sp.n));
-      TQ_TRY(pack_null_mask(sp.in, n_cols, sp.key_col, selected, sp.n, ps.mask.as<uint64_t>(), ps.sel.as<uint8_t>(), s));
+  if (n > 0) {
+    if (pack) {  // the mask word and the effective selection first
+      TQ_TRY(ps.mask.reserve((size_t)n * 8));
+      TQ_TRY(ps.sel.reserve((size_t)n));
+      TQ_TRY(pack_null_mask(sp.in, n_cols, key_col, selected, n, ps.mask.as<uint64_t>(), ps.sel.as<uint8_t>(), s));
       sp.selected = ps.sel.as<uint8_t>();
-      if (sp.n_cols > n_cols) sp.in[n_cols] = DCol{ps.mask.as<uint64_t>(), nullptr};
+      sp.in[n_cols] = DCol{ps.mask.as<uint64_t>(), nullptr};
     }
     sp.part_cursor = ps.cursor.as<uint32_t>();
     sp.part_lim = ps.lim.as<uint32_t>();
@@ -3884,35 +3788,6 @@ static int32_t push_regions(const char *fn, ScatterParams &sp, const tq_column *
   TQ_TRY(check_launch("k_publish_counts"));
   TQ_CUDA(cudaEventRecord(ps.ev, s));
   return TQ_OK;
-}
-
-int32_t tq_partition_push_regions(int32_t n_cols, const tq_column *cols, int32_t key_col, int64_t n, int32_t n_parts, void *const *dest_data,
-                                  void *const *dest_counts, int64_t region_cap, int32_t slot, uint64_t epoch) {
-  TQ_TRY(ensure_init());
-  TQ_TRY(push_slot_check("tq_partition_push_regions", dest_counts, region_cap, slot));
-  ScatterParams sp;
-  TQ_TRY(push_scatter_params("tq_partition_push_regions", n_cols, cols, key_col, n, n_parts, dest_data, sp));
-  return push_regions("tq_partition_push_regions", sp, cols, n_cols, false, nullptr, n_parts, dest_counts, region_cap, false, nullptr, 0, slot, epoch);
-}
-
-int32_t tq_partition_push_regions_masked(int32_t n_cols, const tq_column *cols, int32_t key_col, int64_t n, int32_t n_parts,
-                                         const uint8_t *selected, int32_t keep_misses, void *const *dest_data, void *const *dest_counts,
-                                         int64_t region_cap, void *const *miss_data, void *miss_count, int64_t miss_cap, int32_t slot,
-                                         uint64_t epoch) {
-  TQ_TRY(ensure_init());
-  const char *fn = "tq_partition_push_regions_masked";
-  TQ_TRY(push_slot_check(fn, dest_counts, region_cap, slot));
-  if (keep_misses && (!miss_data || !miss_count || miss_cap < 0 || miss_cap > 0xFFFFFFF0ll)) {
-    set_error("%s: keep_misses needs miss columns, a miss slot and 0 <= miss_cap < 2^32", fn);
-    return TQ_ERR_INVALID_ARG;
-  }
-  ScatterParams sp;
-  TQ_TRY(push_scatter_params(fn, n_cols, cols, key_col, n, n_parts, dest_data, sp, true));
-  if (keep_misses) {
-    for (int c = 0; c < sp.n_cols; c++) sp.out_bin[n_parts][c] = (uint64_t *)miss_data[c];
-  }
-  const bool pack = sp.n_cols > n_cols;  // a NULL bitmap somewhere: the mask word travels, and a NULL key routes like an unselected row
-  return push_regions(fn, sp, cols, n_cols, pack, selected, n_parts, dest_counts, region_cap, keep_misses != 0, miss_count, miss_cap, slot, epoch);
 }
 
 int32_t tq_region_wait(const void *slots, int32_t n_sources, uint64_t epoch) {

@@ -163,16 +163,24 @@ class RegionExchange:
         self.epoch += 1
         return self.epoch
 
-    def push(self, t, cols, n, slot):
-        """scatter this rank's rows of table t into its region on every rank; asynchronous (push stream)"""
-        nc, w = self.ncols[t], self.world
-        dest = (C.c_void_p * (w * nc))()
+    def push(self, t, cols, n, slot, bitmaps=None, selected=None, miss=None):
+        """scatter this rank's rows of table t into its region on every rank; asynchronous (push stream).  bitmaps: a device
+        NULL bitmap pointer (or None) per column; with any, the mask word travels as table t's last wire column.  selected:
+        device address of n bytes (0/1) or None.  miss: (wire column pointers, slot pointer, rows) that keep the rows which
+        cannot match on this rank, or None to drop them."""
+        nw, w = self.ncols[t], self.world
+        arr = _tq_cols(self.L, cols, n)
+        for c, b in enumerate(bitmaps or []):
+            arr[c].null_bitmap = b
+        dest = (C.c_void_p * (w * nw))()
         cnts = (C.c_void_p * w)()
         for d in range(w):
-            for c in range(nc):
-                dest[d * nc + c] = self.region_ptr(d, t, self.rank, c)
+            for c in range(nw):
+                dest[d * nw + c] = self.region_ptr(d, t, self.rank, c)
             cnts[d] = self.slot_ptr(d, t, self.rank)
-        self.L.check(self.lib.tq_partition_push_regions(nc, _tq_cols(self.L, cols, n), 0, n, w, dest, cnts, self.cap[t], slot, self.epoch))
+        miss_cols, miss_slot, miss_cap = (None, None, 0) if miss is None else ((C.c_void_p * nw)(*miss[0]), miss[1], miss[2])
+        self.L.check(self.lib.tq_partition_push_regions(len(cols), arr, 0, n, w, selected, int(miss is not None), dest, cnts, self.cap[t],
+                                                        miss_cols, miss_slot, miss_cap, slot, self.epoch))
 
     def wait(self, t):
         """device-side: the compute stream waits until every source has published table t for this epoch"""
@@ -376,10 +384,10 @@ class RegionJoin:
 
     The join is an ordinary tq_join_desc with the key in column 0 of both sides: join_type / outer_is_right as on one GPU,
     INT64 / UINT64 / FLOAT64 columns, optional defaultInner.  An inner join of NOT NULL columns reads the regions in place
-    (tq_join_put_probe_segments).  Otherwise (an outer join, or a side declared nullable) the pushes are
-    tq_partition_push_regions_masked: a nullable side carries the mask word, the probe rows of an outer join that cannot
-    match (NULL key, selected == 0) stay on this rank, and the receiver copies each table's regions into contiguous columns
-    with tq_region_gather before tq_join_put_build / tq_join_put_probe; the kept rows are one more probe batch, unselected."""
+    (tq_join_put_probe_segments).  Otherwise (an outer join, or a side declared nullable) a nullable side's push carries the
+    mask word, the probe rows of an outer join that cannot match (NULL key, selected == 0) stay on this rank, and the
+    receiver copies each table's regions into contiguous columns with tq_region_gather before tq_join_put_build /
+    tq_join_put_probe; the kept rows are one more probe batch, unselected."""
 
     def __init__(self, lib, L, world, rank, n_build_max, n_probe_max, n_chunks, slack=1.25, join_type=0, outer_is_right=True,
                  build_types=None, probe_types=None, build_nullable=False, probe_nullable=False, default_inner=None):
@@ -400,12 +408,12 @@ class RegionJoin:
         tables = [(nb + self.bmask, cap(n_build_max))] + [(npc + self.pmask, cap(self.chunk_max)) for c in range(n_chunks)]
         self.rx = RegionExchange(lib, L, world, rank, tables)
         self._bufs = []
+        self.outer = join_type != 0
         if not self.segmented:
             rx = self.rx
             # receive side: the build table and one probe chunk as contiguous columns (+ bitmaps), and the kept miss rows
             self.g_build = self._cols(nb, world * rx.cap[0], self.bmask)
             self.g_probe = self._cols(npc, world * rx.cap[1], self.pmask)
-            self.outer = join_type != 0
             if self.outer:
                 self.g_miss = self._cols(npc, self.chunk_max, self.pmask)
                 # this rank's miss rows of chunk c: wire columns of chunk_max rows and a 16-byte {rows, epoch} slot
@@ -567,29 +575,13 @@ class RegionJoin:
         return total, list(st), result
 
     def _push(self, t, cols, bitmaps, selected, n, slot, row0, chunk=None):
-        """push this rank's rows of table t; on the masked path bitmaps / selected are taken from row row0 on"""
-        rx = self.rx
-        if self.segmented:
-            rx.push(t, cols, n, slot)
-            return
-        L, w, nw = self.L, self.world, rx.ncols[t]
-        nc = nw - (self.bmask if t == 0 else self.pmask)
-        arr = _tq_cols(self.L, cols, n)
-        for c, b in enumerate(bitmaps or []):
-            arr[c].null_bitmap = None if b is None else b + row0 // 8
-        if nw > nc and n and not any(arr[c].null_bitmap for c in range(nc)):
-            arr[0].null_bitmap = self._ones(n)          # a side declared nullable always carries the mask word: the layout is shared
-        dest = (C.c_void_p * (w * nw))()
-        cnts = (C.c_void_p * w)()
-        for d in range(w):
-            for c in range(nw):
-                dest[d * nw + c] = rx.region_ptr(d, t, rx.rank, c)
-            cnts[d] = rx.slot_ptr(d, t, rx.rank)
-        keep = t > 0 and self.outer
-        miss = (C.c_void_p * nw)(*self.miss_data[chunk]) if keep else None
+        """push this rank's rows of table t; bitmaps / selected are taken from row row0 on"""
+        bms = [None if b is None else b + row0 // 8 for b in bitmaps or []]
+        if (self.bmask if t == 0 else self.pmask) and n and not any(bms):
+            bms = [self._ones(n)]                      # a side declared nullable always carries the mask word: the layout is shared
         sel = None if (t == 0 or selected is None) else selected.data_ptr() + row0
-        L.check(self.lib.tq_partition_push_regions_masked(nc, arr, 0, n, w, sel, int(keep), dest, cnts, rx.cap[t], miss,
-                                                          self.miss_slot[chunk] if keep else None, self.chunk_max, slot, rx.epoch))
+        miss = (self.miss_data[chunk], self.miss_slot[chunk], self.chunk_max) if t > 0 and self.outer else None
+        self.rx.push(t, cols, n, slot, bms, sel, miss)
 
     def _gather(self, t, target, has_mask):
         """wait (device-side) for table t from every source and copy its regions into target; returns the rows"""
