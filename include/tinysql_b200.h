@@ -478,6 +478,32 @@ int32_t tq_agg_stats(tq_agg *a, int64_t *stats4);
 int32_t tq_agg_partial_width(tq_agg *a, int32_t *n_cols);
 int32_t tq_agg_export_partial(tq_agg *a, tq_column *out_cols, int64_t *n_rows);
 int32_t tq_agg_merge_partial(tq_agg *a, const tq_column *cols, int32_t mem);
+/* The same partial -> shuffle -> final over the region exchange (tq_partition_push_regions, below): no count exchange, no
+ * staging copy, nullable columns and GROUP BYs of any number of items.  Wire format: with w = tq_agg_partial_width(a), a partial
+ * row (the layout of tq_agg_export_partial: key columns, then states) travels as w + 1 8-byte words, the last the NULL mask
+ * (bit c = column c is NOT NULL); w + 1 > 64 is TQ_ERR_INVALID_ARG.
+ *
+ * tq_agg_push_partial, after the raw rows of a tq_agg_create handle (tq_agg_eof is implied): exports the partial rows (one
+ * host read of the group count) and scatters them on the push stream — dest_data[q * (w + 1) + c] = THIS rank's region for
+ * wire column c on rank q (local or PEER pointer), region_cap rows; dest_counts[q] = its 16-byte {u64 rows, u64 epoch} slot
+ * there — then publishes the slots as tq_partition_push_regions does (same slots 0..15, waited for with
+ * tq_partition_push_sync(slot); overflow of any region makes every slot read ~0).  The handle's partial rows are read until
+ * the push has finished.  A row goes to the rank its group names, a pure function of the group: h = 0, then per GROUP BY item
+ * g  h = mix64(h ^ v_g), v_g = the item's 8 bytes (REAL: -0.0 read as +0.0) or 0x4E554C4C4E554C4C for NULL; rank =
+ * (h >> 40) % n_parts.  One NOT NULL item: (mix64(v) >> 40) % n_parts, the rank tq_partition_push_regions sends that key to;
+ * a scalar aggregate (no GROUP BY) sends its row to rank 0.  n_parts 1..8, 1 <= region_cap < 2^32.
+ *
+ * tq_agg_merge_regions, on a handle created with the same desc that has taken no raw rows (queue tq_region_wait first):
+ * reads the n_regions (1..8) consecutive slots at `slots` (one host read) and merges regions[g * (w + 1) + c] (wire column c
+ * of region g) with tq_agg_merge_partial's semantics, reading the regions in place.  A slot above region_cap (or ~0) is
+ * TQ_ERR_OOM and merges nothing.  Then tq_agg_eof / next as usual.
+ *
+ * Both refuse what tq_agg_export_partial / tq_agg_merge_partial refuse (var-len columns: TQ_ERR_UNSUPPORTED_TYPE; a FinalMode
+ * handle, or raw and partial rows on one handle: TQ_ERR_STATE), and check every argument before anything is enqueued: a
+ * refused push writes no region and publishes no slot. */
+int32_t tq_agg_push_partial(tq_agg *a, int32_t n_parts, void *const *dest_data, void *const *dest_counts, int64_t region_cap,
+                            int32_t slot, uint64_t epoch);
+int32_t tq_agg_merge_regions(tq_agg *a, int32_t n_regions, const void *slots, int64_t region_cap, const tq_column *regions);
 
 /* FinalMode HashAgg over pushed-down partial results (SURVEY §8 f4).  The planner splits an aggregation into a Partial1
  * half that runs inside the coprocessor (planner/core/task.go:564-625, store/mockstore/mocktikv/aggregate.go:81-124: each row

@@ -1,0 +1,153 @@
+"""Reference of the GROUP BY over the region exchange (tq_agg_push_partial / tq_agg_merge_regions), and the runner that drives
+it with every rank emulated in one process on exchange_ref's Regions layout.
+
+group_dest is the Python twin of the destination rule (include/tinysql_b200.h, csrc/scatter.cuh): h = 0, then per GROUP BY
+item h = mix64(h ^ v), v = the item's 8 bytes (REAL: -0.0 read as +0.0) or GROUP_NULL_WORD for NULL; rank = (h >> 40) % W."""
+import ctypes as C
+
+import numpy as np
+
+import exchange_ref as X
+import oracle_py as O
+from tinysql_b200 import _lib as L
+from tinysql_b200.chunk import Column
+from tinysql_b200.dist import agg_drain, mix64_np
+
+GROUP_NULL_WORD = np.uint64(0x4E554C4C4E554C4C)
+NEG_ZERO = np.uint64(1 << 63)
+NP_TYPE = {L.TQ_TYPE_INT64: np.int64, L.TQ_TYPE_UINT64: np.uint64, L.TQ_TYPE_FLOAT64: np.float64}
+
+
+def group_dest(n, items, nns, reals, n_parts):
+    """destination of n partial rows; items: the GROUP BY columns as uint64 arrays, nns: NOT-NULL bool arrays or None,
+    reals: per item, whether it is REAL"""
+    h = np.zeros(n, np.uint64)
+    for v, nn, real in zip(items, nns, reals):
+        v = np.asarray(v).view(np.uint64)
+        if real:
+            v = np.where(v == NEG_ZERO, np.uint64(0), v)
+        if nn is not None:
+            v = np.where(nn, v, GROUP_NULL_WORD)
+        h = mix64_np(h ^ v)
+    return ((h >> np.uint64(40)) % np.uint64(n_parts)).astype(np.int64)
+
+
+# ------------------------------------------------------------------------------------------------ emulated ranks
+def desc(types, group_by, funcs, not_null=()):
+    """a tq_agg_desc (and what keeps its arrays alive); not_null: input columns declared NOT NULL"""
+    it = (C.c_int32 * len(types))(*[t | (L.TQ_TYPE_NOT_NULL if c in not_null else 0) for c, t in enumerate(types)])
+    gb = (C.c_int32 * max(len(group_by), 1))(*group_by)
+    fa = (L.TQAggFunc * max(len(funcs), 1))(*[L.TQAggFunc(f, a) for f, a in funcs])
+    return L.TQAggDesc(len(types), it, len(group_by), gb, len(funcs), fa, 0), (it, gb, fa)
+
+
+def create(lib, d):
+    h = C.c_void_p()
+    L.check(lib.tq_agg_create(C.byref(d), C.byref(h)))
+    return h
+
+
+def width(lib, d):
+    h = create(lib, d)
+    try:
+        w = C.c_int32(0)
+        L.check(lib.tq_agg_partial_width(h, C.byref(w)))
+        return w.value
+    finally:
+        lib.tq_agg_destroy(h)
+
+
+def push_args(reg, src):
+    """(dest_data, dest_counts) of source src on every destination of reg"""
+    w, nw = reg.world, reg.ncols
+    dest = (C.c_void_p * (w * nw))()
+    cnts = (C.c_void_p * w)()
+    for d in range(w):
+        for c in range(nw):
+            dest[d * nw + c] = reg.region_ptr(d, src, c)
+        cnts[d] = reg.slot_ptr(d, src)
+    return dest, cnts
+
+
+def merge_args(reg, dst):
+    w, nw = reg.world, reg.ncols
+    regs = (L.TQColumn * (w * nw))()
+    for g in range(w):
+        for c in range(nw):
+            regs[g * nw + c].data = reg.region_ptr(dst, g, c)
+    return regs
+
+
+def partial_handle(lib, d, src):
+    """a Partial1 handle fed one shard (an R.Source in device memory), eof'd"""
+    h = create(lib, d)
+    if src.n:
+        arr = (L.TQColumn * len(src.ptrs))()
+        for c in range(len(src.ptrs)):
+            arr[c].length, arr[c].data, arr[c].null_bitmap = src.n, src.ptrs[c], src.bms[c]
+        L.check(lib.tq_agg_put(h, arr, L.TQ_MEM_DEVICE))
+    L.check(lib.tq_agg_eof(h))
+    return h
+
+
+def run(lib, W, types, group_by, funcs, shards, reg, epoch=1, not_null=()):
+    """one step: every source's Partial1 handle pushes (slot = source), every destination waits and merges into a Final handle.
+    shards: per source an R.Source.  Returns per destination (status of tq_agg_merge_regions, host Columns or None).  A scalar
+    aggregate is finished on destination 0 only (dist.RegionAgg): the others return None."""
+    d, keep = desc(types, group_by, funcs, not_null)
+    hs = []
+    try:
+        for s in range(W):
+            hs.append(partial_handle(lib, d, shards[s]))
+            dest, cnts = push_args(reg, s)
+            L.check(lib.tq_agg_push_partial(hs[-1], W, dest, cnts, reg.cap, s, epoch))
+        out = []
+        for q in range(W):
+            L.check(reg.wait(q, epoch))                      # queued after every push that satisfies it
+            hf = create(lib, d)
+            try:
+                st = lib.tq_agg_merge_regions(hf, W, C.c_void_p(reg.slot_ptr(q, 0)), reg.cap, merge_args(reg, q))
+                if st != L.TQ_OK:
+                    out.append((st, None))
+                    continue
+                L.check(lib.tq_agg_eof(hf))
+                out.append((st, agg_drain(lib, L, hf, len(funcs)) if group_by or q == 0 else None))
+            finally:
+                lib.tq_agg_destroy(hf)
+        for s in range(W):
+            L.check(lib.tq_partition_push_sync(s))
+    finally:
+        for h in hs:
+            lib.tq_agg_destroy(h)
+    return out
+
+
+# ------------------------------------------------------------------------------------------------ comparison
+def canon(cols, skip=()):
+    """rows of host Columns as one uint64 matrix (NULL = 0 with a 0 flag column, REAL -0.0 as +0.0), rows sorted; columns in
+    skip are left out"""
+    m = []
+    for i, c in enumerate(cols):
+        if i in skip:
+            continue
+        nn = c.not_null()
+        v = np.asarray(c.values)
+        if v.dtype == np.float64:
+            v = v + 0.0
+        bits = np.where(nn, np.ascontiguousarray(v).view(np.uint64), np.uint64(0))
+        m += [nn.astype(np.uint64), bits]
+    if not m:
+        return np.zeros((cols[0].length if cols else 0, 0), np.uint64)
+    return X.sorted_rows(np.stack(m, axis=1))
+
+
+def oracle(types, shards_host, group_by, funcs):
+    """O.hash_agg over the concatenation of every shard: shards_host = per source (value arrays, NOT-NULL arrays or None)"""
+    cols = []
+    for c, t in enumerate(types):
+        vals = np.concatenate([np.asarray(v[c]).view(NP_TYPE[t]) for v, _ in shards_host]) if shards_host else np.zeros(0, NP_TYPE[t])
+        nns = [nn[c] if nn[c] is not None else np.ones(len(v[c]), bool) for v, nn in shards_host]
+        cols.append(Column(t, vals, np.concatenate(nns) if nns else np.zeros(0, bool)))
+    rc, want = O.hash_agg(types, cols, group_by, funcs)
+    assert rc == 0, rc
+    return want

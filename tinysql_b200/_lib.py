@@ -125,6 +125,8 @@ SYMBOLS = {
     "tq_agg_partial_width": (_I32, [_P, C.POINTER(_I32)]),
     "tq_agg_export_partial": (_I32, [_P, _COL, C.POINTER(_I64)]),
     "tq_agg_merge_partial": (_I32, [_P, _COL, _I32]),
+    "tq_agg_push_partial": (_I32, [_P, _I32, C.POINTER(_P), C.POINTER(_P), _I64, _I32, C.c_uint64]),
+    "tq_agg_merge_regions": (_I32, [_P, _I32, _P, _I64, _COL]),
     "tq_sort_create": (_I32, [C.POINTER(TQSortDesc), C.POINTER(_P)]),
     "tq_sort_put": (_I32, [_P, _COL, _I32]), "tq_sort_eof": (_I32, [_P]),
     "tq_sort_next_bytes": (_I32, [_P, _I64, C.POINTER(_I64)]),

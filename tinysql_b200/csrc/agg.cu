@@ -14,6 +14,7 @@
 
 #include "common.cuh"
 #include "dict.cuh"
+#include "push.cuh"
 #include "scatter.cuh"
 #include "strdict.cuh"
 #include "varlen.cuh"
@@ -588,6 +589,8 @@ struct tq_agg {
   DevBuf pre_aos;
   DevBuf pre_lo, pre_hi, pre_lim, pre_meta;
   cudaEvent_t ev_pa = nullptr, ev_pb = nullptr;
+  std::vector<DevBuf> region_bm;   // tq_agg_merge_regions: the NOT-NULL bitmaps expanded from a region's mask words
+  PinBuf region_slots;
   tq_agg_func funcs[AGG_MAXF];
   int arg_type[AGG_MAXF];
   int out_type[AGG_MAXF];
@@ -1504,6 +1507,113 @@ int32_t tq_agg_export_partial(tq_agg *a, tq_column *out_cols, int64_t *n_rows) {
     out_cols[c].offsets = nullptr;
   }
   *n_rows = a->result.n;
+  return TQ_OK;
+}
+
+// The GROUP BY push: every argument is checked before anything is enqueued (a refused push writes no region and publishes no
+// slot); then the export (one host read of the group count, on the compute stream, which it also drains), and on the push
+// stream the destination of every partial row, the scatter into the regions and k_publish_counts.
+int32_t tq_agg_push_partial(tq_agg *a, int32_t n_parts, void *const *dest_data, void *const *dest_counts, int64_t region_cap, int32_t slot,
+                            uint64_t epoch) {
+  if (!a) return TQ_ERR_INVALID_ARG;
+  TQ_TRY(ensure_init());
+  const char *fn = "tq_agg_push_partial";
+  if (a->final_mode) { set_error("%s: a FinalMode handle takes partial rows, it does not make them", fn); return TQ_ERR_STATE; }
+  if (a->merge_mode_seen) { set_error("%s: the handle has merged partial rows; push from a handle fed raw rows", fn); return TQ_ERR_STATE; }
+  if (agg_has_varlen(a)) { set_error("partial export / merge with var-len columns is not supported"); return TQ_ERR_UNSUPPORTED_TYPE; }
+  const int w = partial_width(a), nw = w + 1;
+  if (nw > 64) { set_error("%s: %d partial columns and the mask word exceed 64 words per row", fn, w); return TQ_ERR_INVALID_ARG; }
+  if (!dest_data || !dest_counts || n_parts < 1 || n_parts > 8 || slot < 0 || slot >= PUSH_SLOTS || region_cap < 1 || region_cap > 0xFFFFFFF0ll) {
+    set_error("%s: 1..8 destinations with their regions and count slots, slot 0..%d, 1 <= region_cap < 2^32", fn, PUSH_SLOTS - 1);
+    return TQ_ERR_INVALID_ARG;
+  }
+  for (int q = 0; q < n_parts; q++) {
+    if (!dest_counts[q]) { set_error("%s: destination %d has no count slot", fn, q); return TQ_ERR_INVALID_ARG; }
+    for (int c = 0; c < nw; c++)
+      if (!dest_data[q * nw + c]) { set_error("%s: destination %d has no region for wire column %d", fn, q, c); return TQ_ERR_INVALID_ARG; }
+  }
+  Runtime &r = rt();
+  std::lock_guard<std::recursive_mutex> lk(r.mu);
+  if (!a->eof) TQ_TRY(tq_agg_eof(a));
+  TQ_TRY(agg_finalize(a, true, a->result, w));   // synchronises the compute stream: the partial rows are complete
+  const int64_t n = a->result.n;
+  if (n > 0xFFFFFFF0ll) { set_error("%s: %lld partial rows", fn, (long long)n); return TQ_ERR_INVALID_ARG; }
+  cudaStream_t s = r.h2d;   // the push stream, as tq_partition_push_regions
+  PushSlot *ps = nullptr;
+  TQ_TRY(push_slot_acquire(slot, &ps));
+  for (int q = 0; q < n_parts; q++) ps->h_ptrs.as<void *>()[q] = dest_counts[q];
+  if (n == 0) {
+    TQ_CUDA(cudaMemsetAsync(ps->cursor.p, 0, 64, s));
+    TQ_CUDA(cudaMemsetAsync(ps->ovf.p, 0, 8, s));
+  } else {
+    const size_t tab = (size_t)n_parts * nw * 8;
+    TQ_TRY(ps->out_ptrs.reserve(tab));
+    TQ_TRY(ps->h_out_ptrs.reserve(tab));
+    TQ_TRY(ps->dest.reserve((size_t)n));
+    memcpy(ps->h_out_ptrs.p, dest_data, tab);
+    TQ_CUDA(cudaMemcpyAsync(ps->out_ptrs.p, ps->h_out_ptrs.p, tab, cudaMemcpyHostToDevice, s));
+    DCol cols[64];
+    for (int c = 0; c < w; c++) cols[c] = DCol{a->result.data[c].as<uint64_t>(), a->result.bm[c].as<uint32_t>()};
+    uint32_t real_mask = 0;
+    for (int g = 0; g < a->n_group_by; g++)
+      if (a->types[a->gb_cols[g]] == TQ_TYPE_FLOAT64) real_mask |= 1u << g;
+    TQ_TRY(group_dest(cols, a->n_group_by, real_mask, n, n_parts, ps->dest.as<uint8_t>(), s));
+    TQ_TRY(scatter_to_regions(cols, w, ps->dest.as<uint8_t>(), n, n_parts, ps->out_ptrs.as<uint64_t *>(), region_cap, ps->cursor.as<uint32_t>(),
+                              ps->ovf.as<unsigned long long>(), ps->region, s));
+  }
+  return push_publish(*ps, n_parts, epoch, s);
+}
+
+// The GROUP BY receive: one host read of the slots (queued behind tq_region_wait on the compute stream), then each region's
+// rows straight into the merge update, with the mask words expanded into NOT-NULL bitmaps first.
+int32_t tq_agg_merge_regions(tq_agg *a, int32_t n_regions, const void *slots, int64_t region_cap, const tq_column *regions) {
+  if (!a) return TQ_ERR_INVALID_ARG;
+  TQ_TRY(ensure_init());
+  const char *fn = "tq_agg_merge_regions";
+  if (a->final_mode) { set_error("a FinalMode handle takes its partial rows through tq_agg_put"); return TQ_ERR_STATE; }
+  if (agg_has_varlen(a)) { set_error("partial export / merge with var-len columns is not supported"); return TQ_ERR_UNSUPPORTED_TYPE; }
+  if (a->eof) { set_error("put after eof"); return TQ_ERR_STATE; }
+  if (a->raw_mode_seen) { set_error("one handle cannot mix raw rows and partial rows"); return TQ_ERR_STATE; }
+  const int w = partial_width(a), nw = w + 1;
+  if (nw > 64) { set_error("%s: %d partial columns and the mask word exceed 64 words per row", fn, w); return TQ_ERR_INVALID_ARG; }
+  if (n_regions < 1 || n_regions > 8 || !slots || region_cap < 1 || region_cap > 0xFFFFFFF0ll || !regions) {
+    set_error("%s: 1..8 regions with their slots, 1 <= region_cap < 2^32", fn);
+    return TQ_ERR_INVALID_ARG;
+  }
+  for (int k = 0; k < n_regions * nw; k++)
+    if (!regions[k].data) { set_error("%s: region %d has no data for wire column %d", fn, k / nw, k % nw); return TQ_ERR_INVALID_ARG; }
+  Runtime &r = rt();
+  std::lock_guard<std::recursive_mutex> lk(r.mu);
+  cudaStream_t s = r.compute;
+  TQ_TRY(a->region_slots.reserve((size_t)n_regions * 16));
+  TQ_CUDA(cudaMemcpyAsync(a->region_slots.p, slots, (size_t)n_regions * 16, cudaMemcpyDeviceToHost, s));
+  TQ_CUDA(cudaStreamSynchronize(s));
+  const unsigned long long *sl = a->region_slots.as<unsigned long long>();
+  int64_t rows[8], most = 0;
+  for (int g = 0; g < n_regions; g++) {
+    if (sl[2 * g] > (unsigned long long)region_cap) {
+      set_error("%s: a region overflowed (its slot reads more than %lld rows)", fn, (long long)region_cap);
+      return TQ_ERR_OOM;
+    }
+    rows[g] = (int64_t)sl[2 * g];
+    if (rows[g] > most) most = rows[g];
+  }
+  a->merge_mode_seen = true;
+  if (most == 0) return TQ_OK;
+  TQ_TRY(agg_flush_stage(a, true, w));
+  if ((int)a->region_bm.size() < w) a->region_bm.resize(w);
+  for (int c = 0; c < w; c++) TQ_TRY(a->region_bm[c].reserve(bitmap_alloc_bytes(most)));
+  std::vector<uint32_t *> bm(w);
+  for (int c = 0; c < w; c++) bm[c] = a->region_bm[c].as<uint32_t>();
+  std::vector<DCol> view(w);
+  for (int g = 0; g < n_regions; g++) {
+    if (rows[g] == 0) continue;
+    const tq_column *reg = regions + (size_t)g * nw;
+    TQ_TRY(expand_null_mask((const uint64_t *)reg[w].data, rows[g], w, bm.data(), s));
+    for (int c = 0; c < w; c++) view[c] = DCol{(const uint64_t *)reg[c].data, a->region_bm[c].as<uint32_t>()};
+    a->rows_total += rows[g];
+    TQ_TRY(agg_update_device(a, view.data(), w, rows[g], true));   // in stream order after the expansion; it synchronises
+  }
   return TQ_OK;
 }
 

@@ -30,6 +30,7 @@
 #include "dict.cuh"
 #include "varlen.cuh"
 #include "strdict.cuh"
+#include "push.cuh"
 #include "scatter.cuh"
 #include "othercond.cuh"
 #include "nlj.cuh"
@@ -3666,42 +3667,8 @@ int32_t tq_join_build_path(tq_join *j, int32_t *path) {
 // straight into "its" region on every peer (stores over NVLink) and then publishes how many rows it wrote to each peer in
 // that peer's count table (one 8-byte peer store per destination).  The receiver joins the regions as ONE segmented batch
 // (tq_join_put_probe_segments) whose kernels read the counts from device memory — between the exchange and the join there
-// is no host round trip, only the cross-rank barrier that says "all pushes of this chunk have landed".
-static constexpr int PUSH_SLOTS = 16;
-// One 16-byte slot per (destination, table, source): {rows written, epoch}.  The count is stored first, the epoch flag after a
-// system-scope fence: a receiver that sees the flag sees the count, and — the push kernel having completed before this
-// kernel started — the rows.
-__global__ void k_publish_counts(const uint32_t *cursor, const unsigned long long *overflow, int n_parts, unsigned long long *const *dest_slots,
-                                 unsigned long long epoch) {
-  const int q = threadIdx.x;
-  if (q < n_parts) {
-    volatile unsigned long long *slot = dest_slots[q];
-    slot[0] = *overflow ? ~0ull : (unsigned long long)cursor[q];
-    __threadfence_system();
-    slot[1] = epoch;
-  }
-}
-// Device-side wait for the peers: spins (bounded: ~4 s) until the n slots of this rank's table carry `epoch`.  Enqueued on the
-// compute stream in front of the kernels that read the regions, so the exchange needs no host barrier.
-__global__ void k_region_wait(const unsigned long long *slots, int n, unsigned long long epoch, unsigned *timed_out) {
-  const int g = threadIdx.x;
-  if (g >= n) return;
-  const volatile unsigned long long *flag = slots + 2 * g + 1;
-  unsigned long long t0;
-  asm volatile("mov.u64 %0, %%globaltimer;" : "=l"(t0));
-  while (*flag < epoch) {
-    __nanosleep(500);
-    unsigned long long t1;
-    asm volatile("mov.u64 %0, %%globaltimer;" : "=l"(t1));
-    if (t1 - t0 > 4000000000ull) { atomicOr(timed_out, 1u << g); return; }
-  }
-}
-struct PushSlot {
-  DevBuf cursor, lim, ovf, counts_ptrs, mask, sel;
-  PinBuf h_lim, h_ptrs;
-  cudaEvent_t ev = nullptr;
-};
-static PushSlot g_push_slot[PUSH_SLOTS];
+// is no host round trip, only the cross-rank barrier that says "all pushes of this chunk have landed".  The slots and the
+// device-side wait live in push.cu.
 
 // One region push (include/tinysql_b200.h): every argument is checked before anything is enqueued, so a refused push writes
 // no region and publishes no slot.  Then the scatter of n rows into n_parts destinations (+ the miss bin with keep_misses)
@@ -3750,15 +3717,9 @@ int32_t tq_partition_push_regions(int32_t n_cols, const tq_column *cols, int32_t
   Runtime &r = rt();
   std::lock_guard<std::recursive_mutex> lk(r.mu);
   cudaStream_t s = r.h2d;  // the push stream: rows cross NVLink while the compute stream joins what has already arrived
-  PushSlot &ps = g_push_slot[slot];
-  if (!ps.ev) TQ_CUDA(cudaEventCreateWithFlags(&ps.ev, cudaEventDisableTiming));
-  TQ_TRY(ps.cursor.reserve(64));
-  TQ_TRY(ps.lim.reserve(64));
-  TQ_TRY(ps.ovf.reserve(8));
-  TQ_TRY(ps.counts_ptrs.reserve(128));
-  TQ_TRY(ps.h_lim.reserve(64));
-  TQ_TRY(ps.h_ptrs.reserve(128));
-  TQ_CUDA(cudaEventSynchronize(ps.ev));  // the previous push of this slot no longer reads the pinned tables or the mask below
+  PushSlot *slot_state = nullptr;
+  TQ_TRY(push_slot_acquire(slot, &slot_state));  // the previous push of this slot no longer reads the pinned tables or the mask below
+  PushSlot &ps = *slot_state;
   const int n_pub = n_parts + (keep_misses ? 1 : 0);
   for (int q = 0; q < 16; q++) ps.h_lim.as<uint32_t>()[q] = (uint32_t)region_cap;
   for (int q = 0; q < n_parts; q++) ps.h_ptrs.as<void *>()[q] = dest_counts[q];
@@ -3769,7 +3730,6 @@ int32_t tq_partition_push_regions(int32_t n_cols, const tq_column *cols, int32_t
   TQ_CUDA(cudaMemsetAsync(ps.cursor.p, 0, 64, s));
   TQ_CUDA(cudaMemsetAsync(ps.ovf.p, 0, 8, s));
   TQ_CUDA(cudaMemcpyAsync(ps.lim.p, ps.h_lim.p, 64, cudaMemcpyHostToDevice, s));
-  TQ_CUDA(cudaMemcpyAsync(ps.counts_ptrs.p, ps.h_ptrs.p, 128, cudaMemcpyHostToDevice, s));
   if (n > 0) {
     if (pack) {  // the mask word and the effective selection first
       TQ_TRY(ps.mask.reserve((size_t)n * 8));
@@ -3783,30 +3743,7 @@ int32_t tq_partition_push_regions(int32_t n_cols, const tq_column *cols, int32_t
     sp.overflow = ps.ovf.as<unsigned long long>();
     TQ_TRY(launch_scatter_fast(sp, s, "k_probe_scatter_fast(push regions)"));
   }
-  k_publish_counts<<<1, 32, 0, s>>>(ps.cursor.as<uint32_t>(), ps.ovf.as<unsigned long long>(), n_pub, ps.counts_ptrs.as<unsigned long long *>(), epoch);
-  count_launch();
-  TQ_TRY(check_launch("k_publish_counts"));
-  TQ_CUDA(cudaEventRecord(ps.ev, s));
-  return TQ_OK;
-}
-
-int32_t tq_region_wait(const void *slots, int32_t n_sources, uint64_t epoch) {
-  TQ_TRY(ensure_init());
-  if (!slots || n_sources < 1 || n_sources > 32) return TQ_ERR_INVALID_ARG;
-  Runtime &r = rt();
-  std::lock_guard<std::recursive_mutex> lk(r.mu);
-  static DevBuf timed_out;
-  if (!timed_out.p) { TQ_TRY(timed_out.reserve(8)); TQ_CUDA(cudaMemsetAsync(timed_out.p, 0, 8, r.compute)); }
-  k_region_wait<<<1, 32, 0, r.compute>>>(reinterpret_cast<const unsigned long long *>(slots), n_sources, epoch, timed_out.as<unsigned>());
-  count_launch();
-  return check_launch("k_region_wait");
-}
-
-int32_t tq_partition_push_sync(int32_t slot) {
-  TQ_TRY(ensure_init());
-  if (slot < 0 || slot >= PUSH_SLOTS || !g_push_slot[slot].ev) return TQ_ERR_INVALID_ARG;
-  TQ_CUDA(cudaEventSynchronize(g_push_slot[slot].ev));
-  return TQ_OK;
+  return push_publish(ps, n_pub, epoch, s);
 }
 
 int32_t tq_join_destroy(tq_join *j) {

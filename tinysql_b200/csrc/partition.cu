@@ -4,6 +4,9 @@
 // (partition-major, chunk-minor) counts, ordered scatter of every column.
 // Also both ends of the nullable region exchange: the mask word a pushing rank packs (k_pack_null_mask) and the receiver's
 // tq_region_gather, which copies the arrived regions into contiguous columns and expands the mask word into NULL bitmaps.
+// And the GROUP BY push's kernels (tq_agg_push_partial): the destination of a partial row from its group, the same histogram /
+// scan / scatter writing each destination's run column-wise into that destination's region with the mask word packed on the
+// way, and the mask word's expansion into NULL bitmaps on the receiving side.
 #include "scatter.cuh"
 
 namespace tq {
@@ -12,6 +15,12 @@ static constexpr int PART_MAXC = 16;
 static constexpr int PART_MAX = 256;
 static constexpr int PART_CHUNK = 2048;  // rows owned by one warp, walked in order (=> stable)
 
+// k_part_hist / k_part_scatter take their routing and their stores from the parameter struct (the policy):
+//   dest_of(r)         destination of row r
+//   run_base(q)        subtracted from destination q's scanned offsets (0: one output array; its first offset: one region per q)
+//   store(r, q, pos)   writes row r at position pos of destination q
+// PartParams is tq_partition_device (destination from the key's hash, every column into one output array at the global offset);
+// RegionParams is the GROUP BY push (destination from an array, column-wise into per-destination regions with the mask word).
 struct PartParams {
   int n_cols;
   DCol in[PART_MAXC];
@@ -21,14 +30,49 @@ struct PartParams {
   int64_t n;
   int64_t n_chunks;
   uint32_t *counts;  // [part * n_chunks + chunk]
+
+  __device__ __forceinline__ int dest_of(int64_t r) const {
+    if (!tqd::bm_not_null(in[key_col].bm, r)) return (int)(r % n_parts);  // NULL keys never match; spread them
+    return (int)((tqd::mix64(in[key_col].data[r]) >> 40) % (uint64_t)n_parts);
+  }
+  __device__ __forceinline__ uint32_t run_base(int) const { return 0; }
+  __device__ __forceinline__ void store(int64_t r, int, uint32_t pos) const {
+    for (int c = 0; c < n_cols; c++) {
+      out[c].data[pos] = in[c].data[r];
+      if (out[c].bm && tqd::bm_not_null(in[c].bm, r)) atomicOr(&out[c].bm[pos >> 5], 1u << (pos & 31));
+    }
+  }
 };
 
-__device__ __forceinline__ int part_of(const PartParams &p, int64_t r) {
-  if (!tqd::bm_not_null(p.in[p.key_col].bm, r)) return (int)(r % p.n_parts);  // NULL keys never match; spread them
-  return (int)((tqd::mix64(p.in[p.key_col].data[r]) >> 40) % (uint64_t)p.n_parts);
-}
+static constexpr int REGION_MAXW = 63;  // wire columns before the mask word: the mask's 64 bits cover them
 
-__global__ void __launch_bounds__(256) k_part_hist(const PartParams p) {
+struct RegionParams {
+  int n_cols;  // wire columns before the mask word
+  int n_parts;
+  int64_t n;
+  int64_t n_chunks;
+  uint32_t *counts;
+  DCol in[REGION_MAXW];
+  const uint8_t *dest;
+  uint64_t *const *out;  // DEVICE table: out[q * (n_cols + 1) + c] = destination q's region of wire column c, the mask word last
+  uint32_t cap;          // rows per region: a row at or past it is not written (the push publishes ~0)
+
+  __device__ __forceinline__ int dest_of(int64_t r) const { return dest[r]; }
+  __device__ __forceinline__ uint32_t run_base(int q) const { return counts[(int64_t)q * n_chunks]; }
+  __device__ __forceinline__ void store(int64_t r, int q, uint32_t pos) const {
+    if (pos >= cap) return;
+    uint64_t *const *o = out + (int64_t)q * (n_cols + 1);
+    uint64_t m = 0;
+    for (int c = 0; c < n_cols; c++) {
+      o[c][pos] = in[c].data[r];
+      m |= (uint64_t)tqd::bm_not_null(in[c].bm, r) << c;
+    }
+    o[n_cols][pos] = m;
+  }
+};
+
+template <class P>
+__global__ void __launch_bounds__(256) k_part_hist(const P p) {
   __shared__ uint32_t s_cnt[8][PART_MAX];
   const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
   const int64_t chunk = (int64_t)blockIdx.x * 8 + warp;
@@ -37,25 +81,26 @@ __global__ void __launch_bounds__(256) k_part_hist(const PartParams p) {
   if (chunk < p.n_chunks) {
     const int64_t lo = chunk * PART_CHUNK;
     const int64_t hi = lo + PART_CHUNK < p.n ? lo + PART_CHUNK : p.n;
-    for (int64_t r = lo + lane; r < hi; r += 32) atomicAdd(&s_cnt[warp][part_of(p, r)], 1u);
+    for (int64_t r = lo + lane; r < hi; r += 32) atomicAdd(&s_cnt[warp][p.dest_of(r)], 1u);
     __syncwarp();
     for (int i = lane; i < p.n_parts; i += 32) p.counts[(int64_t)i * p.n_chunks + chunk] = s_cnt[warp][i];
   }
 }
 
-__global__ void __launch_bounds__(256) k_part_scatter(const PartParams p) {
+template <class P>
+__global__ void __launch_bounds__(256) k_part_scatter(const P p) {
   __shared__ uint32_t s_base[8][PART_MAX];
   const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
   const int64_t chunk = (int64_t)blockIdx.x * 8 + warp;
   if (chunk >= p.n_chunks) return;
-  for (int i = lane; i < p.n_parts; i += 32) s_base[warp][i] = p.counts[(int64_t)i * p.n_chunks + chunk];  // scanned: global offsets
+  for (int i = lane; i < p.n_parts; i += 32) s_base[warp][i] = p.counts[(int64_t)i * p.n_chunks + chunk] - p.run_base(i);  // scanned offsets
   __syncwarp();
   const int64_t lo = chunk * PART_CHUNK;
   const int64_t hi = lo + PART_CHUNK < p.n ? lo + PART_CHUNK : p.n;
   for (int64_t r0 = lo; r0 < hi; r0 += 32) {
     const int64_t r = r0 + lane;
     const bool active = r < hi;
-    const int part = active ? part_of(p, r) : -1;
+    const int part = active ? p.dest_of(r) : -1;
     const unsigned peers = __match_any_sync(0xffffffffu, part);
     const unsigned rank = __popc(peers & ((1u << lane) - 1));
     uint32_t pos = 0;
@@ -63,12 +108,7 @@ __global__ void __launch_bounds__(256) k_part_scatter(const PartParams p) {
     __syncwarp();
     if (active && rank == (unsigned)__popc(peers) - 1) s_base[warp][part] = pos + 1;  // last peer advances the cursor
     __syncwarp();
-    if (active) {
-      for (int c = 0; c < p.n_cols; c++) {
-        p.out[c].data[pos] = p.in[c].data[r];
-        if (p.out[c].bm && tqd::bm_not_null(p.in[c].bm, r)) atomicOr(&p.out[c].bm[pos >> 5], 1u << (pos & 31));
-      }
-    }
+    if (active) p.store(r, part, pos);
   }
 }
 
@@ -170,6 +210,123 @@ __global__ void __launch_bounds__(256) k_region_gather(const GatherParams p) {
   }
 }
 
+// ---- the GROUP BY push (tq_agg_push_partial, agg.cu): destination per partial row, scatter into the regions, mask expansion
+struct GroupDestParams {
+  int n_items, n_parts;
+  uint32_t real_mask;  // bit g: item g is REAL
+  DCol item[GROUP_MAX_ITEMS];
+  int64_t n;
+  uint8_t *dest;
+};
+
+__global__ void __launch_bounds__(256) k_group_dest(const GroupDestParams p) {
+  for (int64_t r = (int64_t)blockIdx.x * blockDim.x + threadIdx.x; r < p.n; r += (int64_t)gridDim.x * blockDim.x) {
+    uint64_t h = 0;
+    for (int g = 0; g < p.n_items; g++) {
+      uint64_t v = GROUP_NULL_WORD;
+      if (tqd::bm_not_null(p.item[g].bm, r)) {
+        v = p.item[g].data[r];
+        if (((p.real_mask >> g) & 1) && v == 0x8000000000000000ull) v = 0;  // -0.0 and +0.0 are one group
+      }
+      h = tqd::mix64(h ^ v);
+    }
+    p.dest[r] = (uint8_t)((h >> 40) % (uint64_t)p.n_parts);
+  }
+}
+
+int32_t group_dest(const DCol *items, int n_items, uint32_t real_mask, int64_t n, int n_parts, uint8_t *dest, cudaStream_t s) {
+  if (n_items < 0 || n_items > GROUP_MAX_ITEMS || n_parts < 1 || n_parts > 8 || n < 1) { set_error("internal: group_dest arguments"); return TQ_ERR_INVALID_ARG; }
+  GroupDestParams p{};
+  p.n_items = n_items;
+  p.n_parts = n_parts;
+  p.real_mask = real_mask;
+  for (int g = 0; g < n_items; g++) p.item[g] = items[g];
+  p.n = n;
+  p.dest = dest;
+  const int64_t blocks = (n + 255) / 256, cap = (int64_t)rt().sm_count * 8;
+  TQ_LAUNCH(k_group_dest, (unsigned)(blocks < cap ? blocks : cap), 256, 0, s, p);
+  count_launch();
+  return check_launch("k_group_dest");
+}
+
+// rows[q] = rows destined to q (from the scanned histogram and its total), *overflow = some rows[q] > cap
+__global__ void k_region_rows(const uint32_t *scanned, int64_t n_chunks, int n_parts, const uint64_t *total, uint32_t cap, uint32_t *rows,
+                              unsigned long long *overflow) {
+  if (threadIdx.x != 0) return;
+  unsigned long long ovf = 0;
+  for (int q = 0; q < n_parts; q++) {
+    const uint64_t end = q + 1 < n_parts ? scanned[(int64_t)(q + 1) * n_chunks] : *total;
+    rows[q] = (uint32_t)(end - scanned[(int64_t)q * n_chunks]);
+    ovf |= rows[q] > cap ? 1ull : 0ull;
+  }
+  *overflow = ovf;
+}
+
+int32_t scatter_to_regions(const DCol *cols, int n_cols, const uint8_t *dest, int64_t n, int n_parts, uint64_t *const *out, int64_t cap,
+                           uint32_t *rows, unsigned long long *overflow, RegionScratch &sc, cudaStream_t s) {
+  if (n_cols < 1 || n_cols > REGION_MAXW || n_parts < 1 || n_parts > 8 || n < 1 || n > 0xFFFFFFF0ll || cap < 1 || cap > 0xFFFFFFF0ll) {
+    set_error("internal: scatter_to_regions arguments");
+    return TQ_ERR_INVALID_ARG;
+  }
+  RegionParams p{};
+  p.n_cols = n_cols;
+  p.n_parts = n_parts;
+  p.n = n;
+  p.n_chunks = (n + PART_CHUNK - 1) / PART_CHUNK;
+  for (int c = 0; c < n_cols; c++) p.in[c] = cols[c];
+  p.dest = dest;
+  p.out = out;
+  p.cap = (uint32_t)cap;
+  const int64_t n_counts = p.n_chunks * n_parts;
+  TQ_TRY(sc.hist.reserve((size_t)n_counts * 4));
+  TQ_TRY(sc.total.reserve(8));
+  p.counts = sc.hist.as<uint32_t>();
+  const unsigned blocks = (unsigned)((p.n_chunks + 7) / 8);
+  TQ_LAUNCH(k_part_hist<RegionParams>, blocks, 256, 0, s, p);
+  count_launch();
+  TQ_TRY(check_launch("k_part_hist(regions)"));
+  TQ_TRY(exclusive_scan_u32(p.counts, 1, p.counts, 1, n_counts, sc.total.as<uint64_t>(), sc.scan, s));
+  TQ_LAUNCH(k_region_rows, 1, 32, 0, s, p.counts, p.n_chunks, n_parts, sc.total.as<uint64_t>(), p.cap, rows, overflow);
+  TQ_LAUNCH(k_part_scatter<RegionParams>, blocks, 256, 0, s, p);
+  count_launch(2);
+  return check_launch("k_part_scatter(regions)");
+}
+
+struct ExpandParams {
+  int n_cols;
+  const uint64_t *mask;
+  int64_t n;
+  uint32_t *bm[REGION_MAXW];
+};
+
+// One warp covers 32 consecutive rows: one ballot per column = one bitmap word.  Words are written for the whole 64-row groups
+// that hold the rows, 0 past the last row.
+__global__ void __launch_bounds__(256) k_expand_mask(const ExpandParams p) {
+  const int64_t padded = (p.n + 63) & ~63ll;
+  const int lane = threadIdx.x & 31;
+  for (int64_t base = (int64_t)blockIdx.x * blockDim.x; base < padded; base += (int64_t)gridDim.x * blockDim.x) {
+    const int64_t r = base + threadIdx.x;
+    const uint64_t m = r < p.n ? p.mask[r] : 0;
+    for (int c = 0; c < p.n_cols; c++) {
+      const unsigned w = __ballot_sync(0xffffffffu, (m >> c) & 1);
+      if (lane == 0 && r < padded) p.bm[c][r >> 5] = w;
+    }
+  }
+}
+
+int32_t expand_null_mask(const uint64_t *mask, int64_t n, int n_cols, uint32_t *const *bm, cudaStream_t s) {
+  if (n_cols < 1 || n_cols > REGION_MAXW || n < 1) { set_error("internal: expand_null_mask arguments"); return TQ_ERR_INVALID_ARG; }
+  ExpandParams p{};
+  p.n_cols = n_cols;
+  p.mask = mask;
+  p.n = n;
+  for (int c = 0; c < n_cols; c++) p.bm[c] = bm[c];
+  const int64_t blocks = ((n + 63) / 64 * 64 + 255) / 256, cap = (int64_t)rt().sm_count * 8;
+  TQ_LAUNCH(k_expand_mask, (unsigned)(blocks < cap ? blocks : cap), 256, 0, s, p);
+  count_launch();
+  return check_launch("k_expand_mask");
+}
+
 }  // namespace tq
 
 using namespace tq;
@@ -220,12 +377,12 @@ extern "C" int32_t tq_partition_device(int32_t n_cols, const tq_column *cols, co
   TQ_TRY(h_off.reserve((size_t)(n_parts + 1) * 8));
   p.counts = counts.as<uint32_t>();
   const unsigned blocks = (unsigned)((p.n_chunks + 7) / 8);
-  TQ_LAUNCH(k_part_hist, blocks, 256, 0, s, p);
+  TQ_LAUNCH(k_part_hist<PartParams>, blocks, 256, 0, s, p);
   count_launch();
   TQ_TRY(check_launch("k_part_hist"));
   TQ_TRY(exclusive_scan_u32(p.counts, 1, p.counts, 1, n_counts, nullptr, scan_scratch, s));
   TQ_LAUNCH(k_part_offsets, (n_parts + 1 + 255) / 256, 256, 0, s, p.counts, p.n_chunks, n_parts, n, d_off.as<int64_t>());
-  TQ_LAUNCH(k_part_scatter, blocks, 256, 0, s, p);
+  TQ_LAUNCH(k_part_scatter<PartParams>, blocks, 256, 0, s, p);
   count_launch(2);
   TQ_TRY(check_launch("k_part_scatter"));
   TQ_CUDA(cudaMemcpyAsync(h_off.p, d_off.p, (size_t)(n_parts + 1) * 8, cudaMemcpyDeviceToHost, s));

@@ -1,0 +1,86 @@
+// push.cu — the publish / wait halves of the region exchange (push.cuh), shared by the join's and the GROUP BY's pushes.
+#include "push.cuh"
+
+namespace tq {
+
+// One 16-byte slot per (destination, table, source): {rows written, epoch}.  The count is stored first, the epoch flag after a
+// system-scope fence: a receiver that sees the flag sees the count, and — the push kernel having completed before this
+// kernel started — the rows.
+__global__ void k_publish_counts(const uint32_t *cursor, const unsigned long long *overflow, int n_parts, unsigned long long *const *dest_slots,
+                                 unsigned long long epoch) {
+  const int q = threadIdx.x;
+  if (q < n_parts) {
+    volatile unsigned long long *slot = dest_slots[q];
+    slot[0] = *overflow ? ~0ull : (unsigned long long)cursor[q];
+    __threadfence_system();
+    slot[1] = epoch;
+  }
+}
+
+// Device-side wait for the peers: spins (bounded: ~4 s) until the n slots of this rank's table carry `epoch`.  Enqueued on the
+// compute stream in front of the kernels that read the regions, so the exchange needs no host barrier.
+__global__ void k_region_wait(const unsigned long long *slots, int n, unsigned long long epoch, unsigned *timed_out) {
+  const int g = threadIdx.x;
+  if (g >= n) return;
+  const volatile unsigned long long *flag = slots + 2 * g + 1;
+  unsigned long long t0;
+  asm volatile("mov.u64 %0, %%globaltimer;" : "=l"(t0));
+  while (*flag < epoch) {
+    __nanosleep(500);
+    unsigned long long t1;
+    asm volatile("mov.u64 %0, %%globaltimer;" : "=l"(t1));
+    if (t1 - t0 > 4000000000ull) { atomicOr(timed_out, 1u << g); return; }
+  }
+}
+
+static PushSlot g_push_slot[PUSH_SLOTS];
+
+int32_t push_slot_acquire(int slot, PushSlot **out) {
+  PushSlot &ps = g_push_slot[slot];
+  if (!ps.ev) TQ_CUDA(cudaEventCreateWithFlags(&ps.ev, cudaEventDisableTiming));
+  TQ_TRY(ps.cursor.reserve(64));
+  TQ_TRY(ps.lim.reserve(64));
+  TQ_TRY(ps.ovf.reserve(8));
+  TQ_TRY(ps.counts_ptrs.reserve(128));
+  TQ_TRY(ps.h_lim.reserve(64));
+  TQ_TRY(ps.h_ptrs.reserve(128));
+  TQ_CUDA(cudaEventSynchronize(ps.ev));  // the previous push of this slot no longer reads the pinned tables or the scratch
+  *out = &ps;
+  return TQ_OK;
+}
+
+int32_t push_publish(PushSlot &ps, int n_pub, uint64_t epoch, cudaStream_t s) {
+  TQ_CUDA(cudaMemcpyAsync(ps.counts_ptrs.p, ps.h_ptrs.p, 128, cudaMemcpyHostToDevice, s));
+  k_publish_counts<<<1, 32, 0, s>>>(ps.cursor.as<uint32_t>(), ps.ovf.as<unsigned long long>(), n_pub, ps.counts_ptrs.as<unsigned long long *>(), epoch);
+  count_launch();
+  TQ_TRY(check_launch("k_publish_counts"));
+  TQ_CUDA(cudaEventRecord(ps.ev, s));
+  return TQ_OK;
+}
+
+}  // namespace tq
+
+using namespace tq;
+
+extern "C" {
+
+int32_t tq_region_wait(const void *slots, int32_t n_sources, uint64_t epoch) {
+  TQ_TRY(ensure_init());
+  if (!slots || n_sources < 1 || n_sources > 32) return TQ_ERR_INVALID_ARG;
+  Runtime &r = rt();
+  std::lock_guard<std::recursive_mutex> lk(r.mu);
+  static DevBuf timed_out;
+  if (!timed_out.p) { TQ_TRY(timed_out.reserve(8)); TQ_CUDA(cudaMemsetAsync(timed_out.p, 0, 8, r.compute)); }
+  k_region_wait<<<1, 32, 0, r.compute>>>(reinterpret_cast<const unsigned long long *>(slots), n_sources, epoch, timed_out.as<unsigned>());
+  count_launch();
+  return check_launch("k_region_wait");
+}
+
+int32_t tq_partition_push_sync(int32_t slot) {
+  TQ_TRY(ensure_init());
+  if (slot < 0 || slot >= PUSH_SLOTS || !g_push_slot[slot].ev) return TQ_ERR_INVALID_ARG;
+  TQ_CUDA(cudaEventSynchronize(g_push_slot[slot].ev));
+  return TQ_OK;
+}
+
+}  // extern "C"

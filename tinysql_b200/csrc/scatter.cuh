@@ -27,4 +27,26 @@ static constexpr int SCATTER_AOS_MAX_PBITS = 9;
 int32_t pack_null_mask(const DCol *cols, int n_cols, int key_col, const uint8_t *selected, int64_t n, uint64_t *mask, uint8_t *sel_out,
                        cudaStream_t s);
 
+// ---- the GROUP BY push (partition.cu; tq_agg_push_partial in agg.cu)
+// Destination of a partial row, a pure function of its group: h = 0, then per GROUP BY item g  h = mix64(h ^ v_g), where v_g
+// is the item's 8 bytes (a REAL item with -0.0 read as +0.0) or GROUP_NULL_WORD for a NULL item; destination = (h >> 40) %
+// n_parts.  One NOT NULL item gives (mix64(v) >> 40) % n_parts, the join's rank of the same key; no item (a scalar aggregate)
+// gives 0.  Only placement depends on the rule — equality of groups is decided by the merge — so a collision costs nothing.
+static constexpr int GROUP_MAX_ITEMS = 8;
+static constexpr uint64_t GROUP_NULL_WORD = 0x4E554C4C4E554C4Cull;
+// dest[r] for n >= 1 rows; items: the n_items GROUP BY columns (device), real_mask bit g = item g is REAL.  Enqueued on s.
+int32_t group_dest(const DCol *items, int n_items, uint32_t real_mask, int64_t n, int n_parts, uint8_t *dest, cudaStream_t s);
+struct RegionScratch {
+  DevBuf hist, scan, total;
+};
+// Scatters n >= 1 rows of n_cols (1..63) 8-byte columns to destination dest[r] < n_parts (<= 8): row i of destination q's run
+// (input order) goes to out[q * (n_cols + 1) + c][i] for every column c, the mask word (bit c = column c is NOT NULL) to
+// out[q * (n_cols + 1) + n_cols][i].  out is a DEVICE table of pointers.  rows[q] (device u32) = rows destined to q,
+// *overflow (device u64) = 1 when some rows[q] > cap, 0 otherwise; rows at or past cap are not written.  Enqueued on s.
+int32_t scatter_to_regions(const DCol *cols, int n_cols, const uint8_t *dest, int64_t n, int n_parts, uint64_t *const *out, int64_t cap,
+                           uint32_t *rows, unsigned long long *overflow, RegionScratch &sc, cudaStream_t s);
+// The receiving side: bitmap bm[c] (a host array of n_cols <= 63 device bitmaps) gets bit c of mask[r] for the n >= 1 rows, whole 64-row
+// groups, 0 past the last row.  Enqueued on s.
+int32_t expand_null_mask(const uint64_t *mask, int64_t n, int n_cols, uint32_t *const *bm, cudaStream_t s);
+
 }  // namespace tq

@@ -1,13 +1,19 @@
-"""Multi-GPU hash join: radix-partition both sides on the join key across the ranks, exchange the partitions, run the
-single-GPU join on what arrived.  One process per GPU; torch.distributed is plumbing only (process group, barriers, the NCCL
-variant); partitioning, exchange and join are the CUDA kernels of libtinysql_b200.so.
+"""Multi-GPU hash join and GROUP BY: radix-partition the rows (the join's) or the partial groups (the GROUP BY's) on the key
+across the ranks, exchange the partitions, run the single-GPU operator on what arrived.  One process per GPU;
+torch.distributed is plumbing only (process group, barriers, the NCCL variant); partitioning, exchange, join and aggregation
+are the CUDA kernels of libtinysql_b200.so.
 
 Two exchanges:
-  * RegionExchange / RegionJoin (the default of bench.py --gpus N): the scatter kernel stores every row straight into the
-    destination rank's receive region over NVLink peer memory (CUDA IPC), chunk by chunk, overlapped with the local join of
-    the chunks that have already arrived; device-side epoch flags replace host barriers.
+  * RegionExchange: the scatter kernel stores every row straight into the destination rank's receive region over NVLink peer
+    memory (CUDA IPC); device-side epoch flags replace host barriers.
+      - RegionJoin (the default of bench.py --gpus N): chunk by chunk, overlapped with the local join of the chunks that have
+        already arrived.
+      - RegionAgg: each rank's Partial1 aggregation pushes its partial rows (tq_agg_push_partial, NULL mask word included, any
+        number of GROUP BY items) to the rank its group names; that rank merges the regions in place
+        (tq_agg_merge_regions) and finalises.
   * exchange() (distributed_join / distributed_agg): partition locally, then ONE grouped NCCL send/recv — the all-to-all at the
-    shard boundary (NCCL 2.27/2.28 has no ncclAllToAllv); also what the gloo CPU tests drive.
+    shard boundary (NCCL 2.27/2.28 has no ncclAllToAllv); also what the gloo CPU tests drive.  distributed_agg takes one
+    NOT NULL GROUP BY item.
 
 The moral equivalent of the reference's partial->final hash shuffle (executor/aggregate.go:96-133,352-356): a row goes to
 rank  (mix64(key) >> 40) % world  — a pure function of its key, so equal keys meet on one rank and nothing else moves.
@@ -608,6 +614,127 @@ class RegionJoin:
         L.check(self.lib.tq_region_gather(1, C.c_void_p(self.miss_slot[c]), max(self.chunk_max, 1), len(self.probe_types), self.pmask, regs,
                                           self.g_miss[0], self.g_miss[1], C.byref(n)))
         return n.value
+
+
+def agg_drain(lib, L, h, n_funcs):
+    """the finished groups of an aggregation handle after tq_agg_eof, as host Columns: tq_agg_next_device, and — when it has
+    no groups — tq_agg_next, which returns the one default row of a scalar aggregate over no rows (COUNT 0, the rest NULL)"""
+    from .chunk import Column, device_to_host
+    types = []
+    for i in range(n_funcs):
+        t = C.c_int32(0)
+        L.check(lib.tq_agg_output_type(h, i, C.byref(t)))
+        types.append(t.value)
+    out = (L.TQColumn * max(n_funcs, 1))()
+    rows, eof = C.c_int64(0), C.c_int32(0)
+    L.check(lib.tq_agg_next_device(h, out, C.byref(rows), C.byref(eof)))
+    if rows.value:
+        return [device_to_host(types[i], out[i].data, out[i].null_bitmap, rows.value) for i in range(n_funcs)]
+    data = [np.zeros(1, np.uint64) for _ in range(n_funcs)]
+    bms = [np.zeros(8, np.uint8) for _ in range(n_funcs)]
+    for i in range(n_funcs):
+        out[i].data, out[i].null_bitmap, out[i].offsets = data[i].ctypes.data, bms[i].ctypes.data, None
+    L.check(lib.tq_agg_next(h, 1, out, C.byref(rows), C.byref(eof)))
+    if rows.value == 0:
+        return [Column.empty(t, 0) for t in types]
+    return [Column(t, data[i].view(np.float64 if t == L.TQ_TYPE_FLOAT64 else (np.uint64 if t == L.TQ_TYPE_UINT64 else np.int64)),
+                   np.array([bool(bms[i][0] & 1)])) for i, t in enumerate(types)]
+
+
+class RegionAgg:
+    """The multi-GPU GROUP BY over a RegionExchange of one table: w + 1 wire columns (w = tq_agg_partial_width: the partial
+    row, then its NULL mask word).  One step:
+
+        this rank      Partial1 handle <- tq_agg_put(shard) -> eof -> tq_agg_push_partial        (push stream)
+        compute stream tq_region_wait -> Final handle <- tq_agg_merge_regions -> eof -> next_device
+
+    A partial group travels to the rank its group names (tq_agg_push_partial: with one NOT NULL item the rank the join sends
+    that key to), so every group is finished on exactly one rank; a scalar aggregate is finished on rank 0 only, which returns
+    its one row even when every shard is empty.  Host synchronisation per step: the export's group count, the merge's slot
+    read, the result drain and ONE barrier at the end (nobody may push into a region a peer is still merging)."""
+
+    def __init__(self, lib, L, world, rank, types, group_by, funcs, max_groups_per_rank, slack=1.25, est_groups=0, slot=0):
+        """types: TQ_TYPE_* per input column (| TQ_TYPE_NOT_NULL where declared so); group_by: input column indices;
+        funcs: [(TQ_AGG_*, arg_col)].  max_groups_per_rank: the most groups one rank's shard holds (every rank passes the same
+        numbers: the layout is shared)."""
+        self.lib, self.L, self.world, self.rank, self.slot = lib, L, world, rank, slot
+        self.types, self.group_by, self.funcs, self.est_groups = list(types), list(group_by), list(funcs), est_groups
+        h, keep = self._create()
+        try:
+            width = C.c_int32(0)
+            L.check(lib.tq_agg_partial_width(h, C.byref(width)))
+        finally:
+            lib.tq_agg_destroy(h)
+        self.width = width.value
+        if self.width + 1 > 64:
+            raise ValueError(f"RegionAgg: {self.width} partial columns and the mask word exceed 64 words per row")
+        # a group lands on one rank by its hash: +25 % covers the imbalance between (source, destination) pairs
+        cap = 1 if not group_by else int(max_groups_per_rank / world * slack) + (1 << 14)
+        self.rx = RegionExchange(lib, L, world, rank, [(self.width + 1, cap)])
+        self.last_phase = {}
+
+    def _create(self):
+        L = self.L
+        it = (C.c_int32 * len(self.types))(*self.types)
+        gb = (C.c_int32 * max(len(self.group_by), 1))(*self.group_by)
+        fa = (L.TQAggFunc * max(len(self.funcs), 1))(*[L.TQAggFunc(f, a) for f, a in self.funcs])
+        d = L.TQAggDesc(len(self.types), it, len(self.group_by), gb, len(self.funcs), fa, self.est_groups)
+        h = C.c_void_p()
+        L.check(self.lib.tq_agg_create(C.byref(d), C.byref(h)))
+        return h, (it, gb, fa)
+
+    def close(self):
+        self.rx.close()
+
+    def step(self, cols, bitmaps=None, keep_result=False):
+        """cols: this rank's shard of every input column ((device pointer, rows)-like objects); bitmaps: a device NULL bitmap
+        pointer (or None) per column.  Returns (groups finished on this rank, result): result (keep_result) = host Columns of
+        the function outputs, None otherwise."""
+        lib, L, rx, w = self.lib, self.L, self.rx, self.world
+        nw = self.width + 1
+        n = int(cols[0].numel()) if cols else 0
+        rx.next_epoch()
+        hp, keep_p = self._create()
+        hf, keep_f = self._create()
+        try:
+            if n:
+                arr = _tq_cols(L, cols, n)
+                for c, b in enumerate(bitmaps or []):
+                    arr[c].null_bitmap = b
+                L.check(lib.tq_agg_put(hp, arr, L.TQ_MEM_DEVICE))
+            L.check(lib.tq_agg_eof(hp))
+            dest = (C.c_void_p * (w * nw))()
+            cnts = (C.c_void_p * w)()
+            for d in range(w):
+                for c in range(nw):
+                    dest[d * nw + c] = rx.region_ptr(d, 0, self.rank, c)
+                cnts[d] = rx.slot_ptr(d, 0, self.rank)
+            L.check(lib.tq_agg_push_partial(hp, w, dest, cnts, rx.cap[0], self.slot, rx.epoch))
+            rx.wait(0)
+            regs = (L.TQColumn * (w * nw))()
+            for g in range(w):
+                for c in range(nw):
+                    regs[g * nw + c].data = rx.region_ptr(self.rank, 0, g, c)
+            L.check(lib.tq_agg_merge_regions(hf, w, C.c_void_p(rx.slot_ptr(self.rank, 0, 0)), rx.cap[0], regs))
+            L.check(lib.tq_agg_eof(hf))
+            L.check(lib.tq_partition_push_sync(self.slot))     # the push reads the Partial1 handle's rows until it is done
+            res, groups = None, 0
+            if keep_result and (self.group_by or self.rank == 0):
+                res = agg_drain(lib, L, hf, len(self.funcs))
+                groups = res[0].length if res else 0
+            elif self.group_by or self.rank == 0:
+                out = (L.TQColumn * max(len(self.funcs), 1))()
+                rows, eof = C.c_int64(0), C.c_int32(0)
+                L.check(lib.tq_agg_next_device(hf, out, C.byref(rows), C.byref(eof)))   # the groups stay in HBM
+                if rows.value or self.group_by:
+                    groups = rows.value
+                else:                                        # a scalar aggregate over no rows: the default row, unless all FIRSTROW
+                    groups = int(any(f != 5 for f, _ in self.funcs))
+        finally:
+            lib.tq_agg_destroy(hp)
+            lib.tq_agg_destroy(hf)
+        dist.barrier()
+        return groups, res
 
 
 def gen_dist_tables(rank, world, n_b, n_p):
