@@ -2,7 +2,8 @@
 SUM(x) and COUNT(*) (plus FIRSTROW(k), which names each result row's group), in two variants: NOT NULL, and nullable with 5 %
 NULL x and 1 % NULL keys.
 
-  emulated : W ranks on ONE GPU in this process (every rank's regions in this GPU's memory).  Per source: the partial
+  emulated : W ranks on ONE GPU in this process (every rank's regions in this GPU's memory: tests/exchange_ref.py's Regions,
+             with dist.RegionLayout's argument tables).  Per source: the partial
              aggregation (tq_agg_put + tq_agg_eof) and the push (tq_agg_push_partial: export, destination, scatter, publish);
              per destination: the merge (tq_region_wait + tq_agg_merge_regions) and the final (tq_agg_eof + tq_agg_next_device).
              Each phase is host time around calls that end in a device synchronise; bytes pushed from the published slots.
@@ -26,6 +27,7 @@ import numpy as np
 
 ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 sys.path.insert(0, ROOT)
+sys.path.insert(0, os.path.join(ROOT, "tests"))
 
 COUNT, SUM, FIRSTROW = 0, 1, 5
 FUNCS = [(SUM, 1), (COUNT, -1), (FIRSTROW, 0)]
@@ -61,6 +63,7 @@ def timed(lib, L, fn):
 
 def emulated(torch, lib, L, D, dev, args, nullable):
     """W ranks on this GPU: per-phase ms (mean over sources / destinations, best rep) and bytes pushed"""
+    import exchange_ref as X
     W = args.ranks
     t = L.TQ_TYPE_INT64 if nullable else L.TQ_TYPE_INT64 | L.TQ_TYPE_NOT_NULL
     it = (C.c_int32 * 2)(t, t)
@@ -78,10 +81,7 @@ def emulated(torch, lib, L, D, dev, args, nullable):
     lib.tq_agg_destroy(h)
     nw = wd.value + 1
     cap = int(args.keys / W * 1.25) + (1 << 14)
-    slots = torch.zeros(W * W * 2, dtype=torch.int64, device=dev)         # [dst][src] {rows, epoch}
-    regions = torch.empty(W * W * nw * cap, dtype=torch.int64, device=dev)
-    reg = lambda dst, src, c: regions.data_ptr() + (((dst * W + src) * nw + c) * cap) * 8
-    slot = lambda dst, src: slots.data_ptr() + (dst * W + src) * 16
+    reg = X.Regions(lib, W, nw, cap, guard=0)
     data = [shard(torch, dev, 1000 * (1 + nullable) + s, args.rows, args.keys, nullable) for s in range(W)]
     torch.cuda.synchronize()
     best, groups, pushed = None, 0, 0
@@ -97,24 +97,19 @@ def emulated(torch, lib, L, D, dev, args, nullable):
             h = create()
             hs.append(h)
             ph["partial_agg"].append(timed(lib, L, lambda: (L.check(lib.tq_agg_put(h, arr, L.TQ_MEM_DEVICE)), L.check(lib.tq_agg_eof(h)))))
-            dest = (C.c_void_p * (W * nw))(*[reg(q, s, c) for q in range(W) for c in range(nw)])
-            cnts = (C.c_void_p * W)(*[slot(q, s) for q in range(W)])
+            dest, cnts = reg.push_tables(0, s)
             ph["push"].append(timed(lib, L, lambda: (L.check(lib.tq_agg_push_partial(h, W, dest, cnts, cap, s, epoch)),
                                                       L.check(lib.tq_partition_push_sync(s)))))
         groups, pushed = 0, 0
         for q in range(W):
             hf = create()
-            regs = (L.TQColumn * (W * nw))()
-            for g in range(W):
-                for c in range(nw):
-                    regs[g * nw + c].data = reg(q, g, c)
-            ph["merge"].append(timed(lib, L, lambda: (L.check(lib.tq_region_wait(C.c_void_p(slot(q, 0)), W, epoch)),
-                                                       L.check(lib.tq_agg_merge_regions(hf, W, C.c_void_p(slot(q, 0)), cap, regs)))))
+            regs, slots = reg.region_table(q, 0), C.c_void_p(reg.slot_ptr(q, 0, 0))
+            ph["merge"].append(timed(lib, L, lambda: (L.check(reg.wait(q, epoch)), L.check(lib.tq_agg_merge_regions(hf, W, slots, cap, regs)))))
             out = (L.TQColumn * 3)()
             n, eof = C.c_int64(0), C.c_int32(0)
             ph["final"].append(timed(lib, L, lambda: (L.check(lib.tq_agg_eof(hf)), L.check(lib.tq_agg_next_device(hf, out, C.byref(n), C.byref(eof))))))
             groups += n.value
-            pushed += int(slots[q * W * 2: (q + 1) * W * 2: 2].sum()) * nw * 8
+            pushed += sum(rows for rows, _ in reg.slots(q)) * nw * 8
             lib.tq_agg_destroy(hf)
         for h in hs:
             lib.tq_agg_destroy(h)
@@ -123,7 +118,8 @@ def emulated(torch, lib, L, D, dev, args, nullable):
         mean = {k: float(np.mean(v)) for k, v in ph.items()}
         if best is None or sum(mean.values()) < sum(best.values()):
             best = mean
-    del regions, slots, data
+    reg.free()
+    del data
     torch.cuda.empty_cache()
     return {"ranks_emulated": W, "ms_per_rank": {k: round(v, 3) for k, v in best.items()}, "groups": groups,
             "bytes_pushed_per_rank": pushed // W, "wire_words_per_row": nw,
@@ -132,9 +128,7 @@ def emulated(torch, lib, L, D, dev, args, nullable):
 
 def group_runs(torch, lib, L, D, dist, dev, args, rank, world):
     """RegionAgg over the process group on both variants, the NCCL path on the NOT NULL one; results compared"""
-    import importlib
-    sys.path.insert(0, os.path.join(ROOT, "tests"))
-    RA = importlib.import_module("region_agg_ref")
+    import region_agg_ref as RA
     out = {}
     for nullable in (False, True):
         cols, bms = shard(torch, dev, 7000 * (1 + nullable) + rank, args.rows, args.keys, nullable)

@@ -5,7 +5,8 @@ matches once).  W sources push into one destination, which times, with CUDA even
            column so the mask word travels) -> tq_region_gather -> tq_join_put_probe of the gathered rows
   inner  : tq_partition_push_regions of NOT NULL columns -> tq_join_put_probe_segments over the regions in place
 on the same data and the same build table (every rank's build shard), and checks every output row of both (B.v = 7 B.k + 1,
-B.k = P.k = mix64(P.v) % N_build, as many rows as probe rows).  Prints one JSON line with the card name and power limit.
+B.k = P.k = mix64(P.v) % N_build, as many rows as probe rows).  The receive buffers and the kept miss rows are
+tests/exchange_ref.py's Regions, with dist.RegionLayout's argument tables.  Prints one JSON line with the card name and power limit.
 
     python scripts/region_outer_probe.py [--ranks 2] [--build-rows 12500000] [--probe-rows 125000000] [--reps 3]
 """
@@ -20,6 +21,7 @@ import numpy as np
 
 ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 sys.path.insert(0, ROOT)
+sys.path.insert(0, os.path.join(ROOT, "tests"))
 
 
 def card():
@@ -36,6 +38,7 @@ def main():
     args = ap.parse_args()
     import torch
 
+    import exchange_ref as X
     from tinysql_b200 import _lib as L
     from tinysql_b200 import dist as D
     lib = L.load()
@@ -55,14 +58,12 @@ def main():
     def alloc(nbytes):
         return torch.empty((nbytes + 7) // 8, dtype=torch.int64, device=dev)
 
-    # receive side of one destination at a time: W regions of 3 wire columns (k, v, mask) + slots; misses of one source
-    regions = alloc(W * 3 * cap * 8)
-    slots = torch.zeros(W * 2, dtype=torch.int64, device=dev)
-    miss = alloc(3 * 64 * 8)
-    miss_slot = torch.zeros(2, dtype=torch.int64, device=dev)
+    # the destination's regions: (k, v) for the inner join, (k, v, mask) for the masked one; the kept misses of the sources
+    regs = {False: X.Regions(lib, W, 2, cap, guard=0), True: X.Regions(lib, W, 3, cap, guard=0)}
+    miss = X.Regions(lib, 1, 3, 64, guard=0)
     g_cols = [alloc(W * cap * 8) for _ in range(2)]
     g_bm = [alloc(((W * cap + 63) // 64) * 8 + 8) for _ in range(2)]
-    reg_ptr = lambda g, c: ptr(regions) + ((g * 3 + c) * cap) * 8
+    epoch = [0]
 
     def build_handle(jt):
         bk = np.concatenate(shards_bk)
@@ -99,47 +100,36 @@ def main():
         jt = 1 if masked else 0
         h, keep = build_handle(jt)
         e = [ev() for _ in range(4)]
+        reg = regs[masked]
+        epoch[0] += 1
         try:
-            slots.zero_()
             torch.cuda.synchronize()
             lib.tq_device_synchronize()
             e[0].record()
             for s in range(W):
                 pk, pv = src[s][2], src[s][3]
                 cols = D._tq_cols(L, [pk, pv], npr)
-                nw = 3 if masked else 2
-                dest = (C.c_void_p * nw)(*[reg_ptr(s, c) for c in range(nw)])
-                cnts = (C.c_void_p * 1)(ptr(slots) + s * 16)
+                dest, cnts = reg.push_tables(0, s)                   # n_parts = 1: destination 0's entries
                 md, ms = None, None
                 if masked:
                     cols[1].null_bitmap = ptr(pv_nn)
-                    md, ms = (C.c_void_p * 3)(*[ptr(miss) + c * 64 * 8 for c in range(3)]), C.c_void_p(ptr(miss_slot))
-                L.check(lib.tq_partition_push_regions(2, cols, 0, npr, 1, None, int(masked), dest, cnts, cap, md, ms, 64 if masked else 0, s, 1))
+                    md, ms = miss.push_tables(0, 0)[0], miss.slot_ptr(0, 0, 0)
+                L.check(lib.tq_partition_push_regions(2, cols, 0, npr, 1, None, int(masked), dest, cnts, cap, md, ms, 64 if masked else 0, s, epoch[0]))
             for s in range(W):
                 L.check(lib.tq_partition_push_sync(s))
             e[1].record()
-            L.check(lib.tq_region_wait(C.c_void_p(ptr(slots)), W, 1))
+            L.check(reg.wait(0, epoch[0]))
             if masked:
-                regs = (L.TQColumn * (W * 3))()
-                for g in range(W):
-                    for c in range(3):
-                        regs[g * 3 + c].data = reg_ptr(g, c)
                 outc = (L.TQColumn * 2)()
                 for c in range(2):
                     outc[c].data, outc[c].null_bitmap = ptr(g_cols[c]), ptr(g_bm[c])
                 n = C.c_int64(0)
-                L.check(lib.tq_region_gather(W, C.c_void_p(ptr(slots)), cap, 2, 1, regs, outc, W * cap, C.byref(n)))
+                L.check(lib.tq_region_gather(W, C.c_void_p(reg.slot_ptr(0, 0, 0)), cap, 2, 1, reg.region_table(0, 0), outc, W * cap, C.byref(n)))
                 e[2].record()
                 L.check(lib.tq_join_put_probe(h, outc, None, L.TQ_MEM_DEVICE))
             else:
                 e[2].record()
-                cols = (L.TQColumn * (W * 2))()
-                cnts = (C.c_void_p * W)()
-                for g in range(W):
-                    for c in range(2):
-                        cols[g * 2 + c].length, cols[g * 2 + c].data = cap, reg_ptr(g, c)
-                    cnts[g] = ptr(slots) + g * 16
-                L.check(lib.tq_join_put_probe_segments(h, W, cols, cnts, cap))
+                L.check(lib.tq_join_put_probe_segments(h, W, reg.region_table(0, 0), reg.count_ptrs(0, 0), cap))
             L.check(lib.tq_join_probe_eof(h))
             rows, ok = drain(h, check)
             e[3].record()

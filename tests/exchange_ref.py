@@ -7,17 +7,15 @@ and part_offsets compare bit for bit.
 tq_partition_push_regions: a row whose key is NULL is neither counted nor sent; a destination receives a multiset of rows
 (runs of a destination are claimed with atomics: the order inside it is not promised).
 
-Regions: the exchange of dist.RegionExchange with all W ranks' receive buffers in this GPU's memory.  RegionExchange itself
-needs a process group and CUDA IPC (which cannot open a handle in the process that exported it), so its layout is restated
-here: per table one tq_device_alloc holding the W x W slots {u64 rows, u64 epoch} and the W x W x ncols regions of `cap`
-rows, each region followed by `guard` rows of a sentinel, so a row written past the cap lands inside the allocation and
-shows up in the guard instead of faulting."""
+Regions: dist.RegionLayout of one table with all W ranks' receive buffers in one tq_device_alloc of W x layout.bytes
+(rank d's at offset d x bytes), each region followed by `guard` rows of a sentinel (pad_rows), so a row written past the
+cap lands inside the allocation and shows up in the guard instead of faulting."""
 import ctypes as C
 
 import numpy as np
 
 from tinysql_b200 import _lib as L
-from tinysql_b200.dist import dest_rank_np
+from tinysql_b200.dist import RegionLayout, dest_rank_np
 
 SENTINEL_BYTE = 0xA7
 SENTINEL = np.uint64(0xA7A7A7A7A7A7A7A7)
@@ -123,70 +121,43 @@ def bitmap_words(nn):
     return np.concatenate([b, np.zeros(pad - len(b), np.uint8)])
 
 
-class Regions:
-    """W emulated ranks' receive buffers of one table: slots[dst][src] = {rows, epoch}, region(dst, src, col) = cap rows
-    followed by `guard` sentinel rows.  Slots start at zero (epoch 0: nothing published), regions and guards at the
-    sentinel."""
+class Regions(RegionLayout):
+    """W emulated ranks' receive buffers of one table (t = 0): slots start at zero (epoch 0: nothing published), regions and
+    guards at the sentinel."""
 
     def __init__(self, lib, world, ncols, cap, guard=64):
-        self.lib, self.world, self.ncols, self.cap, self.guard = lib, world, ncols, int(cap), guard
-        self.stride = self.cap + guard
-        self.slot_bytes = ((world * world * 16 + 4095) // 4096) * 4096
-        self.buf = Buf(lib, self.slot_bytes + world * world * ncols * self.stride * 8)
-        L.check(lib.tq_memset_device(self.buf.p, 0, self.slot_bytes))
+        super().__init__(lib, L, world, [(ncols, cap)], pad_rows=guard)
+        self.buf = Buf(lib, world * self.bytes)
+        self.bases = [self.buf.addr(d * self.bytes) for d in range(world)]
+        for d in range(world):
+            L.check(lib.tq_memset_device(C.c_void_p(self.slot_ptr(d, 0, 0)), 0, world * 16))
         compute_sync(lib)
 
-    # RegionExchange.region_ptr / slot_ptr with every rank's buffer in this allocation
-    def region_off(self, dst, src, c):
-        return self.slot_bytes + (((dst * self.world + src) * self.ncols + c) * self.stride) * 8
-
-    def region_ptr(self, dst, src, c):
-        return self.buf.addr(self.region_off(dst, src, c))
-
-    def slot_ptr(self, dst, src):
-        return self.buf.addr((dst * self.world + src) * 16)
-
-    def push(self, src, cols, n, slot, epoch, key_col=0, bitmaps=None, selected=None, miss=None, miss_slot=None, miss_cap=0):
+    def push(self, src, cols, n, slot, epoch, key_col=0, bitmaps=None, selected=None, miss=None):
         """source `src` scatters its n rows (device column pointers; bitmaps: a device NULL bitmap pointer or None per
-        column) into its region on every destination.  selected: device bytes or None.  miss (ncols wire column pointers),
-        miss_slot and miss_cap keep the rows that cannot match on the source (keep_misses); without miss they are dropped."""
-        w, nw = self.world, self.ncols
-        dest = (C.c_void_p * (w * nw))()
-        cnts = (C.c_void_p * w)()
-        for d in range(w):
-            for c in range(nw):
-                dest[d * nw + c] = self.region_ptr(d, src, c)
-            cnts[d] = self.slot_ptr(d, src)
+        column) into its region on every destination.  selected: device bytes or None.  miss: (Regions of one rank, miss
+        cap) that keeps the rows which cannot match on the source (keep_misses); without it they are dropped."""
+        dest, cnts = self.push_tables(0, src)
         tq = (L.TQColumn * len(cols))()
         for c in range(len(cols)):
             tq[c].length, tq[c].data = n, cols[c]
             tq[c].null_bitmap = bitmaps[c] if bitmaps else None
-        md = (C.c_void_p * nw)(*miss) if miss is not None else None
-        return self.lib.tq_partition_push_regions(len(cols), tq, key_col, n, w, selected, int(miss is not None), dest, cnts, self.cap, md,
-                                                  miss_slot, miss_cap, slot, epoch)
+        md, ms, mcap = (None, None, 0) if miss is None else (miss[0].push_tables(0, 0)[0], miss[0].slot_ptr(0, 0, 0), miss[1])
+        return self.lib.tq_partition_push_regions(len(cols), tq, key_col, n, self.world, selected, int(miss is not None), dest, cnts, self.cap[0],
+                                                  md, ms, mcap, slot, epoch)
 
     def wait(self, dst, epoch):
-        return self.lib.tq_region_wait(C.c_void_p(self.slot_ptr(dst, 0)), self.world, epoch)
+        return self.lib.tq_region_wait(C.c_void_p(self.slot_ptr(dst, 0, 0)), self.world, epoch)
 
     def slots(self, dst):
         """[(rows, epoch)] of every source on `dst` (host read)"""
-        raw = self.buf.get(np.uint64, (dst * self.world) * 16, self.world * 16)
-        return [(int(raw[2 * s]), int(raw[2 * s + 1])) for s in range(self.world)]
+        return [(int(r), int(e)) for r, e in self.read_slots(dst)[0]]
 
     def region(self, dst, src, c):
         """the region's cap rows followed by its guard rows"""
-        return self.buf.get(np.uint64, self.region_off(dst, src, c), self.stride * 8)
-
-    def segment_args(self, dst):
-        """(tq_column array [src][col], count pointer array) of dst's regions, as tq_join_put_probe_segments takes them"""
-        w, nc = self.world, self.ncols
-        cols = (L.TQColumn * (w * nc))()
-        cnts = (C.c_void_p * w)()
-        for g in range(w):
-            for c in range(nc):
-                cols[g * nc + c].length, cols[g * nc + c].data = self.cap, self.region_ptr(dst, g, c)
-            cnts[g] = self.slot_ptr(dst, g)
-        return cols, cnts
+        out = np.empty(self.cap[0] + self.pad_rows, np.uint64)
+        L.check(self.lib.tq_memcpy_d2h(out.ctypes.data, C.c_void_p(self.region_ptr(dst, 0, src, c)), out.nbytes))
+        return out
 
     def free(self):
         self.buf.free()

@@ -1,5 +1,5 @@
 """Reference of the GROUP BY over the region exchange (tq_agg_push_partial / tq_agg_merge_regions), and the runner that drives
-it with every rank emulated in one process on exchange_ref's Regions layout.
+it with every rank emulated in one process on exchange_ref's Regions, whose argument tables are dist.RegionLayout's.
 
 group_dest is the Python twin of the destination rule (include/tinysql_b200.h, csrc/scatter.cuh): h = 0, then per GROUP BY
 item h = mix64(h ^ v), v = the item's 8 bytes (REAL: -0.0 read as +0.0) or GROUP_NULL_WORD for NULL; rank = (h >> 40) % W."""
@@ -57,27 +57,6 @@ def width(lib, d):
         lib.tq_agg_destroy(h)
 
 
-def push_args(reg, src):
-    """(dest_data, dest_counts) of source src on every destination of reg"""
-    w, nw = reg.world, reg.ncols
-    dest = (C.c_void_p * (w * nw))()
-    cnts = (C.c_void_p * w)()
-    for d in range(w):
-        for c in range(nw):
-            dest[d * nw + c] = reg.region_ptr(d, src, c)
-        cnts[d] = reg.slot_ptr(d, src)
-    return dest, cnts
-
-
-def merge_args(reg, dst):
-    w, nw = reg.world, reg.ncols
-    regs = (L.TQColumn * (w * nw))()
-    for g in range(w):
-        for c in range(nw):
-            regs[g * nw + c].data = reg.region_ptr(dst, g, c)
-    return regs
-
-
 def partial_handle(lib, d, src):
     """a Partial1 handle fed one shard (an R.Source in device memory), eof'd"""
     h = create(lib, d)
@@ -99,14 +78,14 @@ def run(lib, W, types, group_by, funcs, shards, reg, epoch=1, not_null=()):
     try:
         for s in range(W):
             hs.append(partial_handle(lib, d, shards[s]))
-            dest, cnts = push_args(reg, s)
-            L.check(lib.tq_agg_push_partial(hs[-1], W, dest, cnts, reg.cap, s, epoch))
+            dest, cnts = reg.push_tables(0, s)
+            L.check(lib.tq_agg_push_partial(hs[-1], W, dest, cnts, reg.cap[0], s, epoch))
         out = []
         for q in range(W):
             L.check(reg.wait(q, epoch))                      # queued after every push that satisfies it
             hf = create(lib, d)
             try:
-                st = lib.tq_agg_merge_regions(hf, W, C.c_void_p(reg.slot_ptr(q, 0)), reg.cap, merge_args(reg, q))
+                st = lib.tq_agg_merge_regions(hf, W, C.c_void_p(reg.slot_ptr(q, 0, 0)), reg.cap[0], reg.region_table(q, 0))
                 if st != L.TQ_OK:
                     out.append((st, None))
                     continue

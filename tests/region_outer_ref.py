@@ -1,6 +1,7 @@
 """Outer joins and nullable columns over the region exchange with W ranks emulated in one process (tests/exchange_ref.py's
-Regions layout): each source pushes its shards with tq_partition_push_regions, each destination copies its regions
-with tq_region_gather and joins them with an ordinary join handle, as dist.RegionJoin does across processes.
+Regions, on dist.RegionLayout): each source pushes its shards with tq_partition_push_regions, each destination copies its
+regions with tq_region_gather and joins them with an ordinary join handle, as dist.RegionJoin does across processes; the
+probe rows that cannot match stay on their source in a Regions of one rank, as RegionJoin keeps them.
 
 A shard is (cols, nns): uint64 arrays and NOT-NULL bool arrays (None = no bitmap), key = column 0.  Every output buffer a
 wrong count could reach is a sentinel-filled part of a larger allocation (GUARD rows before and after)."""
@@ -103,19 +104,15 @@ class Source:
             b.free()
 
 
-def push(reg, src_idx, source, slot, epoch, miss=None, miss_slot=None, miss_cap=0):
-    """source src_idx pushes its rows into its region on every destination of `reg` (wire columns = reg.ncols)"""
-    return reg.push(src_idx, source.ptrs, source.n, slot, epoch, bitmaps=source.bms, selected=source.sel, miss=miss, miss_slot=miss_slot,
-                    miss_cap=miss_cap)
+def push(reg, src_idx, source, slot, epoch, miss=None):
+    """source src_idx pushes its rows into its region on every destination of `reg` (wire columns = reg.ncols[0]); miss:
+    (Regions of one rank, miss cap) keeps the rows that cannot match"""
+    return reg.push(src_idx, source.ptrs, source.n, slot, epoch, bitmaps=source.bms, selected=source.sel, miss=miss)
 
 
-def gather(lib, n_regions, slots_ptr, cap, ncols, has_mask, region_ptr, out, out_cap=None):
-    """tq_region_gather of regions region_ptr(g, c) into GuardedCols `out`: (status, rows)"""
-    nw = ncols + has_mask
-    regs = (L.TQColumn * (n_regions * nw))()
-    for g in range(n_regions):
-        for c in range(nw):
-            regs[g * nw + c].data = region_ptr(g, c)
+def gather(lib, n_regions, slots_ptr, cap, ncols, has_mask, regs, out, out_cap=None):
+    """tq_region_gather of the tq_column table regs ([region][wire column], RegionLayout.region_table) into GuardedCols
+    `out`: (status, rows)"""
     n = C.c_int64(-1)
     st = lib.tq_region_gather(n_regions, C.c_void_p(slots_ptr), cap, ncols, has_mask, regs, out.arr, out.rows if out_cap is None else out_cap, C.byref(n))
     return st, n.value
@@ -188,13 +185,11 @@ def run(lib, W, jt, oir, btypes, ptypes, bshards, pshards, psel=None, default_in
     try:
         srcs = [Source(lib, cols, nns) for cols, nns in bshards] + [Source(lib, cols, nns, psel[s]) for s, (cols, nns) in enumerate(pshards)]
         keep += srcs
-        miss = [X.Buf(lib, (max(mcap, 1) + GUARD) * 8 * nwp) for _ in range(W)] if outer else []
-        mslot = [X.Buf(lib, 16, 0) for _ in range(W)] if outer else []
-        keep += miss + mslot
+        miss = [X.Regions(lib, 1, nwp, max(mcap, 1), GUARD) for _ in range(W)] if outer else []
+        keep += miss
         for s in range(W):
             L.check(push(breg, s, srcs[s], s, epoch))
-            mp = [miss[s].addr(c * (max(mcap, 1) + GUARD) * 8) for c in range(nwp)] if outer else None
-            L.check(push(preg, s, srcs[W + s], 8 + s, epoch, mp, mslot[s].addr() if outer else None, mcap))
+            L.check(push(preg, s, srcs[W + s], 8 + s, epoch, (miss[s], mcap) if outer else None))
         for slot in list(range(W)) + list(range(8, 8 + W)):
             L.check(lib.tq_partition_push_sync(slot))
         for d in range(W):
@@ -204,13 +199,12 @@ def run(lib, W, jt, oir, btypes, ptypes, bshards, pshards, psel=None, default_in
             gp = GuardedCols(lib, npc, W * pcap, pmask)
             gm = GuardedCols(lib, npc, max(mcap, 1), pmask)
             keep += [gb, gp, gm]
-            st_b, rb = gather(lib, W, breg.slot_ptr(d, 0), bcap, nb, bmask, lambda g, c: breg.region_ptr(d, g, c), gb)
-            st_p, rp = gather(lib, W, preg.slot_ptr(d, 0), pcap, npc, pmask, lambda g, c: preg.region_ptr(d, g, c), gp)
+            st_b, rb = gather(lib, W, breg.slot_ptr(d, 0, 0), bcap, nb, bmask, breg.region_table(d, 0), gb)
+            st_p, rp = gather(lib, W, preg.slot_ptr(d, 0, 0), pcap, npc, pmask, preg.region_table(d, 0), gp)
             st_m, rm = L.TQ_OK, 0
             if outer:
-                L.check(lib.tq_region_wait(C.c_void_p(mslot[d].addr()), 1, epoch))
-                st_m, rm = gather(lib, 1, mslot[d].addr(), max(mcap, 1), npc, pmask,
-                                  lambda g, c: miss[d].addr(c * (max(mcap, 1) + GUARD) * 8), gm)
+                L.check(miss[d].wait(0, epoch))
+                st_m, rm = gather(lib, 1, miss[d].slot_ptr(0, 0, 0), max(mcap, 1), npc, pmask, miss[d].region_table(0, 0), gm)
             bad = [s for s in (st_b, st_p, st_m) if s != L.TQ_OK]
             if bad:
                 for g, st, r in ((gb, st_b, rb), (gp, st_p, rp), (gm, st_m, rm)):

@@ -63,14 +63,15 @@ def _regions(lib, rng, counts, ncols, has_mask, cap):
     """one destination's W regions filled as the push leaves them: rows (+ mask words) and published slots"""
     W = len(counts)
     reg = X.Regions(lib, W, ncols + has_mask, cap)
+    put = lambda a, g, c: reg.buf.put(a, reg.region_ptr(0, 0, g, c) - reg.buf.addr())
     rows, nns = [], []
     for g, m in enumerate(counts):
         v = [rng.integers(0, 1 << 62, m).astype(np.uint64) for _ in range(ncols)]
         nn = [rng.random(m) >= 0.4 for _ in range(ncols)]
         for c in range(ncols):
-            reg.buf.put(v[c], reg.region_off(0, g, c))
+            put(v[c], g, c)
         if has_mask and m:
-            reg.buf.put(sum(nn[c].astype(np.uint64) << np.uint64(c) for c in range(ncols)), reg.region_off(0, g, ncols))
+            put(sum(nn[c].astype(np.uint64) << np.uint64(c) for c in range(ncols)), g, ncols)
         rows.append(v)
         nns.append(nn if has_mask else [np.ones(m, bool)] * ncols)
     return reg, rows, nns
@@ -78,7 +79,7 @@ def _regions(lib, rng, counts, ncols, has_mask, cap):
 
 def _publish(reg, counts, epoch=1):
     slots = np.array([[c, epoch] for c in counts], np.uint64).reshape(-1)
-    reg.buf.put(slots, 0)
+    reg.buf.put(slots, reg.slot_ptr(0, 0, 0) - reg.buf.addr())
 
 
 @pytest.mark.parametrize("has_mask", [0, 1])
@@ -96,7 +97,7 @@ def test_emu_region_gather_counts(emu, W, has_mask):
         _publish(reg, counts)
         out = R.GuardedCols(emu, ncols, 65 * W, True)
         try:
-            st, n = R.gather(emu, W, reg.slot_ptr(0, 0), 65, ncols, has_mask, lambda g, c: reg.region_ptr(0, g, c), out)
+            st, n = R.gather(emu, W, reg.slot_ptr(0, 0, 0), 65, ncols, has_mask, reg.region_table(0, 0), out)
             assert st == L.TQ_OK and n == sum(counts), (counts, st, n)
             assert all(out.arr[c].length == n for c in range(ncols))
             assert out.guards_ok(n), f"{counts}: a write past the rows / bitmap words"
@@ -116,14 +117,14 @@ def test_emu_region_gather_without_bitmaps_and_empty(emu):
     _publish(reg, [5, 0, 70])
     out = R.GuardedCols(emu, 2, 200, False)
     try:
-        st, n = R.gather(emu, 3, reg.slot_ptr(0, 0), 70, 2, 1, lambda g, c: reg.region_ptr(0, g, c), out)
+        st, n = R.gather(emu, 3, reg.slot_ptr(0, 0, 0), 70, 2, 1, reg.region_table(0, 0), out)
         assert st == L.TQ_OK and n == 75
         assert out.guards_ok(75)
         for c, (v, nn) in enumerate(out.read(75)):
             assert nn is None and np.array_equal(v, np.concatenate([r[c] for r in rows]))
         _publish(reg, [0, 0, 0])
         out2 = R.GuardedCols(emu, 2, 64, True)
-        st, n = R.gather(emu, 3, reg.slot_ptr(0, 0), 70, 2, 1, lambda g, c: reg.region_ptr(0, g, c), out2)
+        st, n = R.gather(emu, 3, reg.slot_ptr(0, 0, 0), 70, 2, 1, reg.region_table(0, 0), out2)
         assert st == L.TQ_OK and n == 0 and out2.untouched()
         out2.free()
     finally:
@@ -142,11 +143,11 @@ def test_emu_region_gather_refusals(emu, bad):
     _publish(reg, published)
     out = R.GuardedCols(emu, 2, 200, True)
     try:
-        st, n = R.gather(emu, 3, reg.slot_ptr(0, 0), 65, 2, 1, lambda g, c: reg.region_ptr(0, g, c), out, out_cap=129 if bad == "out_cap" else None)
+        st, n = R.gather(emu, 3, reg.slot_ptr(0, 0, 0), 65, 2, 1, reg.region_table(0, 0), out, out_cap=129 if bad == "out_cap" else None)
         assert st == (L.TQ_ERR_INVALID_ARG if bad == "out_cap" else L.TQ_ERR_OOM), st
         assert n == -1 and out.untouched(), "a refused gather wrote"
         for args in ((0, 65, 2, 1), (9, 65, 2, 1), (3, 0, 2, 1), (3, 65, 4, 1), (3, 65, 0, 0), (3, 65, 2, 2)):
-            st, _ = R.gather(emu, args[0], reg.slot_ptr(0, 0), args[1], args[2], args[3], lambda g, c: reg.region_ptr(0, g % 3, c % 3), out)
+            st, _ = R.gather(emu, args[0], reg.slot_ptr(0, 0, 0), args[1], args[2], args[3], reg.region_table(0, 0), out)
             assert st == L.TQ_ERR_INVALID_ARG, args
         assert out.untouched()
     finally:

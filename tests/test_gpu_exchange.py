@@ -232,7 +232,7 @@ def _check_source(reg, s, cols, dest, epoch):
     for d in range(reg.world):
         idx = np.flatnonzero(dest == d)
         assert reg.slots(d)[s] == (len(idx), epoch), f"slot ({d}, {s})"
-        got = np.stack([reg.region(d, s, c) for c in range(reg.ncols)], axis=1)
+        got = np.stack([reg.region(d, s, c) for c in range(reg.ncols[0])], axis=1)
         assert np.all(got[len(idx):] == X.SENTINEL), f"region ({d}, {s}): a row past its count"
         assert np.array_equal(X.sorted_rows(got[:len(idx)]), X.rows_of(cols, idx)), f"region ({d}, {s}) rows"
 
@@ -327,19 +327,19 @@ def test_push_regions_refusals(lib):
     n, W, ncols = 5_000, 3, 2
     keep = []
     reg = X.Regions(lib, W, ncols, n)
-    miss = X.Buf(lib, ncols * (n + GUARD) * 8)
-    mslot = X.Buf(lib, 16, 0)
+    miss = X.Regions(lib, 1, ncols, n, GUARD)
     try:
         cols = _push_data(rng, n, ncols, 0, 0)
         tq = _tq(_dev_cols(lib, cols, keep), n)
-        args = dict(n_cols=ncols, cols=tq, key_col=0, n=n, n_parts=W, selected=None, keep_misses=1,
-                    dest_data=(C.c_void_p * (W * ncols))(*[reg.region_ptr(d, 0, c) for d in range(W) for c in range(ncols)]),
-                    dest_counts=(C.c_void_p * W)(*[reg.slot_ptr(d, 0) for d in range(W)]), region_cap=reg.cap,
-                    miss_data=(C.c_void_p * ncols)(*[miss.addr(c * (n + GUARD) * 8) for c in range(ncols)]), miss_count=mslot.addr(),
-                    miss_cap=n, slot=0, epoch=1)
+        dest, cnts = reg.push_tables(0, 0)
+        args = dict(n_cols=ncols, cols=tq, key_col=0, n=n, n_parts=W, selected=None, keep_misses=1, dest_data=dest, dest_counts=cnts,
+                    region_cap=reg.cap[0], miss_data=miss.push_tables(0, 0)[0], miss_count=miss.slot_ptr(0, 0, 0), miss_cap=n, slot=0, epoch=1)
         push = lambda **bad: lib.tq_partition_push_regions(*{**args, **bad}.values())
+        holes = [(C.c_void_p * len(a))(*a) for a in (dest, cnts)]      # the last destination without its last region / its count slot
+        holes[0][len(dest) - 1] = holes[1][W - 1] = None
         for bad in (dict(n_parts=0), dict(n_parts=9), dict(n_parts=-1), dict(n=-1), dict(n=1 << 32), dict(key_col=-1),
                     dict(key_col=ncols), dict(n_cols=0), dict(cols=None), dict(dest_data=None), dict(dest_counts=None),
+                    dict(dest_data=holes[0]), dict(dest_counts=holes[1]),
                     dict(slot=-1), dict(slot=16), dict(region_cap=0), dict(region_cap=1 << 32), dict(miss_data=None),
                     dict(miss_count=None), dict(miss_cap=-1), dict(miss_cap=1 << 32)):
             assert push(**bad) == L.TQ_ERR_INVALID_ARG, bad
@@ -347,15 +347,14 @@ def test_push_regions_refusals(lib):
         for d in range(W):
             assert reg.slots(d) == [(0, 0)] * W, "a refused push published a slot"
             assert all(np.all(reg.region(d, 0, c) == X.SENTINEL) for c in range(ncols)), "a refused push wrote rows"
-        assert np.all(mslot.get() == 0), "a refused push published its miss slot"
+        assert miss.slots(0) == [(0, 0)], "a refused push published its miss slot"
         L.check(push())
         L.check(lib.tq_partition_push_sync(0))
         _check_source(reg, 0, cols, X.push_dest(cols[0], None, W), 1)
-        assert list(mslot.get()) == [0, 1], "no row misses: the miss slot reads {0, epoch}"
-        assert np.all(miss.get() == X.SENTINEL), "a miss column was written"
+        assert miss.slots(0) == [(0, 1)], "no row misses: the miss slot reads {0, epoch}"
+        assert all(np.all(miss.region(0, 0, c) == X.SENTINEL) for c in range(ncols)), "a miss column was written"
     finally:
-        reg.free()
-        for b in keep + [miss, mslot]:
+        for b in keep + [reg, miss]:
             b.free()
 
 
@@ -376,8 +375,8 @@ def _check_regions(reg, shards, epoch, overflowed=()):
             continue
         for d in range(w):
             assert reg.slots(d)[s] == ((1 << 64) - 1, epoch), f"source {s} overflowed: destination {d} must read ~0"
-            got = np.stack([reg.region(d, s, c) for c in range(reg.ncols)], axis=1)
-            assert np.all(got[reg.cap:] == X.SENTINEL), f"region ({d}, {s}): a row past its cap"
+            got = np.stack([reg.region(d, s, c) for c in range(reg.ncols[0])], axis=1)
+            assert np.all(got[reg.cap[0]:] == X.SENTINEL), f"region ({d}, {s}): a row past its cap"
 
 
 def _push_all(lib, reg, shards, epoch, keep, slot0=0, wait=True):
@@ -458,8 +457,7 @@ def _join_step(lib, reg, joins, shards, epoch, keep):
         L.check(reg.push(s, _dev_cols(lib, cols, keep), len(cols[0]), s, epoch))
     for d in range(w):
         L.check(reg.wait(d, epoch))
-        cols, cnts = reg.segment_args(d)
-        L.check(lib.tq_join_put_probe_segments(joins[d].h, w, cols, cnts, reg.cap))
+        L.check(lib.tq_join_put_probe_segments(joins[d].h, w, reg.region_table(d, 0), reg.count_ptrs(d, 0), reg.cap[0]))
     for s in range(len(shards)):
         L.check(lib.tq_partition_push_sync(s))
     for j in joins:
@@ -533,16 +531,15 @@ def test_segmented_join_segment_limit(lib, _stream_partitions):
     j = T._Join(lib, bcols, 2)
     try:
         sh = [[T._probe_keys(rng, bk, 5_000, 0.1), np.arange(5_000 * s, 5_000 * (s + 1), dtype=np.int64)] for s in range(8)]
-        for s, cols in enumerate(sh):       # 8 sources into destination 0's regions of a 9-rank table, one destination each
+        for s, cols in enumerate(sh):       # 8 sources into destination 0's regions of a 9-rank table (n_parts = 1: its entries come first)
             ptrs = _dev_cols(lib, cols, keep)
-            dest = (C.c_void_p * 2)(reg.region_ptr(0, s, 0), reg.region_ptr(0, s, 1))
-            cnts = (C.c_void_p * 1)(reg.slot_ptr(0, s))
-            L.check(lib.tq_partition_push_regions(2, _tq(ptrs, 5_000), 0, 5_000, 1, None, 0, dest, cnts, reg.cap, None, None, 0, s, 1))
+            dest, cnts = reg.push_tables(0, s)
+            L.check(lib.tq_partition_push_regions(2, _tq(ptrs, 5_000), 0, 5_000, 1, None, 0, dest, cnts, reg.cap[0], None, None, 0, s, 1))
         for s in range(8):
             L.check(lib.tq_partition_push_sync(s))
-        cols, cnts = reg.segment_args(0)
-        assert lib.tq_join_put_probe_segments(j.h, 9, cols, cnts, reg.cap) == L.TQ_ERR_INVALID_ARG
-        L.check(lib.tq_join_put_probe_segments(j.h, 8, cols, cnts, reg.cap))
+        cols, cnts = reg.region_table(0, 0), reg.count_ptrs(0, 0)
+        assert lib.tq_join_put_probe_segments(j.h, 9, cols, cnts, reg.cap[0]) == L.TQ_ERR_INVALID_ARG
+        L.check(lib.tq_join_put_probe_segments(j.h, 8, cols, cnts, reg.cap[0]))
         got, _ = j.finish()
         assert_same_multiset(got, T._want(bcols, [np.concatenate([c[i] for c in sh]) for i in range(2)]))
     finally:

@@ -266,7 +266,7 @@ def test_region_agg_refusals_write_nothing(lib):
     try:
         h = RA.partial_handle(lib, d, src)
         handles.append(h)
-        dest, cnts = RA.push_args(reg, 0)
+        dest, cnts = reg.push_tables(0, 0)
         bad = [(0, dest, cnts, 64, 0), (9, dest, cnts, 64, 0), (W, None, cnts, 64, 0), (W, dest, None, 64, 0), (W, dest, cnts, 0, 0),
                (W, dest, cnts, 1 << 32, 0), (W, dest, cnts, 64, -1), (W, dest, cnts, 64, 16)]
         for n_parts, dd, cc, cap, slot in bad:
@@ -279,7 +279,7 @@ def test_region_agg_refusals_write_nothing(lib):
         hv = RA.create(lib, dv)
         handles.append(hv)
         assert lib.tq_agg_push_partial(hv, W, dest, cnts, 64, 0, 1) == L.TQ_ERR_UNSUPPORTED_TYPE
-        assert lib.tq_agg_merge_regions(hv, W, C.c_void_p(reg.slot_ptr(0, 0)), 64, RA.merge_args(reg, 0)) == L.TQ_ERR_UNSUPPORTED_TYPE
+        assert lib.tq_agg_merge_regions(hv, W, C.c_void_p(reg.slot_ptr(0, 0, 0)), 64, reg.region_table(0, 0)) == L.TQ_ERR_UNSUPPORTED_TYPE
         # FinalMode handle
         it = (C.c_int32 * 2)(I64, I64)
         gb = (C.c_int32 * 1)(0)
@@ -289,21 +289,21 @@ def test_region_agg_refusals_write_nothing(lib):
         L.check(lib.tq_agg_create_final(C.byref(fd), C.byref(hf)))
         handles.append(hf)
         assert lib.tq_agg_push_partial(hf, W, dest, cnts, 64, 0, 1) == L.TQ_ERR_STATE
-        assert lib.tq_agg_merge_regions(hf, W, C.c_void_p(reg.slot_ptr(0, 0)), 64, RA.merge_args(reg, 0)) == L.TQ_ERR_STATE
+        assert lib.tq_agg_merge_regions(hf, W, C.c_void_p(reg.slot_ptr(0, 0, 0)), 64, reg.region_table(0, 0)) == L.TQ_ERR_STATE
         # raw rows and partial rows on one handle
-        assert lib.tq_agg_merge_regions(h, W, C.c_void_p(reg.slot_ptr(0, 0)), 64, RA.merge_args(reg, 0)) == L.TQ_ERR_STATE
+        assert lib.tq_agg_merge_regions(h, W, C.c_void_p(reg.slot_ptr(0, 0, 0)), 64, reg.region_table(0, 0)) == L.TQ_ERR_STATE
         hm = RA.create(lib, d)
         handles.append(hm)
-        regs = RA.merge_args(reg, 0)
-        for n_regions, slots, cap in ((0, reg.slot_ptr(0, 0), 64), (9, reg.slot_ptr(0, 0), 64), (W, None, 64), (W, reg.slot_ptr(0, 0), 0)):
+        regs = reg.region_table(0, 0)
+        for n_regions, slots, cap in ((0, reg.slot_ptr(0, 0, 0), 64), (9, reg.slot_ptr(0, 0, 0), 64), (W, None, 64), (W, reg.slot_ptr(0, 0, 0), 0)):
             assert lib.tq_agg_merge_regions(hm, n_regions, C.c_void_p(slots) if slots else None, cap, regs) == L.TQ_ERR_INVALID_ARG
         regs[1].data = None
-        assert lib.tq_agg_merge_regions(hm, W, C.c_void_p(reg.slot_ptr(0, 0)), 64, regs) == L.TQ_ERR_INVALID_ARG
+        assert lib.tq_agg_merge_regions(hm, W, C.c_void_p(reg.slot_ptr(0, 0, 0)), 64, regs) == L.TQ_ERR_INVALID_ARG
         X.compute_sync(lib)
         assert untouched(), "a refused call wrote a region or a slot"
         # a handle that merged partial rows cannot push
-        regs = RA.merge_args(reg, 0)
-        assert lib.tq_agg_merge_regions(hm, W, C.c_void_p(reg.slot_ptr(0, 0)), 64, regs) == L.TQ_OK   # all slots read 0 rows
+        regs = reg.region_table(0, 0)
+        assert lib.tq_agg_merge_regions(hm, W, C.c_void_p(reg.slot_ptr(0, 0, 0)), 64, regs) == L.TQ_OK   # all slots read 0 rows
         assert lib.tq_agg_push_partial(hm, W, dest, cnts, 64, 0, 1) == L.TQ_ERR_STATE
         X.compute_sync(lib)
         assert untouched()

@@ -190,7 +190,7 @@ def test_push_word_limit_refused_before_any_push(lib):
             else:
                 assert st == L.TQ_ERR_UNSUPPORTED_TYPE, (ncols, bm_col, st)
                 assert all(reg.slots(d)[0] == (0, 0) for d in range(W)), "a refused push published a slot"
-                assert all(np.all(reg.region(d, 0, c) == X.SENTINEL) for d in range(W) for c in range(reg.ncols)), "a refused push wrote rows"
+                assert all(np.all(reg.region(d, 0, c) == X.SENTINEL) for d in range(W) for c in range(reg.ncols[0])), "a refused push wrote rows"
     finally:
         for b in keep:
             b.free()

@@ -1523,15 +1523,7 @@ int32_t tq_agg_push_partial(tq_agg *a, int32_t n_parts, void *const *dest_data, 
   if (agg_has_varlen(a)) { set_error("partial export / merge with var-len columns is not supported"); return TQ_ERR_UNSUPPORTED_TYPE; }
   const int w = partial_width(a), nw = w + 1;
   if (nw > 64) { set_error("%s: %d partial columns and the mask word exceed 64 words per row", fn, w); return TQ_ERR_INVALID_ARG; }
-  if (!dest_data || !dest_counts || n_parts < 1 || n_parts > 8 || slot < 0 || slot >= PUSH_SLOTS || region_cap < 1 || region_cap > 0xFFFFFFF0ll) {
-    set_error("%s: 1..8 destinations with their regions and count slots, slot 0..%d, 1 <= region_cap < 2^32", fn, PUSH_SLOTS - 1);
-    return TQ_ERR_INVALID_ARG;
-  }
-  for (int q = 0; q < n_parts; q++) {
-    if (!dest_counts[q]) { set_error("%s: destination %d has no count slot", fn, q); return TQ_ERR_INVALID_ARG; }
-    for (int c = 0; c < nw; c++)
-      if (!dest_data[q * nw + c]) { set_error("%s: destination %d has no region for wire column %d", fn, q, c); return TQ_ERR_INVALID_ARG; }
-  }
+  TQ_TRY(push_check_dests(fn, n_parts, nw, dest_data, dest_counts, region_cap, slot));
   Runtime &r = rt();
   std::lock_guard<std::recursive_mutex> lk(r.mu);
   if (!a->eof) TQ_TRY(tq_agg_eof(a));
@@ -1540,12 +1532,8 @@ int32_t tq_agg_push_partial(tq_agg *a, int32_t n_parts, void *const *dest_data, 
   if (n > 0xFFFFFFF0ll) { set_error("%s: %lld partial rows", fn, (long long)n); return TQ_ERR_INVALID_ARG; }
   cudaStream_t s = r.h2d;   // the push stream, as tq_partition_push_regions
   PushSlot *ps = nullptr;
-  TQ_TRY(push_slot_acquire(slot, &ps));
-  for (int q = 0; q < n_parts; q++) ps->h_ptrs.as<void *>()[q] = dest_counts[q];
-  if (n == 0) {
-    TQ_CUDA(cudaMemsetAsync(ps->cursor.p, 0, 64, s));
-    TQ_CUDA(cudaMemsetAsync(ps->ovf.p, 0, 8, s));
-  } else {
+  TQ_TRY(push_begin(slot, n_parts, dest_counts, nullptr, s, &ps));
+  if (n > 0) {
     const size_t tab = (size_t)n_parts * nw * 8;
     TQ_TRY(ps->out_ptrs.reserve(tab));
     TQ_TRY(ps->h_out_ptrs.reserve(tab));

@@ -3679,13 +3679,8 @@ int32_t tq_partition_push_regions(int32_t n_cols, const tq_column *cols, int32_t
                                   uint64_t epoch) {
   TQ_TRY(ensure_init());
   const char *fn = "tq_partition_push_regions";
-  if (!cols || !dest_data || !dest_counts || n_cols < 1 || key_col < 0 || key_col >= n_cols) {
-    set_error("%s: needs columns, destinations, count slots and 0 <= key_col < n_cols", fn);
-    return TQ_ERR_INVALID_ARG;
-  }
-  if (n_parts < 1 || n_parts > 8 || n < 0 || n > 0xFFFFFFF0ll) { set_error("%s: 1..8 destinations and < 2^32 rows", fn); return TQ_ERR_INVALID_ARG; }
-  if (slot < 0 || slot >= PUSH_SLOTS || region_cap < 1 || region_cap > 0xFFFFFFF0ll) {
-    set_error("%s: slot 0..%d and 1 <= region_cap < 2^32", fn, PUSH_SLOTS - 1);
+  if (!cols || n_cols < 1 || key_col < 0 || key_col >= n_cols || n < 0 || n > 0xFFFFFFF0ll) {
+    set_error("%s: needs columns, 0 <= key_col < n_cols and < 2^32 rows", fn);
     return TQ_ERR_INVALID_ARG;
   }
   if (keep_misses && (!miss_data || !miss_count || miss_cap < 0 || miss_cap > 0xFFFFFFF0ll)) {
@@ -3697,6 +3692,7 @@ int32_t tq_partition_push_regions(int32_t n_cols, const tq_column *cols, int32_t
   for (int c = 0; c < n_cols; c++) pack = pack || cols[c].null_bitmap;
   const int n_wire = n_cols + (pack ? 1 : 0);
   if (n_wire > 4) { set_error("%s: %d columns%s: the push moves at most 4 words per row", fn, n_cols, pack ? " and the NULL mask word" : ""); return TQ_ERR_UNSUPPORTED_TYPE; }
+  TQ_TRY(push_check_dests(fn, n_parts, n_wire, dest_data, dest_counts, region_cap, slot));
   ScatterParams sp{};
   sp.n_cols = n_wire;
   sp.key_col = key_col;
@@ -3718,17 +3714,12 @@ int32_t tq_partition_push_regions(int32_t n_cols, const tq_column *cols, int32_t
   std::lock_guard<std::recursive_mutex> lk(r.mu);
   cudaStream_t s = r.h2d;  // the push stream: rows cross NVLink while the compute stream joins what has already arrived
   PushSlot *slot_state = nullptr;
-  TQ_TRY(push_slot_acquire(slot, &slot_state));  // the previous push of this slot no longer reads the pinned tables or the mask below
+  // the previous push of this slot no longer reads the pinned tables or the mask below
+  TQ_TRY(push_begin(slot, n_parts, dest_counts, keep_misses ? miss_count : nullptr, s, &slot_state));
   PushSlot &ps = *slot_state;
   const int n_pub = n_parts + (keep_misses ? 1 : 0);
   for (int q = 0; q < 16; q++) ps.h_lim.as<uint32_t>()[q] = (uint32_t)region_cap;
-  for (int q = 0; q < n_parts; q++) ps.h_ptrs.as<void *>()[q] = dest_counts[q];
-  if (keep_misses) {
-    ps.h_lim.as<uint32_t>()[n_parts] = (uint32_t)miss_cap;
-    ps.h_ptrs.as<void *>()[n_parts] = miss_count;
-  }
-  TQ_CUDA(cudaMemsetAsync(ps.cursor.p, 0, 64, s));
-  TQ_CUDA(cudaMemsetAsync(ps.ovf.p, 0, 8, s));
+  if (keep_misses) ps.h_lim.as<uint32_t>()[n_parts] = (uint32_t)miss_cap;
   TQ_CUDA(cudaMemcpyAsync(ps.lim.p, ps.h_lim.p, 64, cudaMemcpyHostToDevice, s));
   if (n > 0) {
     if (pack) {  // the mask word and the effective selection first

@@ -35,7 +35,21 @@ __global__ void k_region_wait(const unsigned long long *slots, int n, unsigned l
 
 static PushSlot g_push_slot[PUSH_SLOTS];
 
-int32_t push_slot_acquire(int slot, PushSlot **out) {
+int32_t push_check_dests(const char *fn, int n_parts, int n_wire, void *const *dest_data, void *const *dest_counts, int64_t region_cap,
+                         int slot) {
+  if (!dest_data || !dest_counts || n_parts < 1 || n_parts > 8 || slot < 0 || slot >= PUSH_SLOTS || region_cap < 1 || region_cap > 0xFFFFFFF0ll) {
+    set_error("%s: 1..8 destinations with their regions and count slots, slot 0..%d, 1 <= region_cap < 2^32", fn, PUSH_SLOTS - 1);
+    return TQ_ERR_INVALID_ARG;
+  }
+  for (int q = 0; q < n_parts; q++) {
+    if (!dest_counts[q]) { set_error("%s: destination %d has no count slot", fn, q); return TQ_ERR_INVALID_ARG; }
+    for (int c = 0; c < n_wire; c++)
+      if (!dest_data[q * n_wire + c]) { set_error("%s: destination %d has no region for wire column %d", fn, q, c); return TQ_ERR_INVALID_ARG; }
+  }
+  return TQ_OK;
+}
+
+int32_t push_begin(int slot, int n_parts, void *const *dest_counts, void *extra_count, cudaStream_t s, PushSlot **out) {
   PushSlot &ps = g_push_slot[slot];
   if (!ps.ev) TQ_CUDA(cudaEventCreateWithFlags(&ps.ev, cudaEventDisableTiming));
   TQ_TRY(ps.cursor.reserve(64));
@@ -45,6 +59,10 @@ int32_t push_slot_acquire(int slot, PushSlot **out) {
   TQ_TRY(ps.h_lim.reserve(64));
   TQ_TRY(ps.h_ptrs.reserve(128));
   TQ_CUDA(cudaEventSynchronize(ps.ev));  // the previous push of this slot no longer reads the pinned tables or the scratch
+  for (int q = 0; q < n_parts; q++) ps.h_ptrs.as<void *>()[q] = dest_counts[q];
+  if (extra_count) ps.h_ptrs.as<void *>()[n_parts] = extra_count;
+  TQ_CUDA(cudaMemsetAsync(ps.cursor.p, 0, 64, s));
+  TQ_CUDA(cudaMemsetAsync(ps.ovf.p, 0, 8, s));
   *out = &ps;
   return TQ_OK;
 }

@@ -1,6 +1,7 @@
-// push.cuh — the slot/epoch protocol the region pushes share (push.cu): tq_partition_push_regions (join.cu) and
-// tq_agg_push_partial (agg.cu) scatter into per-source regions of the peers' receive buffers on the push stream, then publish
-// {rows, epoch} in each destination's slot; the receiver waits on those slots with tq_region_wait.
+// push.cuh — what the region pushes share (push.cu): tq_partition_push_regions (join.cu) and tq_agg_push_partial (agg.cu)
+// check their destinations with push_check_dests, set up their slot with push_begin, scatter into per-source regions of the
+// peers' receive buffers on the push stream, then publish {rows, epoch} in each destination's slot with push_publish; the
+// receiver waits on those slots with tq_region_wait.  Where the regions and slots sit is the caller's (dist.RegionLayout).
 #pragma once
 #include "scatter.cuh"
 
@@ -18,9 +19,15 @@ struct PushSlot {
   cudaEvent_t ev = nullptr;
 };
 
-// Slot `slot` (0..PUSH_SLOTS-1, checked by the caller) once its previous push has finished: its event exists, its tables are
-// reserved (cursor, lim, ovf, counts_ptrs, h_lim, h_ptrs) and the caller may rewrite them.
-int32_t push_slot_acquire(int slot, PushSlot **out);
+// The destinations of a push, checked before anything is enqueued: 1 <= n_parts <= 8, 0 <= slot < PUSH_SLOTS,
+// 1 <= region_cap < 2^32, a count slot dest_counts[q] and a region dest_data[q * n_wire + c] for every destination q and wire
+// column c.  A refusal sets the error text under the caller's name fn and returns TQ_ERR_INVALID_ARG.
+int32_t push_check_dests(const char *fn, int n_parts, int n_wire, void *const *dest_data, void *const *dest_counts, int64_t region_cap,
+                         int slot);
+// Slot `slot` (checked by push_check_dests) once its previous push has finished, set up for a new push on s: its tables are
+// reserved (cursor, lim, ovf, counts_ptrs, h_lim, h_ptrs), h_ptrs holds the n_parts count slots (then extra_count, when not
+// null) that push_publish writes, and cursor / ovf are zeroed on s.
+int32_t push_begin(int slot, int n_parts, void *const *dest_counts, void *extra_count, cudaStream_t s, PushSlot **out);
 // Enqueues k_publish_counts on s — slot q (dest_counts[q], q < n_pub) gets {cursor[q] or ~0 when *ovf, epoch} — after copying
 // the n_pub count-slot pointers of ps.h_ptrs to the device, and records ps.ev.
 int32_t push_publish(PushSlot &ps, int n_pub, uint64_t epoch, cudaStream_t s);

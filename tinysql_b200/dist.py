@@ -109,46 +109,111 @@ class RawCol:
         return RawCol(self.ptr, min(self.n, sl.stop))
 
 
-class RegionExchange:
-    """The exchange the multi-GPU join runs on: every rank owns ONE device allocation (tq_device_alloc, exported once through
-    CUDA IPC and opened by every peer under its own device) that holds, per table t (0 = build side, 1.. = probe chunks):
-        slots[t][src] = {u64 rows, u64 epoch}                  16-byte slot per source rank
-        region[t][src][col] = cap_t rows x 8 bytes             where source `src` scatters its rows for THIS rank
-    A rank pushes table t with tq_partition_push_regions: its scatter kernel stores rows straight into "its" region on every
-    peer (NVLink peer stores, no staging, no count exchange first) and then publishes count + epoch in the peer's slot.  The
-    receiver enqueues tq_region_wait(slots[t], world, epoch) — a device-side wait — in front of the kernels that read the
-    regions and joins them as one segmented batch (tq_join_put_probe_segments): no host round trip and no NCCL call sits
-    between the exchange and the join."""
+def _round_up(x, m):
+    return (x + m - 1) // m * m
 
-    def __init__(self, lib, L, world, rank, tables, align_rows=4096):
-        self.lib, self.L, self.world, self.rank = lib, L, world, rank
+
+class RegionLayout:
+    """Where the region exchange's slots and regions sit in a destination's receive buffer, and the argument tables the C
+    calls take from them.  tables = [(wire columns, cap rows)] per table t; every destination's buffer (bytes long, at
+    bases[d], set by whoever places the buffers) holds
+
+        slot[t][src]        = {u64 rows, u64 epoch}             16 bytes per (table, source), from offset 0
+        region[t][src][c]   = cap_t rows x 8 bytes              from the first page boundary after the slots
+
+    with pad_rows rows left unused after every region (0 in production; the emulated-rank tests fill them with a sentinel,
+    so a row written past the cap lands inside the allocation).  bytes is page-aligned, so receive buffers placed back to
+    back keep their slot blocks page-aligned.  Needs no process group, no IPC and no torch: RegionExchange places it over
+    the IPC-opened buffers of the ranks, RegionJoin over one local buffer for its kept miss rows, the tests over W
+    emulated ranks in one allocation."""
+
+    def __init__(self, lib, L, world, tables, pad_rows=0):
+        self.lib, self.L, self.world, self.pad_rows = lib, L, world, pad_rows
         self.ncols = [nc for nc, _ in tables]
-        self.cap = [((cap + align_rows - 1) // align_rows) * align_rows for _, cap in tables]
-        self.slot_off = [t * world * 16 for t in range(len(tables))]
-        off = ((len(tables) * world * 16 + 4095) // 4096) * 4096
+        self.cap = [int(cap) for _, cap in tables]
         self.reg_off = []
+        off = _round_up(len(tables) * world * 16, 4096)
         for nc, cap in zip(self.ncols, self.cap):
             self.reg_off.append(off)
-            off += world * nc * cap * 8
-        self.total = off
+            off += world * nc * (cap + pad_rows) * 8
+        self.bytes = _round_up(off, 4096)
+        self.bases = []
+
+    def region_ptr(self, dst, t, src, c):
+        return self.bases[dst] + self.reg_off[t] + ((src * self.ncols[t] + c) * (self.cap[t] + self.pad_rows)) * 8
+
+    def slot_ptr(self, dst, t, src):
+        return self.bases[dst] + (t * self.world + src) * 16
+
+    def push_tables(self, t, src):
+        """(dest_data, dest_counts) of source src for table t, as tq_partition_push_regions and tq_agg_push_partial take them:
+        dest_data[q * nw + c] = its region of wire column c on destination q, dest_counts[q] = its slot there"""
+        w, nw = self.world, self.ncols[t]
+        dest = (C.c_void_p * (w * nw))(*[self.region_ptr(q, t, src, c) for q in range(w) for c in range(nw)])
+        return dest, (C.c_void_p * w)(*[self.slot_ptr(q, t, src) for q in range(w)])
+
+    def region_table(self, dst, t):
+        """destination dst's regions of table t as tq_column [src][col] (length = cap), as tq_region_gather,
+        tq_agg_merge_regions and tq_join_put_probe_segments take them"""
+        w, nw = self.world, self.ncols[t]
+        regs = (self.L.TQColumn * (w * nw))()
+        for k in range(w * nw):
+            regs[k].length, regs[k].data = self.cap[t], self.region_ptr(dst, t, k // nw, k % nw)
+        return regs
+
+    def count_ptrs(self, dst, t):
+        """the slot of every source on destination dst for table t (tq_join_put_probe_segments)"""
+        return (C.c_void_p * self.world)(*[self.slot_ptr(dst, t, g) for g in range(self.world)])
+
+    def read_slots(self, dst, t0=0, nt=None):
+        """one host read of destination dst's slots of tables t0 .. t0 + nt - 1 (every table from t0 by default): uint64 array
+        [table][src][rows, epoch]"""
+        raw = np.zeros((len(self.cap) - t0 if nt is None else nt, self.world, 2), np.uint64)
+        self.L.check(self.lib.tq_memcpy_d2h(raw.ctypes.data, C.c_void_p(self.slot_ptr(dst, t0, 0)), raw.nbytes))
+        return raw
+
+    def counts(self, dst, t0=0, nt=None):
+        """rows every source published on destination dst, per table (read_slots); a count past its table's cap (an overflowed
+        push publishes ~0: it dropped rows) raises RuntimeError"""
+        out = []
+        for t, raw in enumerate(self.read_slots(dst, t0, nt), start=t0):
+            cnt = [int(r) for r in raw[:, 0]]
+            if any(c > self.cap[t] for c in cnt):
+                raise RuntimeError(f"region overflow in table {t}: {cnt} rows, capacity {self.cap[t]} (skewed keys)")
+            out.append(cnt)
+        return out
+
+
+class RegionExchange(RegionLayout):
+    """The exchange the multi-GPU join and GROUP BY run on: a RegionLayout over one device allocation per rank
+    (tq_device_alloc, exported once through CUDA IPC and opened by every peer under its own device); caps are rounded up to
+    align_rows.  A rank pushes table t with tq_partition_push_regions: its scatter kernel stores rows straight into "its"
+    region on every peer (NVLink peer stores, no staging, no count exchange first) and then publishes count + epoch in the
+    peer's slot.  The receiver enqueues tq_region_wait(slots[t], world, epoch) — a device-side wait — in front of the
+    kernels that read the regions and joins them as one segmented batch (tq_join_put_probe_segments): no host round trip
+    and no NCCL call sits between the exchange and the join."""
+
+    def __init__(self, lib, L, world, rank, tables, align_rows=4096):
+        super().__init__(lib, L, world, [(nc, _round_up(cap, align_rows)) for nc, cap in tables])
+        self.rank = rank
         p = C.c_void_p()
-        L.check(lib.tq_device_alloc(self.total, C.byref(p)))
-        L.check(lib.tq_memset_device(p, 0, self.total))
+        L.check(lib.tq_device_alloc(self.bytes, C.byref(p)))
+        L.check(lib.tq_memset_device(p, 0, self.bytes))
         L.check(lib.tq_device_synchronize())
         self.own = p.value
         h = (C.c_ubyte * 64)()
         L.check(lib.tq_ipc_get_handle(p, h))
         gathered = [None] * world
         dist.all_gather_object(gathered, bytes(h))
-        self.base, self._opened = [], []
+        self._opened = []
         for d in range(world):
             if d == rank:
-                self.base.append(self.own)
+                self.bases.append(self.own)
                 continue
             q = C.c_void_p()
             buf = (C.c_ubyte * 64).from_buffer_copy(gathered[d])
             L.check(lib.tq_ipc_open_handle(buf, C.byref(q)))
-            self.base.append(q.value)
+            self.bases.append(q.value)
             self._opened.append(q.value)
         self.epoch = 0
 
@@ -159,12 +224,6 @@ class RegionExchange:
         dist.barrier()  # nobody frees a buffer a peer still has mapped
         self.lib.tq_device_free(C.c_void_p(self.own))
 
-    def region_ptr(self, dst, t, src, c):
-        return self.base[dst] + self.reg_off[t] + ((src * self.ncols[t] + c) * self.cap[t]) * 8
-
-    def slot_ptr(self, dst, t, src):
-        return self.base[dst] + self.slot_off[t] + src * 16
-
     def next_epoch(self):
         self.epoch += 1
         return self.epoch
@@ -172,58 +231,22 @@ class RegionExchange:
     def push(self, t, cols, n, slot, bitmaps=None, selected=None, miss=None):
         """scatter this rank's rows of table t into its region on every rank; asynchronous (push stream).  bitmaps: a device
         NULL bitmap pointer (or None) per column; with any, the mask word travels as table t's last wire column.  selected:
-        device address of n bytes (0/1) or None.  miss: (wire column pointers, slot pointer, rows) that keep the rows which
-        cannot match on this rank, or None to drop them."""
-        nw, w = self.ncols[t], self.world
+        device address of n bytes (0/1) or None.  miss: (RegionLayout of one destination, its table) that keeps the rows
+        which cannot match on this rank, or None to drop them."""
         arr = _tq_cols(self.L, cols, n)
         for c, b in enumerate(bitmaps or []):
             arr[c].null_bitmap = b
-        dest = (C.c_void_p * (w * nw))()
-        cnts = (C.c_void_p * w)()
-        for d in range(w):
-            for c in range(nw):
-                dest[d * nw + c] = self.region_ptr(d, t, self.rank, c)
-            cnts[d] = self.slot_ptr(d, t, self.rank)
-        miss_cols, miss_slot, miss_cap = (None, None, 0) if miss is None else ((C.c_void_p * nw)(*miss[0]), miss[1], miss[2])
-        self.L.check(self.lib.tq_partition_push_regions(len(cols), arr, 0, n, w, selected, int(miss is not None), dest, cnts, self.cap[t],
+        dest, cnts = self.push_tables(t, self.rank)
+        miss_cols, miss_slot, miss_cap = None, None, 0
+        if miss is not None:
+            ml, mt = miss
+            miss_cols, miss_slot, miss_cap = ml.push_tables(mt, 0)[0], ml.slot_ptr(0, mt, 0), ml.cap[mt]
+        self.L.check(self.lib.tq_partition_push_regions(len(cols), arr, 0, n, self.world, selected, int(miss is not None), dest, cnts, self.cap[t],
                                                         miss_cols, miss_slot, miss_cap, slot, self.epoch))
 
     def wait(self, t):
         """device-side: the compute stream waits until every source has published table t for this epoch"""
         self.L.check(self.lib.tq_region_wait(C.c_void_p(self.slot_ptr(self.rank, t, 0)), self.world, self.epoch))
-
-    def counts(self, t):
-        """rows each source wrote into this rank's regions of table t (host read: synchronises the compute stream)"""
-        self.wait(t)
-        self.L.check(self.lib.tq_compute_synchronize())   # the compute stream only: the pushes of later tables keep running
-        raw = np.zeros(2 * self.world, dtype=np.uint64)
-        self.L.check(self.lib.tq_memcpy_d2h(raw.ctypes.data, C.c_void_p(self.slot_ptr(self.rank, t, 0)), 16 * self.world))
-        cnt = [int(raw[2 * g]) for g in range(self.world)]
-        if any(c > self.cap[t] for c in cnt):
-            raise RuntimeError(f"region overflow in table {t}: {cnt} rows, capacity {self.cap[t]} (skewed keys)")
-        return cnt
-
-    def check_all_counts(self):
-        """one host read of every slot of this rank (after the step's joins have consumed the regions): overflow check"""
-        nt = len(self.ncols)
-        raw = np.zeros(2 * self.world * nt, dtype=np.uint64)
-        self.L.check(self.lib.tq_memcpy_d2h(raw.ctypes.data, C.c_void_p(self.slot_ptr(self.rank, 0, 0)), 16 * self.world * nt))
-        for t in range(nt):
-            cnt = [int(raw[2 * (t * self.world + g)]) for g in range(self.world)]
-            if any(c > self.cap[t] for c in cnt):
-                raise RuntimeError(f"region overflow in table {t}: {cnt} rows, capacity {self.cap[t]} (skewed keys)")
-
-    def segment_args(self, t):
-        """(tq_column array [src][col], count pointer array) of this rank's regions of table t"""
-        nc, w = self.ncols[t], self.world
-        cols = (self.L.TQColumn * (w * nc))()
-        cnts = (C.c_void_p * w)()
-        for g in range(w):
-            for c in range(nc):
-                k = g * nc + c
-                cols[k].length, cols[k].data, cols[k].null_bitmap, cols[k].offsets = self.cap[t], self.region_ptr(self.rank, t, g, c), None, None
-            cnts[g] = self.slot_ptr(self.rank, t, g)
-        return cols, cnts
 
 
 def distributed_join(build_cols, probe_cols, world, rank, partition_fn, local_join_fn, group=None):
@@ -393,7 +416,8 @@ class RegionJoin:
     (tq_join_put_probe_segments).  Otherwise (an outer join, or a side declared nullable) a nullable side's push carries the
     mask word, the probe rows of an outer join that cannot match (NULL key, selected == 0) stay on this rank, and the
     receiver copies each table's regions into contiguous columns with tq_region_gather before tq_join_put_build /
-    tq_join_put_probe; the kept rows are one more probe batch, unselected."""
+    tq_join_put_probe; the kept rows are one more probe batch, unselected.  They land in a local RegionLayout of one
+    destination (one table per probe chunk), so _gather reads them as it reads the exchanged tables."""
 
     def __init__(self, lib, L, world, rank, n_build_max, n_probe_max, n_chunks, slack=1.25, join_type=0, outer_is_right=True,
                  build_types=None, probe_types=None, build_nullable=False, probe_nullable=False, default_inner=None):
@@ -422,10 +446,8 @@ class RegionJoin:
             self.g_probe = self._cols(npc, world * rx.cap[1], self.pmask)
             if self.outer:
                 self.g_miss = self._cols(npc, self.chunk_max, self.pmask)
-                # this rank's miss rows of chunk c: wire columns of chunk_max rows and a 16-byte {rows, epoch} slot
-                nw = npc + self.pmask
-                self.miss_data = [[self._alloc(max(self.chunk_max, 1) * 8) for _ in range(nw)] for _ in range(n_chunks)]
-                self.miss_slot = [self._alloc(16, zero=True) for _ in range(n_chunks)]
+                self.misses = RegionLayout(lib, L, 1, [(npc + self.pmask, self.chunk_max)] * n_chunks)
+                self.misses.bases = [self._alloc(self.misses.bytes, zero=True)]
 
     def _alloc(self, nbytes, zero=False):
         p = C.c_void_p()
@@ -508,14 +530,16 @@ class RegionJoin:
         try:
             if self.segmented:
                 # ---- build side: the only place the host needs row counts
-                cnt_b = rx.counts(0)
+                rx.wait(0)
+                L.check(lib.tq_compute_synchronize())        # the compute stream only: the pushes of later tables keep running
+                cnt_b = rx.counts(self.rank, 0, 1)[0]
                 mark("build rows arrived (host read)")
                 for g in range(w):
                     if cnt_b[g]:
                         cols = [RawCol(rx.region_ptr(self.rank, 0, g, c), cnt_b[g]) for c in range(len(self.build_types))]
                         L.check(lib.tq_join_put_build(h, _tq_cols(L, cols, cnt_b[g]), L.TQ_MEM_DEVICE))
             else:
-                rows = self._gather(0, self.g_build, self.bmask)
+                rows = self._gather(rx, self.rank, 0, self.g_build, self.bmask)
                 if rows:
                     L.check(lib.tq_join_put_build(h, self.g_build[0], L.TQ_MEM_DEVICE))
                 mark("build rows arrived (gathered)")
@@ -543,8 +567,7 @@ class RegionJoin:
             for c in range(self.n_chunks):
                 if self.segmented:
                     rx.wait(1 + c)                                   # device-side: chunk c has landed from every source
-                    cols, cnts = rx.segment_args(1 + c)
-                    L.check(lib.tq_join_put_probe_segments(h, w, cols, cnts, rx.cap[1 + c]))
+                    L.check(lib.tq_join_put_probe_segments(h, w, rx.region_table(self.rank, 1 + c), rx.count_ptrs(self.rank, 1 + c), rx.cap[1 + c]))
                     mark(f"chunk {c} enqueued")
                     if c >= 1:
                         drain(False)                                 # hand back the batch before last (keeps two result sets alive, not n_chunks)
@@ -552,10 +575,10 @@ class RegionJoin:
                     continue
                 # gather path: a put borrows its columns until its batch is finished, so the chunk is drained before the
                 # next one reuses the gather buffers
-                if self._gather(1 + c, self.g_probe, self.pmask):
+                if self._gather(rx, self.rank, 1 + c, self.g_probe, self.pmask):
                     L.check(lib.tq_join_put_probe(h, self.g_probe[0], None, L.TQ_MEM_DEVICE))
                 if self.outer:
-                    m = self._gather_misses(c)
+                    m = self._gather(self.misses, 0, c, self.g_miss, self.pmask)
                     if m:
                         zeros = np.zeros(m, np.uint8)
                         L.check(lib.tq_join_put_probe(h, self.g_miss[0], zeros.ctypes.data, L.TQ_MEM_DEVICE))
@@ -573,7 +596,7 @@ class RegionJoin:
                     result = Chunk.concat([Chunk(ch) for ch in chunks], out_types).cols if chunks else [Column.empty(t, 0) for t in out_types]
         finally:
             lib.tq_join_destroy(h)
-        rx.check_all_counts()                                    # a region overflow would have dropped rows: fail loudly
+        rx.counts(self.rank)                                     # a region overflow would have dropped rows: fail loudly
         mark("overflow checks")
         dist.barrier()
         mark("barrier")
@@ -586,33 +609,17 @@ class RegionJoin:
         if (self.bmask if t == 0 else self.pmask) and n and not any(bms):
             bms = [self._ones(n)]                      # a side declared nullable always carries the mask word: the layout is shared
         sel = None if (t == 0 or selected is None) else selected.data_ptr() + row0
-        miss = (self.miss_data[chunk], self.miss_slot[chunk], self.chunk_max) if t > 0 and self.outer else None
+        miss = (self.misses, chunk) if t > 0 and self.outer else None
         self.rx.push(t, cols, n, slot, bms, sel, miss)
 
-    def _gather(self, t, target, has_mask):
-        """wait (device-side) for table t from every source and copy its regions into target; returns the rows"""
-        rx, L, w = self.rx, self.L, self.world
-        rx.wait(t)
-        nw = rx.ncols[t]
-        regs = (L.TQColumn * (w * nw))()
-        for g in range(w):
-            for c in range(nw):
-                regs[g * nw + c].data = rx.region_ptr(self.rank, t, g, c)
+    def _gather(self, layout, dst, t, target, has_mask):
+        """wait (device-side) for table t of destination dst of layout from every source and copy its regions into target;
+        returns the rows"""
+        slots = C.c_void_p(layout.slot_ptr(dst, t, 0))
+        self.L.check(self.lib.tq_region_wait(slots, layout.world, self.rx.epoch))
         n = C.c_int64(0)
-        L.check(self.lib.tq_region_gather(w, C.c_void_p(rx.slot_ptr(self.rank, t, 0)), rx.cap[t], nw - has_mask, has_mask, regs, target[0], target[1], C.byref(n)))
-        return n.value
-
-    def _gather_misses(self, c):
-        """this rank's kept probe rows of chunk c (published by its own push) as contiguous columns; returns the rows"""
-        L = self.L
-        nw = len(self.probe_types) + self.pmask
-        L.check(self.lib.tq_region_wait(C.c_void_p(self.miss_slot[c]), 1, self.rx.epoch))
-        regs = (L.TQColumn * nw)()
-        for k in range(nw):
-            regs[k].data = self.miss_data[c][k]
-        n = C.c_int64(0)
-        L.check(self.lib.tq_region_gather(1, C.c_void_p(self.miss_slot[c]), max(self.chunk_max, 1), len(self.probe_types), self.pmask, regs,
-                                          self.g_miss[0], self.g_miss[1], C.byref(n)))
+        self.L.check(self.lib.tq_region_gather(layout.world, slots, layout.cap[t], layout.ncols[t] - has_mask, has_mask, layout.region_table(dst, t),
+                                               target[0], target[1], C.byref(n)))
         return n.value
 
 
@@ -691,7 +698,6 @@ class RegionAgg:
         pointer (or None) per column.  Returns (groups finished on this rank, result): result (keep_result) = host Columns of
         the function outputs, None otherwise."""
         lib, L, rx, w = self.lib, self.L, self.rx, self.world
-        nw = self.width + 1
         n = int(cols[0].numel()) if cols else 0
         rx.next_epoch()
         hp, keep_p = self._create()
@@ -703,19 +709,10 @@ class RegionAgg:
                     arr[c].null_bitmap = b
                 L.check(lib.tq_agg_put(hp, arr, L.TQ_MEM_DEVICE))
             L.check(lib.tq_agg_eof(hp))
-            dest = (C.c_void_p * (w * nw))()
-            cnts = (C.c_void_p * w)()
-            for d in range(w):
-                for c in range(nw):
-                    dest[d * nw + c] = rx.region_ptr(d, 0, self.rank, c)
-                cnts[d] = rx.slot_ptr(d, 0, self.rank)
+            dest, cnts = rx.push_tables(0, self.rank)
             L.check(lib.tq_agg_push_partial(hp, w, dest, cnts, rx.cap[0], self.slot, rx.epoch))
             rx.wait(0)
-            regs = (L.TQColumn * (w * nw))()
-            for g in range(w):
-                for c in range(nw):
-                    regs[g * nw + c].data = rx.region_ptr(self.rank, 0, g, c)
-            L.check(lib.tq_agg_merge_regions(hf, w, C.c_void_p(rx.slot_ptr(self.rank, 0, 0)), rx.cap[0], regs))
+            L.check(lib.tq_agg_merge_regions(hf, w, C.c_void_p(rx.slot_ptr(self.rank, 0, 0)), rx.cap[0], rx.region_table(self.rank, 0)))
             L.check(lib.tq_agg_eof(hf))
             L.check(lib.tq_partition_push_sync(self.slot))     # the push reads the Partial1 handle's rows until it is done
             res, groups = None, 0
