@@ -659,6 +659,28 @@ int32_t tq_partition_push_regions(int32_t n_cols, const tq_column *cols, int32_t
                                   const uint8_t *selected, int32_t keep_misses, void *const *dest_data, void *const *dest_counts,
                                   int64_t region_cap, void *const *miss_data, void *miss_count, int64_t miss_cap, int32_t slot,
                                   uint64_t epoch);
+/* The broadcast push (the other classic distributed join: replicate the build side, keep the probe side in place): copies
+ * this rank's n rows into its region on each of the n_parts destinations, this rank included, then publishes {n, epoch} in
+ * each destination's slot as tq_partition_push_regions does.  Every destination receives the rows in input order.
+ *  - n_parts 1..8, 1..16 columns, 0 <= n <= region_cap < 2^32.
+ *  - types[c] & 0xFF: INT64, UINT64 and FLOAT64 travel as 8-byte values; BYTES as its offsets, rebased to start at 0 (n + 1
+ *    entries), and its cells [offsets[0], offsets[n]) copied to the start of a byte area of byte_cap[c] bytes.  FLOAT32 (and
+ *    any other type) is TQ_ERR_UNSUPPORTED_TYPE: device puts refuse FLOAT columns.  offsets must be set exactly on the BYTES
+ *    columns (TQ_ERR_INVALID_ARG otherwise), and may start anywhere, as for a TQ_MEM_DEVICE put.
+ *  - nullable != 0: every column also travels as its ceil(n / 64) 64-row NULL bitmap words, all ones for a column without a
+ *    bitmap, so the layout depends only on the declaration.  The receiver hands the words to tq_join_put_build as they are.
+ *  - Areas per destination q, column by column: dest_data[q * n_areas + a] with, for each column c in order, its values (n
+ *    words) or offsets (n + 1 words), then for BYTES its byte area, then on a nullable side its bitmap words.  n_areas =
+ *    n_cols + (BYTES columns) + (nullable ? n_cols : 0).  Each area is stored with 16-byte stores where it is 16-byte aligned.
+ *  - dest_counts[q]: the 16-byte slot {u64 rows, u64 epoch} on rank q.
+ * Every argument is checked before anything is enqueued: a refused push writes no region and publishes no slot.  Cells that
+ * exceed byte_cap[c] are found on the device: that column's cells are not copied and every slot this push publishes reads
+ * ~0, so the receiver fails (tq_region_gather: TQ_ERR_OOM; dist.RegionLayout.counts: RuntimeError).  The push is enqueued
+ * on the push stream; tq_partition_push_sync(slot) waits for it.  The receiver waits with tq_region_wait, reads the slots
+ * and puts each source's region as one device build chunk (tq_join_put_build, TQ_MEM_DEVICE). */
+int32_t tq_partition_push_broadcast(int32_t n_cols, const tq_column *cols, const int32_t *types, int32_t nullable, int64_t n, int32_t n_parts,
+                                    void *const *dest_data, void *const *dest_counts, int64_t region_cap, const int64_t *byte_cap, int32_t slot,
+                                    uint64_t epoch);
 int32_t tq_partition_push_sync(int32_t slot);
 /* Enqueues, on the compute stream, a kernel that waits (bounded) until the n_sources consecutive slots at `slots` (this rank's
  * own table) carry `epoch` — the device-side barrier between the peers' pushes and the kernels that read the regions; no host

@@ -150,6 +150,8 @@ SYMBOLS = {
     "tq_ipc_get_handle": (_I32, [_P, _P]), "tq_ipc_open_handle": (_I32, [_P, C.POINTER(_P)]), "tq_ipc_close_handle": (_I32, [_P]),
     "tq_partition_push_regions": (_I32, [_I32, _COL, _I32, _I64, _I32, _P, _I32, C.POINTER(_P), C.POINTER(_P), _I64, C.POINTER(_P), _P,
                                          _I64, _I32, C.c_uint64]),
+    "tq_partition_push_broadcast": (_I32, [_I32, _COL, C.POINTER(_I32), _I32, _I64, _I32, C.POINTER(_P), C.POINTER(_P), _I64, C.POINTER(_I64),
+                                           _I32, C.c_uint64]),
     "tq_region_wait": (_I32, [_P, _I32, C.c_uint64]),
     "tq_region_gather": (_I32, [_I32, _P, _I64, _I32, _I32, _COL, _COL, _I64, C.POINTER(_I64)]),
     "tq_partition_push_sync": (_I32, [_I32]),

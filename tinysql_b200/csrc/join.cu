@@ -38,6 +38,21 @@
 namespace tq {
 
 static constexpr int MAXC = 16;  // columns per join side
+
+// Bits [off, off + rows) of a concatenated device bitmap from one chunk's bitmap (bit i = row i of the chunk), for a chunk that
+// does not start on a byte boundary: each thread owns one 32-bit destination word and rewrites only the chunk's bits in it.
+__global__ void k_bitmap_append(uint32_t *dst, int64_t off, const uint8_t *src, int64_t rows) {
+  const int64_t w1 = (off + rows + 31) >> 5;
+  for (int64_t w = (off >> 5) + (int64_t)blockIdx.x * blockDim.x + threadIdx.x; w < w1; w += (int64_t)gridDim.x * blockDim.x) {
+    uint32_t v = dst[w];
+    for (int b = 0; b < 32; b++) {
+      const int64_t i = (w << 5) + b - off;
+      if (i < 0 || i >= rows) continue;
+      v = (v & ~(1u << b)) | ((uint32_t)((src[i >> 3] >> (i & 7)) & 1) << b);
+    }
+    dst[w] = v;
+  }
+}
 static constexpr uint64_t EMPTY_KEY = 0xA5C3F00DDEADBEEFull;  // empty-entry marker; a real key with this value lives in a side entry/segment
 static constexpr uint32_t ROW_INVALID = 0xFFFFFFFFu, ROW_SENTINEL = 0xFFFFFFFEu;
 static constexpr uint32_t OFF_MISS = 0xFFFFFFFFu;
@@ -3248,7 +3263,7 @@ int32_t tq_join_finalize_build(tq_join *j) {
       j->b_view[c].bm = (const uint32_t *)j->b_dev_chunks[0][c].null_bitmap;
     }
   } else if (j->build_mem == TQ_MEM_DEVICE) {
-    // several device chunks: concatenate (data D2D; bitmaps need 8-row alignment at chunk boundaries)
+    // several device chunks: concatenate (data D2D; a bitmap copied whole where its chunk starts on a byte, bit-shifted where not)
     for (int c = 0; c < j->nb_user; c++) {
       if (!j->b_ind[c]) TQ_TRY(j->b_cols[c].data.reserve((size_t)j->n_build * 8));
       TQ_TRY(j->b_cols[c].bm.reserve(bitmap_alloc_bytes(j->n_build)));
@@ -3260,8 +3275,13 @@ int32_t tq_join_finalize_build(tq_join *j) {
         const int64_t rows = ch[c].length;
         if (!j->b_ind[c])
           TQ_CUDA(cudaMemcpyAsync(j->b_cols[c].data.as<uint8_t>() + off * 8, ch[c].data, (size_t)rows * 8, cudaMemcpyDeviceToDevice, r.compute));
-        if (ch[c].null_bitmap) {
-          if (off & 7) { set_error("device build chunks with NULL bitmaps must have row counts that are multiples of 8"); return TQ_ERR_INVALID_ARG; }
+        if (ch[c].null_bitmap && (off & 7)) {
+          const int64_t words = ((off + rows + 31) >> 5) - (off >> 5), cap = (int64_t)r.sm_count * 4;
+          TQ_LAUNCH(k_bitmap_append, (unsigned)(words < 256 ? 1 : (words / 256 < cap ? words / 256 : cap)), 256, 0, r.compute, j->b_cols[c].bm.as<uint32_t>(), off,
+                    (const uint8_t *)ch[c].null_bitmap, rows);
+          count_launch();
+          TQ_TRY(check_launch("k_bitmap_append"));
+        } else if (ch[c].null_bitmap) {
           TQ_CUDA(cudaMemcpyAsync(j->b_cols[c].bm.as<uint8_t>() + (off >> 3), ch[c].null_bitmap, bitmap_bytes(rows), cudaMemcpyDeviceToDevice, r.compute));
         }
         off += rows;

@@ -327,6 +327,137 @@ int32_t expand_null_mask(const uint64_t *mask, int64_t n, int n_cols, uint32_t *
   return check_launch("k_expand_mask");
 }
 
+// ---- the broadcast push (tq_partition_push_broadcast, push.cu): every row to every destination, var-len columns included
+struct BcastParams {
+  int n_cols, n_parts, nullable;
+  int64_t n;
+  uint8_t is_bytes[BCAST_MAXC];
+  const uint64_t *data[BCAST_MAXC];  // 8-byte values, or the n + 1 offsets of a BYTES column
+  const uint8_t *cells[BCAST_MAXC];  // a BYTES column's cells
+  const uint64_t *bm[BCAST_MAXC];    // 64-row bitmap words; null = no NULLs
+  uint64_t byte_cap[BCAST_MAXC];
+  uint64_t *dst_data[8][BCAST_MAXC];
+  uint8_t *dst_cells[8][BCAST_MAXC];
+  uint64_t *dst_bm[8][BCAST_MAXC];
+  uint32_t *rows;
+  unsigned long long *overflow;
+};
+static_assert(sizeof(BcastParams) <= 4096, "the broadcast's parameters fit the 4 KB kernel parameter space");
+
+__device__ __forceinline__ void bcast_store16(uint64_t *d, uint64_t a, uint64_t b) {
+  ulonglong2 v;
+  v.x = a;
+  v.y = b;
+  *reinterpret_cast<ulonglong2 *>(d) = v;
+}
+
+// Word k of a copied word area: a value, an offset rebased to 0, or a bitmap word (all ones without a bitmap).
+__device__ __forceinline__ uint64_t bcast_word(const uint64_t *src, int kind, uint64_t base, int64_t k) {
+  if (kind == 2) return src ? src[k] : ~0ull;
+  return src[k] - (kind == 1 ? base : 0);
+}
+
+// One 16-byte chunk per thread and step: two words are read once and stored to every destination, as one 16-byte store where
+// the destination allows it.  kind 0 = values, 1 = offsets, 2 = bitmap words.
+__device__ __forceinline__ void bcast_words(const BcastParams &p, int c, int kind, const uint64_t *src, uint64_t base, int64_t nw, int64_t t,
+                                            int64_t stride) {
+  for (int64_t i = t; 2 * i < nw; i += stride) {
+    const int64_t k = 2 * i;
+    const bool pair = k + 1 < nw;
+    const uint64_t a = bcast_word(src, kind, base, k), b = pair ? bcast_word(src, kind, base, k + 1) : 0;
+    for (int q = 0; q < p.n_parts; q++) {
+      uint64_t *d = (kind == 2 ? p.dst_bm[q][c] : p.dst_data[q][c]) + k;
+      if (pair && ((uintptr_t)d & 15) == 0) {
+        bcast_store16(d, a, b);
+      } else {
+        d[0] = a;
+        if (pair) d[1] = b;
+      }
+    }
+  }
+}
+
+// The cells [off0, off0 + len) of a BYTES column to the start of each byte area.  Destination chunk i needs source bytes
+// [16 i, 16 i + 16): read as the aligned 8-byte words that hold them (each holds at least one of the column's bytes, so no read
+// leaves the cells' allocation), shifted into place.
+__device__ __forceinline__ void bcast_cells(const BcastParams &p, int c, const uint8_t *src, uint64_t len, int64_t t, int64_t stride) {
+  for (uint64_t i = (uint64_t)t; 16 * i < len; i += (uint64_t)stride) {
+    const uint64_t lo = 16 * i, cnt = len - lo < 16 ? len - lo : 16;
+    const uint8_t *s = src + lo;
+    const unsigned a = (unsigned)((uintptr_t)s & 7);
+    const uint64_t *w = reinterpret_cast<const uint64_t *>(s - a);
+    const unsigned last = (unsigned)((a + cnt - 1) >> 3);
+    const uint64_t w0 = w[0], w1 = last >= 1 ? w[1] : 0, w2 = last >= 2 ? w[2] : 0;
+    const uint64_t x = a ? (w0 >> (8 * a)) | (w1 << (64 - 8 * a)) : w0;
+    const uint64_t y = a ? (w1 >> (8 * a)) | (w2 << (64 - 8 * a)) : w1;
+    for (int q = 0; q < p.n_parts; q++) {
+      uint8_t *d = p.dst_cells[q][c] + lo;
+      if (cnt == 16 && ((uintptr_t)d & 15) == 0) {
+        bcast_store16(reinterpret_cast<uint64_t *>(d), x, y);
+      } else {
+        for (unsigned b = 0; b < cnt; b++) d[b] = (uint8_t)((b < 8 ? x >> (8 * b) : y >> (8 * (b - 8))) & 0xFF);
+      }
+    }
+  }
+}
+
+__global__ void __launch_bounds__(256) k_broadcast(const BcastParams p) {
+  const int64_t t = (int64_t)blockIdx.x * blockDim.x + threadIdx.x, stride = (int64_t)gridDim.x * blockDim.x;
+  bool ovf = false;
+  for (int c = 0; c < p.n_cols; c++) {
+    if (p.is_bytes[c]) {
+      const uint64_t off0 = p.data[c][0], len = p.data[c][p.n] - off0;
+      bcast_words(p, c, 1, p.data[c], off0, p.n + 1, t, stride);
+      if (len > p.byte_cap[c]) ovf = true;   // every thread sees it: none writes the cells
+      else bcast_cells(p, c, p.cells[c] + off0, len, t, stride);
+    } else {
+      bcast_words(p, c, 0, p.data[c], 0, p.n, t, stride);
+    }
+    if (p.nullable) bcast_words(p, c, 2, p.bm[c], 0, (p.n + 63) >> 6, t, stride);
+  }
+  if (t < p.n_parts) p.rows[t] = (uint32_t)p.n;
+  if (t == 0 && ovf) *p.overflow = 1;
+}
+
+int32_t broadcast_rows(int n_cols, const tq_column *cols, const int32_t *types, int nullable, int64_t n, int n_parts, void *const *dest_data,
+                       const int64_t *byte_cap, uint32_t *rows, unsigned long long *overflow, cudaStream_t s) {
+  if (n_cols < 1 || n_cols > BCAST_MAXC || n_parts < 1 || n_parts > 8 || n < 0 || n > 0xFFFFFFF0ll) {
+    set_error("internal: broadcast_rows arguments");
+    return TQ_ERR_INVALID_ARG;
+  }
+  BcastParams p{};
+  p.n_cols = n_cols;
+  p.n_parts = n_parts;
+  p.nullable = nullable ? 1 : 0;
+  p.n = n;
+  p.rows = rows;
+  p.overflow = overflow;
+  const int n_wire = broadcast_wire_areas(n_cols, types, nullable);
+  int64_t chunks = 0;   // 16-byte chunks of the largest area: every area is walked by the whole grid
+  for (int c = 0; c < n_cols; c++) {
+    const bool bytes = (types[c] & 0xFF) == TQ_TYPE_BYTES;
+    p.is_bytes[c] = bytes;
+    p.data[c] = reinterpret_cast<const uint64_t *>(bytes ? (const void *)cols[c].offsets : (const void *)cols[c].data);
+    p.cells[c] = bytes ? cols[c].data : nullptr;
+    p.bm[c] = reinterpret_cast<const uint64_t *>(cols[c].null_bitmap);
+    p.byte_cap[c] = bytes ? (uint64_t)byte_cap[c] : 0;
+    const int64_t area = bytes ? (byte_cap[c] + 15) / 16 : (n + 1) / 2;
+    chunks = area > chunks ? area : chunks;
+  }
+  for (int q = 0; q < n_parts; q++) {
+    int a = q * n_wire;
+    for (int c = 0; c < n_cols; c++) {
+      p.dst_data[q][c] = static_cast<uint64_t *>(dest_data[a++]);
+      if (p.is_bytes[c]) p.dst_cells[q][c] = static_cast<uint8_t *>(dest_data[a++]);
+      if (nullable) p.dst_bm[q][c] = static_cast<uint64_t *>(dest_data[a++]);
+    }
+  }
+  const int64_t blocks = (chunks + 255) / 256, cap = (int64_t)rt().sm_count * 8;
+  TQ_LAUNCH(k_broadcast, (unsigned)(blocks < 1 ? 1 : (blocks < cap ? blocks : cap)), 256, 0, s, p);
+  count_launch();
+  return check_launch("k_broadcast");
+}
+
 }  // namespace tq
 
 using namespace tq;

@@ -94,6 +94,39 @@ int32_t tq_region_wait(const void *slots, int32_t n_sources, uint64_t epoch) {
   return check_launch("k_region_wait");
 }
 
+int32_t tq_partition_push_broadcast(int32_t n_cols, const tq_column *cols, const int32_t *types, int32_t nullable, int64_t n, int32_t n_parts,
+                                    void *const *dest_data, void *const *dest_counts, int64_t region_cap, const int64_t *byte_cap, int32_t slot,
+                                    uint64_t epoch) {
+  TQ_TRY(ensure_init());
+  const char *fn = "tq_partition_push_broadcast";
+  if (!cols || !types || n_cols < 1 || n_cols > BCAST_MAXC || n < 0 || n > 0xFFFFFFF0ll || n > region_cap) {
+    set_error("%s: needs 1..%d columns with their types and 0 <= n <= region_cap rows", fn, BCAST_MAXC);
+    return TQ_ERR_INVALID_ARG;
+  }
+  for (int c = 0; c < n_cols; c++) {
+    const int t = types[c] & 0xFF;
+    if (t != TQ_TYPE_INT64 && t != TQ_TYPE_UINT64 && t != TQ_TYPE_FLOAT64 && t != TQ_TYPE_BYTES) {
+      set_error("%s: column %d has type %d: device columns are INT64, UINT64, FLOAT64 or BYTES", fn, c, types[c]);
+      return TQ_ERR_UNSUPPORTED_TYPE;
+    }
+    const bool bytes = t == TQ_TYPE_BYTES;
+    if (bytes != (cols[c].offsets != nullptr) || (n > 0 && !bytes && !cols[c].data)) {
+      set_error("%s: column %d: offsets exactly on BYTES columns, data on every 8-byte column", fn, c);
+      return TQ_ERR_INVALID_ARG;
+    }
+    if (bytes && (!byte_cap || byte_cap[c] < 0)) { set_error("%s: BYTES column %d needs byte_cap[%d] >= 0", fn, c, c); return TQ_ERR_INVALID_ARG; }
+  }
+  const int n_wire = broadcast_wire_areas(n_cols, types, nullable);
+  TQ_TRY(push_check_dests(fn, n_parts, n_wire, dest_data, dest_counts, region_cap, slot));
+  Runtime &r = rt();
+  std::lock_guard<std::recursive_mutex> lk(r.mu);
+  cudaStream_t s = r.h2d;   // the push stream, as tq_partition_push_regions
+  PushSlot *ps = nullptr;
+  TQ_TRY(push_begin(slot, n_parts, dest_counts, nullptr, s, &ps));
+  TQ_TRY(broadcast_rows(n_cols, cols, types, nullable, n, n_parts, dest_data, byte_cap, ps->cursor.as<uint32_t>(), ps->ovf.as<unsigned long long>(), s));
+  return push_publish(*ps, n_parts, epoch, s);
+}
+
 int32_t tq_partition_push_sync(int32_t slot) {
   TQ_TRY(ensure_init());
   if (slot < 0 || slot >= PUSH_SLOTS || !g_push_slot[slot].ev) return TQ_ERR_INVALID_ARG;

@@ -1,4 +1,5 @@
-// push.cuh — what the region pushes share (push.cu): tq_partition_push_regions (join.cu) and tq_agg_push_partial (agg.cu)
+// push.cuh — what the region pushes share (push.cu): tq_partition_push_regions (join.cu), tq_agg_push_partial (agg.cu) and
+// tq_partition_push_broadcast (push.cu)
 // check their destinations with push_check_dests, set up their slot with push_begin, scatter into per-source regions of the
 // peers' receive buffers on the push stream, then publish {rows, epoch} in each destination's slot with push_publish; the
 // receiver waits on those slots with tq_region_wait.  Where the regions and slots sit is the caller's (dist.RegionLayout).

@@ -49,4 +49,20 @@ int32_t scatter_to_regions(const DCol *cols, int n_cols, const uint8_t *dest, in
 // groups, 0 past the last row.  Enqueued on s.
 int32_t expand_null_mask(const uint64_t *mask, int64_t n, int n_cols, uint32_t *const *bm, cudaStream_t s);
 
+// ---- the broadcast push (partition.cu; tq_partition_push_broadcast in push.cu)
+// The areas of one column on the wire, in order: its values (8-byte types) or its rebased offsets (BYTES), then a BYTES
+// column's cells, then, on a nullable side, its 64-row bitmap words.  Returns the areas per destination.
+static constexpr int BCAST_MAXC = 16;
+inline int broadcast_wire_areas(int n_cols, const int32_t *types, int nullable) {
+  int a = 0;
+  for (int c = 0; c < n_cols; c++) a += 1 + ((types[c] & 0xFF) == TQ_TYPE_BYTES) + (nullable ? 1 : 0);
+  return a;
+}
+// Copies n rows (0 <= n < 2^32) of the n_cols (1..BCAST_MAXC) columns to each of the n_parts (1..8) destinations, whose areas
+// are dest_data[q * n_areas + a] (broadcast_wire_areas).  Types and offsets are the caller's to check.  rows[q] (device u32)
+// = n for every destination; *overflow (device u64, caller-zeroed) = 1 when a BYTES column's cells exceed byte_cap[c], and
+// then no destination gets that column's cells.  One launch, enqueued on s.
+int32_t broadcast_rows(int n_cols, const tq_column *cols, const int32_t *types, int nullable, int64_t n, int n_parts, void *const *dest_data,
+                       const int64_t *byte_cap, uint32_t *rows, unsigned long long *overflow, cudaStream_t s);
+
 }  // namespace tq

@@ -8,6 +8,11 @@ Two exchanges:
     memory (CUDA IPC); device-side epoch flags replace host barriers.
       - RegionJoin (the default of bench.py --gpus N): chunk by chunk, overlapped with the local join of the chunks that have
         already arrived.
+      - BroadcastJoin: every rank copies its build shard to every rank (tq_partition_push_broadcast) and joins its own probe
+        shard in place; runs every join the single-GPU handle runs (key-less, multi-column and string keys, wide rows,
+        OtherConditions).  Use it where RegionJoin cannot route the join, or where the build side is small: it moves
+        (W-1) x the build side over NVLink and holds W x the build side per rank, where the shuffle moves (W-1)/W of both
+        sides.  RegionJoin stays the path for the one-key joins it runs.
       - RegionAgg: each rank's Partial1 aggregation pushes its partial rows (tq_agg_push_partial, NULL mask word included, any
         number of GROUP BY items) to the rank its group names; that rank merges the regions in place
         (tq_agg_merge_regions) and finalises.
@@ -115,13 +120,14 @@ def _round_up(x, m):
 
 class RegionLayout:
     """Where the region exchange's slots and regions sit in a destination's receive buffer, and the argument tables the C
-    calls take from them.  tables = [(wire columns, cap rows)] per table t; every destination's buffer (bytes long, at
-    bases[d], set by whoever places the buffers) holds
+    calls take from them.  tables = [(wire columns, cap rows)] per table t, or (wire columns, cap rows, [words per wire
+    column]) for a table whose areas are not cap rows of 8 bytes each (the broadcast's offsets, cells and bitmap words);
+    every destination's buffer (bytes long, at bases[d], set by whoever places the buffers) holds
 
         slot[t][src]        = {u64 rows, u64 epoch}             16 bytes per (table, source), from offset 0
         region[t][src][c]   = cap_t rows x 8 bytes              from the first page boundary after the slots
 
-    with pad_rows rows left unused after every region (0 in production; the emulated-rank tests fill them with a sentinel,
+    with pad_rows rows (words) left unused after every region (0 in production; the emulated-rank tests fill them with a sentinel,
     so a row written past the cap lands inside the allocation).  bytes is page-aligned, so receive buffers placed back to
     back keep their slot blocks page-aligned.  Needs no process group, no IPC and no torch: RegionExchange places it over
     the IPC-opened buffers of the ranks, RegionJoin over one local buffer for its kept miss rows, the tests over W
@@ -129,18 +135,24 @@ class RegionLayout:
 
     def __init__(self, lib, L, world, tables, pad_rows=0):
         self.lib, self.L, self.world, self.pad_rows = lib, L, world, pad_rows
-        self.ncols = [nc for nc, _ in tables]
-        self.cap = [int(cap) for _, cap in tables]
-        self.reg_off = []
+        self.ncols = [t[0] for t in tables]
+        self.cap = [int(t[1]) for t in tables]
+        # words per wire column: cap, unless the table lists its own (nc, cap, [words per wire column]) — the broadcast's
+        # offsets, cells and bitmap words; every column is followed by pad_rows words
+        self.col_off, self.stride, self.reg_off = [], [], []
+        for t, cap in zip(tables, self.cap):
+            words = [int(x) for x in t[2]] if len(t) > 2 else [cap] * t[0]
+            self.col_off.append([sum(words[:c]) + c * pad_rows for c in range(len(words))])
+            self.stride.append(sum(words) + len(words) * pad_rows)
         off = _round_up(len(tables) * world * 16, 4096)
-        for nc, cap in zip(self.ncols, self.cap):
+        for stride in self.stride:
             self.reg_off.append(off)
-            off += world * nc * (cap + pad_rows) * 8
+            off += world * stride * 8
         self.bytes = _round_up(off, 4096)
         self.bases = []
 
     def region_ptr(self, dst, t, src, c):
-        return self.bases[dst] + self.reg_off[t] + ((src * self.ncols[t] + c) * (self.cap[t] + self.pad_rows)) * 8
+        return self.bases[dst] + self.reg_off[t] + (src * self.stride[t] + self.col_off[t][c]) * 8
 
     def slot_ptr(self, dst, t, src):
         return self.bases[dst] + (t * self.world + src) * 16
@@ -194,7 +206,7 @@ class RegionExchange(RegionLayout):
     and no NCCL call sits between the exchange and the join."""
 
     def __init__(self, lib, L, world, rank, tables, align_rows=4096):
-        super().__init__(lib, L, world, [(nc, _round_up(cap, align_rows)) for nc, cap in tables])
+        super().__init__(lib, L, world, [(t[0], _round_up(t[1], align_rows)) + tuple(t[2:]) for t in tables])
         self.rank = rank
         p = C.c_void_p()
         L.check(lib.tq_device_alloc(self.bytes, C.byref(p)))
@@ -621,6 +633,238 @@ class RegionJoin:
         self.L.check(self.lib.tq_region_gather(layout.world, slots, layout.cap[t], layout.ncols[t] - has_mask, has_mask, layout.region_table(dst, t),
                                                target[0], target[1], C.byref(n)))
         return n.value
+
+
+class VarCol:
+    """a var-len device column that is just (cells pointer, offsets pointer, rows): offsets = rows + 1 int64, offsets[0] may be
+    non-zero"""
+
+    def __init__(self, data, offsets, n):
+        self.data, self.offsets, self.n = data, offsets, n
+
+    def tq(self, length=None):
+        from . import _lib
+        t = _lib.TQColumn()
+        t.length, t.data, t.offsets = self.n if length is None else length, self.data, self.offsets
+        return t
+
+
+def _tq_device(L, cols, bitmaps=None):
+    """(TQColumn array, rows) of device columns: objects with .tq() (DeviceColumn, DeviceVarColumn, VarCol) or (pointer,
+    rows)-like ones; bitmaps, when given, replace the columns' own (a device NULL bitmap pointer or None per column)"""
+    arr = (L.TQColumn * len(cols))()
+    for c, x in enumerate(cols):
+        if hasattr(x, "tq"):
+            arr[c] = x.tq()
+        else:
+            arr[c].length, arr[c].data = int(x.numel()), x.data_ptr()
+    n = int(arr[0].length) if len(cols) else 0
+    for c in range(len(cols)):
+        arr[c].length = n
+    for c, b in enumerate(bitmaps or []):
+        arr[c].null_bitmap = b
+    return arr, n
+
+
+class BroadcastJoin:
+    """The multi-GPU join that replicates the build side: every rank pushes its build shard to every rank, this one
+    included (tq_partition_push_broadcast), and joins its own probe shard, which never moves, against all W build shards.
+    One step:
+
+        push stream    broadcast(build shard)
+        compute stream create handle + conditions | tq_region_wait (W slots) | one host read of the slots |
+                       tq_join_put_build(region of source g) for g = 0..W-1 | finalize | put_probe(local shard) | eof | drain
+
+    then one barrier (nobody may overwrite a region a peer is still building from).  The build side is the inner child, so
+    the side an outer join preserves is the probe side: joining each probe shard against the whole build side is correct for
+    inner, left outer and right outer joins, keyed or key-less, and every probe row's output appears on exactly one rank.  A
+    key-less join puts the build regions in source order, so rank r's output is the single-GPU sequence of its probe shard
+    against the rank-major concatenation of the build shards, and the ranks' outputs in rank order are the whole job's.
+
+    Everything the single-GPU handle takes comes with it: 0..8 key columns of any 8-byte or var-len type, BYTES payloads,
+    nullable columns, selected[], defaultInner and OtherConditions as comparisons or as a program.
+
+    When to use which join: RegionJoin (the hash shuffle) moves (W-1)/W of both sides over NVLink and holds about 1/W of
+    each per rank, but runs one 8-byte NOT NULL-or-masked key in column 0 over at most 4 words per row with no
+    OtherConditions.  BroadcastJoin moves (W-1) x the build side over NVLink and holds W x the build side per rank, and runs
+    every join the single-GPU handle runs: key-less joins, multi-column and string keys, wide rows, conditions.  It suits a
+    small build side (a dimension table) or a join the shuffle cannot route; a build side that does not fit one GPU does not
+    fit it."""
+
+    def __init__(self, lib, L, world, rank, n_build_max, build_types, probe_types, build_keys=(), probe_keys=(), join_type=0,
+                 outer_is_right=True, byte_caps=None, build_nullable=False, probe_nullable=False, default_inner=None,
+                 other_conditions=(), other_program=(), slot=0, exchange=None):
+        """n_build_max: the largest build shard; byte_caps: per build column, the most cell bytes a shard of a BYTES column
+        holds (None for the others) — every rank passes the same numbers, the layout is shared.  build_types / probe_types:
+        TQ_TYPE_INT64 / _UINT64 / _FLOAT64 / _BYTES.  build_keys / probe_keys: 0..8 column indices each (empty: key-less).
+        other_conditions / other_program: OtherConditions over the output row as HashJoinExec takes them.  exchange: a
+        RegionLayout with the attributes of a RegionExchange (rank, epoch) holding BroadcastJoin.table(...) as table 0; by
+        default a RegionExchange over the ranks of the process group."""
+        self.lib, self.L, self.world, self.rank, self.slot = lib, L, world, rank, slot
+        self.build_types, self.probe_types = list(build_types), list(probe_types)
+        self.build_keys, self.probe_keys = list(build_keys), list(probe_keys)
+        if len(self.build_keys) != len(self.probe_keys) or len(self.build_keys) > 8:
+            raise ValueError("BroadcastJoin: build_keys and probe_keys name the same number of columns, 0..8")
+        self.join_type, self.outer_is_right, self.default_inner = join_type, bool(outer_is_right), default_inner
+        self.nullable, self.probe_nullable = int(bool(build_nullable)), bool(probe_nullable)
+        self.other_conditions, self.other_program = list(other_conditions), list(other_program)
+        self.byte_caps = [int((byte_caps or [None] * len(self.build_types))[c] or 0) for c in range(len(self.build_types))]
+        self.table = BroadcastJoin.table_of(self.build_types, n_build_max, self.byte_caps, self.nullable)
+        self.rx = exchange if exchange is not None else RegionExchange(lib, L, world, rank, [self.table], align_rows=1)
+        self.last_phase = {}
+
+    @staticmethod
+    def table_of(build_types, n_build_max, byte_caps, nullable):
+        """the broadcast's RegionLayout table (areas, cap rows, [words per area]): per column its values or offsets, a BYTES
+        column's cells, then on a nullable side its bitmap words (tq_partition_push_broadcast's order), each rounded up to
+        16 bytes so every area starts 16-byte aligned"""
+        from . import _lib
+        cap = _round_up(max(int(n_build_max), 1), 4096)
+        words = []
+        for t, bc in zip(build_types, byte_caps):
+            bytes_col = t == _lib.TQ_TYPE_BYTES
+            words.append(_round_up(cap + (1 if bytes_col else 0), 2))
+            if bytes_col:
+                words.append(_round_up(max(int(bc or 0), 1), 16) // 8)
+            if nullable:
+                words.append(_round_up((cap + 63) // 64, 2))
+        return (len(words), cap, words)
+
+    def close(self):
+        self.rx.close()
+
+    def _areas(self, g, rows):
+        """source g's build region on this rank as tq_column chunk of `rows` rows"""
+        rx, L = self.rx, self.L
+        arr = (L.TQColumn * len(self.build_types))()
+        a = 0
+        for c, t in enumerate(self.build_types):
+            arr[c].length = rows
+            if t == L.TQ_TYPE_BYTES:
+                arr[c].offsets = rx.region_ptr(rx.rank, 0, g, a)
+                arr[c].data = rx.region_ptr(rx.rank, 0, g, a + 1)
+                a += 2
+            else:
+                arr[c].data = rx.region_ptr(rx.rank, 0, g, a)
+                a += 1
+            if self.nullable:
+                arr[c].null_bitmap = rx.region_ptr(rx.rank, 0, g, a)
+                a += 1
+        return arr
+
+    def push(self, build, build_bitmaps=None):
+        """enqueue the broadcast of this rank's build shard (push stream) for the exchange's current epoch"""
+        L, rx = self.L, self.rx
+        arr, n = _tq_device(L, build, build_bitmaps)
+        if build_bitmaps and not self.nullable:
+            raise ValueError("BroadcastJoin: NULL bitmaps on the build side need build_nullable")
+        types = (C.c_int32 * len(self.build_types))(*self.build_types)
+        caps = (C.c_int64 * len(self.byte_caps))(*self.byte_caps)
+        dest, cnts = rx.push_tables(0, rx.rank)
+        L.check(self.lib.tq_partition_push_broadcast(len(self.build_types), arr, types, self.nullable, n, self.world, dest, cnts, rx.cap[0], caps,
+                                                     self.slot, rx.epoch))
+
+    def _create(self):
+        L, lib = self.L, self.lib
+        tb = (C.c_int32 * len(self.build_types))(*self.build_types)
+        tp = (C.c_int32 * len(self.probe_types))(*self.probe_types)
+        nk = len(self.build_keys)
+        bk, pk = (C.c_int32 * max(nk, 1))(*self.build_keys), (C.c_int32 * max(nk, 1))(*self.probe_keys)
+        d = L.TQJoinDesc(self.join_type, 1 if self.outer_is_right else 0, len(tb), tb, len(tp), tp, nk, bk if nk else None, pk if nk else None, 0, 0)
+        keep = [tb, tp, bk, pk]
+        if self.default_inner is not None:
+            dt = {L.TQ_TYPE_INT64: np.int64, L.TQ_TYPE_UINT64: np.uint64, L.TQ_TYPE_FLOAT64: np.float64}
+            keep += [(C.c_uint64 * len(tb))(*[0 if v is None else int(np.array([v], dtype=dt[t]).view(np.uint64)[0])
+                                              for v, t in zip(self.default_inner, self.build_types)]),
+                     (C.c_uint8 * len(tb))(*[0 if v is None else 1 for v in self.default_inner])]
+            d.default_inner_bits, d.default_inner_not_null = keep[-2], keep[-1]
+        h = C.c_void_p()
+        L.check(lib.tq_join_create(C.byref(d), C.byref(h)))
+        try:
+            if self.other_conditions:
+                arr = (L.TQJoinCond * len(self.other_conditions))()
+                for i, c in enumerate(self.other_conditions):
+                    if c[2] is None:
+                        np_t = {L.TQ_TYPE_INT64: np.int64, L.TQ_TYPE_UINT64: np.uint64, L.TQ_TYPE_FLOAT64: np.float64}[c[3]]
+                        arr[i] = L.TQJoinCond(c[0], c[1], -1, c[3], int(np.array([c[4]], dtype=np_t).view(np.uint64)[0]))
+                    else:
+                        arr[i] = L.TQJoinCond(c[0], c[1], c[2], 0, 0)
+                L.check(lib.tq_join_set_other_conditions(h, len(arr), arr))
+            if self.other_program:
+                from .expression import JoinProgram
+                JoinProgram(self.other_program).set_on(lib.tq_join_set_other_program, h)
+        except Exception:
+            lib.tq_join_destroy(h)
+            raise
+        return h
+
+    def join(self, probe, probe_bitmaps=None, selected=None, keep_result=False):
+        """this rank's half of a step after every rank's push was enqueued: wait for the W build regions, build, probe the
+        local shard, drain.  Returns (rows, stats, result); result (keep_result) = host Columns of the output"""
+        lib, L, rx, w = self.lib, self.L, self.rx, self.world
+        if probe_bitmaps and not self.probe_nullable:
+            raise ValueError("BroadcastJoin: NULL bitmaps on the probe side need probe_nullable")
+        phase, t0 = {}, time.perf_counter()
+
+        def mark(name):
+            nonlocal t0
+            t1 = time.perf_counter()
+            phase[name] = (t1 - t0) * 1e3
+            t0 = t1
+        out_types = (self.build_types + self.probe_types) if self.outer_is_right else (self.probe_types + self.build_types)
+        h = self._create()
+        total, chunks, st = 0, [], (C.c_int64 * 8)()
+        try:
+            rx.wait(0)
+            cnt = rx.counts(rx.rank, 0, 1)[0]     # one host read (put_build takes host lengths); ~0 = an overflowed push: raises
+            for g in range(w):
+                if cnt[g]:
+                    L.check(lib.tq_join_put_build(h, self._areas(g, cnt[g]), L.TQ_MEM_DEVICE))
+            L.check(lib.tq_compute_synchronize())
+            mark("wait + build puts")
+            L.check(lib.tq_join_finalize_build(h))
+            L.check(lib.tq_compute_synchronize())
+            mark("finalize")
+            arr, n = _tq_device(L, probe, probe_bitmaps)
+            sel = None if selected is None else np.ascontiguousarray(selected, np.uint8)
+            if n:
+                L.check(lib.tq_join_put_probe(h, arr, None if sel is None else sel.ctypes.data, L.TQ_MEM_DEVICE))
+            L.check(lib.tq_join_probe_eof(h))
+            out = (L.TQColumn * len(out_types))()
+            rows, eof = C.c_int64(0), C.c_int32(0)
+            while True:
+                L.check(lib.tq_join_next_device(h, out, C.byref(rows), C.byref(eof)))
+                if rows.value == 0:
+                    break
+                total += rows.value
+                if keep_result:
+                    from .chunk import device_to_host, device_var_to_host
+                    chunks.append([device_var_to_host(out[c].data, out[c].offsets, out[c].null_bitmap, rows.value) if t == L.TQ_TYPE_BYTES
+                                   else device_to_host(t, out[c].data, out[c].null_bitmap, rows.value) for c, t in enumerate(out_types)])
+            L.check(lib.tq_compute_synchronize())
+            mark("probe + drain")
+            lib.tq_join_stats(h, st)
+        finally:
+            lib.tq_join_destroy(h)
+        result = None
+        if keep_result:
+            from .chunk import Chunk, Column, VarColumn
+            result = (Chunk.concat([Chunk(ch) for ch in chunks], out_types).cols if chunks
+                      else [(VarColumn if t == L.TQ_TYPE_BYTES else Column).empty(t, 0) for t in out_types])
+        self.last_phase = phase
+        return total, list(st), result
+
+    def step_cols(self, build, probe, build_bitmaps=None, probe_bitmaps=None, selected=None, keep_result=False):
+        """build / probe: this rank's shard of every column (device columns: (pointer, rows)-like objects, or VarCol /
+        DeviceVarColumn for BYTES).  *_bitmaps: a device NULL bitmap pointer (or None) per column, on a side declared
+        nullable.  selected: HOST bytes or bools, one per probe row (the outer-side filter), or None.  Returns (rows, stats,
+        result) as RegionJoin.step_cols, result as host Columns."""
+        self.rx.next_epoch()
+        self.push(build, build_bitmaps)
+        res = self.join(probe, probe_bitmaps, selected, keep_result)
+        self.L.check(self.lib.tq_partition_push_sync(self.slot))   # the push reads the caller's build shard until it is done
+        dist.barrier()
+        return res
 
 
 def agg_drain(lib, L, h, n_funcs):
