@@ -504,6 +504,27 @@ int32_t tq_agg_merge_partial(tq_agg *a, const tq_column *cols, int32_t mem);
 int32_t tq_agg_push_partial(tq_agg *a, int32_t n_parts, void *const *dest_data, void *const *dest_counts, int64_t region_cap,
                             int32_t slot, uint64_t epoch);
 int32_t tq_agg_merge_regions(tq_agg *a, int32_t n_regions, const void *slots, int64_t region_cap, const tq_column *regions);
+/* The same pair for handles with var-len (string) partial columns; on a handle without them both behave exactly as the pair
+ * above, wire format included.  A partial column is var-len when it is a GROUP BY item on a BYTES input column or the state
+ * of MAX / MIN / FIRSTROW over a BYTES argument; V = their number (at most 16).  Per source region the wire areas are:
+ *   0 .. w - 1   the partial columns as above, except that a var-len column's area holds region_cap + 1 int64 OFFSETS:
+ *                entry 0 = 0, entry i + 1 = the end of row i's cell in that column's byte area (a NULL cell is empty and its
+ *                mask bit is 0)
+ *   w            the NULL mask word
+ *   w + 1 + v    byte area v of byte_cap[v] bytes: the cells of the v-th var-len column (partial-column order), in row order
+ * tq_agg_push_partial_var: dest_data[q * (w + 1 + V) + a] = this rank's area a on rank q; byte_cap: V entries,
+ * 1 <= byte_cap[v] < 2^32 (may be NULL when V = 0).  A string GROUP BY item routes by the 64-bit content hash of its bytes
+ * (the one its string dictionary keeps), the same on every rank, so the empty string and NULL are different groups; 8-byte
+ * items route as above.  Rows keep the handle's partial-row order in every region, and each cell is copied from the handle's
+ * dictionary.  A region past region_cap rows or a byte area past byte_cap makes every slot read ~0; nothing is written past
+ * either cap.  No host synchronisation beyond the group-count read.
+ * tq_agg_merge_regions_var: regions[g * (w + 1) + c]; a var-len column c has .offsets = its offsets area and .data = its
+ * byte area, every other column .data only.  Each var-len column is encoded into this handle's dictionary of the input
+ * column it came from (GROUP BY s and MAX(s) share one), then merged as tq_agg_merge_regions does.  Refusals as above, less
+ * the var-len one; a var-len column without offsets is TQ_ERR_INVALID_ARG. */
+int32_t tq_agg_push_partial_var(tq_agg *a, int32_t n_parts, void *const *dest_data, void *const *dest_counts, int64_t region_cap,
+                                const int64_t *byte_cap, int32_t slot, uint64_t epoch);
+int32_t tq_agg_merge_regions_var(tq_agg *a, int32_t n_regions, const void *slots, int64_t region_cap, const tq_column *regions);
 
 /* FinalMode HashAgg over pushed-down partial results (SURVEY §8 f4).  The planner splits an aggregation into a Partial1
  * half that runs inside the coprocessor (planner/core/task.go:564-625, store/mockstore/mocktikv/aggregate.go:81-124: each row

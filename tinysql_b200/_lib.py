@@ -127,6 +127,8 @@ SYMBOLS = {
     "tq_agg_merge_partial": (_I32, [_P, _COL, _I32]),
     "tq_agg_push_partial": (_I32, [_P, _I32, C.POINTER(_P), C.POINTER(_P), _I64, _I32, C.c_uint64]),
     "tq_agg_merge_regions": (_I32, [_P, _I32, _P, _I64, _COL]),
+    "tq_agg_push_partial_var": (_I32, [_P, _I32, C.POINTER(_P), C.POINTER(_P), _I64, C.POINTER(_I64), _I32, C.c_uint64]),
+    "tq_agg_merge_regions_var": (_I32, [_P, _I32, _P, _I64, _COL]),
     "tq_sort_create": (_I32, [C.POINTER(TQSortDesc), C.POINTER(_P)]),
     "tq_sort_put": (_I32, [_P, _COL, _I32]), "tq_sort_eof": (_I32, [_P]),
     "tq_sort_next_bytes": (_I32, [_P, _I64, C.POINTER(_I64)]),

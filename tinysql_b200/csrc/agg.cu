@@ -590,6 +590,7 @@ struct tq_agg {
   DevBuf pre_lo, pre_hi, pre_lim, pre_meta;
   cudaEvent_t ev_pa = nullptr, ev_pb = nullptr;
   std::vector<DevBuf> region_bm;   // tq_agg_merge_regions: the NOT-NULL bitmaps expanded from a region's mask words
+  std::vector<DevBuf> region_ids;  // tq_agg_merge_regions_var: a region's var-len partial columns as ids of this handle's dictionaries
   PinBuf region_slots;
   tq_agg_func funcs[AGG_MAXF];
   int arg_type[AGG_MAXF];
@@ -1117,6 +1118,21 @@ static int partial_width(const tq_agg *a) {
   return w;
 }
 
+// The var-len partial columns: src[c] = the input column whose dictionary partial column c's ids belong to (a GROUP BY item
+// on a BYTES column; the state of MAX / MIN / FIRSTROW over a BYTES argument), -1 for an 8-byte column.  Returns their number.
+static int partial_var_src(const tq_agg *a, int *src) {
+  int c = 0, n_var = 0;
+  auto put = [&](int in) { src[c++] = in; n_var += in >= 0; };
+  for (int g = 0; g < a->n_group_by; g++) put(a->in_kind[a->gb_cols[g]] == 2 ? a->gb_cols[g] : -1);
+  for (int i = 0; i < a->n_funcs; i++) {
+    const int fn = a->funcs[i].func, ac = a->funcs[i].arg_col;
+    const bool sel = fn == TQ_AGG_MAX || fn == TQ_AGG_MIN || fn == TQ_AGG_FIRSTROW;
+    put(sel && ac >= 0 && a->in_kind[ac] == 2 ? ac : -1);
+    if (fn == TQ_AGG_AVG && !a->key_passthrough[i]) put(-1);
+  }
+  return n_var;
+}
+
 }  // namespace tq
 
 extern "C" {
@@ -1510,20 +1526,26 @@ int32_t tq_agg_export_partial(tq_agg *a, tq_column *out_cols, int64_t *n_rows) {
   return TQ_OK;
 }
 
-// The GROUP BY push: every argument is checked before anything is enqueued (a refused push writes no region and publishes no
-// slot); then the export (one host read of the group count, on the compute stream, which it also drains), and on the push
-// stream the destination of every partial row, the scatter into the regions and k_publish_counts.
-int32_t tq_agg_push_partial(tq_agg *a, int32_t n_parts, void *const *dest_data, void *const *dest_counts, int64_t region_cap, int32_t slot,
-                            uint64_t epoch) {
+// The GROUP BY push (both entry points): every argument is checked before anything is enqueued (a refused push writes no
+// region and publishes no slot); then the export (one host read of the group count, on the compute stream, which it also
+// drains), and on the push stream the destination of every partial row, the scatter into the regions and k_publish_counts.
+// var_ok: the handle may have var-len partial columns, whose cells travel in byte areas of byte_cap[v] bytes.
+static int32_t agg_push_body(tq_agg *a, const char *fn, bool var_ok, int32_t n_parts, void *const *dest_data, void *const *dest_counts,
+                             int64_t region_cap, const int64_t *byte_cap, int32_t slot, uint64_t epoch) {
   if (!a) return TQ_ERR_INVALID_ARG;
   TQ_TRY(ensure_init());
-  const char *fn = "tq_agg_push_partial";
   if (a->final_mode) { set_error("%s: a FinalMode handle takes partial rows, it does not make them", fn); return TQ_ERR_STATE; }
   if (a->merge_mode_seen) { set_error("%s: the handle has merged partial rows; push from a handle fed raw rows", fn); return TQ_ERR_STATE; }
-  if (agg_has_varlen(a)) { set_error("partial export / merge with var-len columns is not supported"); return TQ_ERR_UNSUPPORTED_TYPE; }
+  if (!var_ok && agg_has_varlen(a)) { set_error("partial export / merge with var-len columns is not supported"); return TQ_ERR_UNSUPPORTED_TYPE; }
   const int w = partial_width(a), nw = w + 1;
   if (nw > 64) { set_error("%s: %d partial columns and the mask word exceed 64 words per row", fn, w); return TQ_ERR_INVALID_ARG; }
-  TQ_TRY(push_check_dests(fn, n_parts, nw, dest_data, dest_counts, region_cap, slot));
+  int src[64];
+  const int n_var = partial_var_src(a, src);
+  if (n_var > REGION_MAXV) { set_error("%s: %d var-len partial columns, at most %d", fn, n_var, REGION_MAXV); return TQ_ERR_INVALID_ARG; }
+  if (n_var && !byte_cap) { set_error("%s: %d var-len partial columns need byte_cap", fn, n_var); return TQ_ERR_INVALID_ARG; }
+  for (int v = 0; v < n_var; v++)
+    if (byte_cap[v] < 1 || byte_cap[v] > 0xFFFFFFF0ll) { set_error("%s: byte_cap[%d] = %lld: 1 <= byte_cap < 2^32", fn, v, (long long)byte_cap[v]); return TQ_ERR_INVALID_ARG; }
+  TQ_TRY(push_check_dests(fn, n_parts, nw + n_var, dest_data, dest_counts, region_cap, slot));
   Runtime &r = rt();
   std::lock_guard<std::recursive_mutex> lk(r.mu);
   if (!a->eof) TQ_TRY(tq_agg_eof(a));
@@ -1534,7 +1556,7 @@ int32_t tq_agg_push_partial(tq_agg *a, int32_t n_parts, void *const *dest_data, 
   PushSlot *ps = nullptr;
   TQ_TRY(push_begin(slot, n_parts, dest_counts, nullptr, s, &ps));
   if (n > 0) {
-    const size_t tab = (size_t)n_parts * nw * 8;
+    const size_t tab = (size_t)n_parts * (nw + n_var) * 8;
     TQ_TRY(ps->out_ptrs.reserve(tab));
     TQ_TRY(ps->h_out_ptrs.reserve(tab));
     TQ_TRY(ps->dest.reserve((size_t)n));
@@ -1543,23 +1565,34 @@ int32_t tq_agg_push_partial(tq_agg *a, int32_t n_parts, void *const *dest_data, 
     DCol cols[64];
     for (int c = 0; c < w; c++) cols[c] = DCol{a->result.data[c].as<uint64_t>(), a->result.bm[c].as<uint32_t>()};
     uint32_t real_mask = 0;
-    for (int g = 0; g < a->n_group_by; g++)
+    const uint64_t *hashes[GROUP_MAX_ITEMS] = {};
+    for (int g = 0; g < a->n_group_by; g++) {
       if (a->types[a->gb_cols[g]] == TQ_TYPE_FLOAT64) real_mask |= 1u << g;
-    TQ_TRY(group_dest(cols, a->n_group_by, real_mask, n, n_parts, ps->dest.as<uint8_t>(), s));
-    TQ_TRY(scatter_to_regions(cols, w, ps->dest.as<uint8_t>(), n, n_parts, ps->out_ptrs.as<uint64_t *>(), region_cap, ps->cursor.as<uint32_t>(),
-                              ps->ovf.as<unsigned long long>(), ps->region, s));
+      if (src[g] >= 0) hashes[g] = a->sd[src[g]].a_hash.as<uint64_t>();   // a string item routes by its content hash
+    }
+    RegionVar var[REGION_MAXV];
+    for (int c = 0, v = 0; c < w; c++) {
+      if (src[c] < 0) continue;
+      const StringDict &sd = a->sd[src[c]];
+      var[v] = RegionVar{c, sd.arena.offsets.as<int64_t>(), sd.arena.bytes.as<uint8_t>(), (uint64_t)byte_cap[v]};
+      v++;
+    }
+    TQ_TRY(group_dest(cols, hashes, a->n_group_by, real_mask, n, n_parts, ps->dest.as<uint8_t>(), s));
+    TQ_TRY(scatter_to_regions_var(cols, w, var, n_var, ps->dest.as<uint8_t>(), n, n_parts, ps->out_ptrs.as<uint64_t *>(), region_cap,
+                                  ps->cursor.as<uint32_t>(), ps->ovf.as<unsigned long long>(), ps->region, s));
   }
   return push_publish(*ps, n_parts, epoch, s);
 }
 
-// The GROUP BY receive: one host read of the slots (queued behind tq_region_wait on the compute stream), then each region's
-// rows straight into the merge update, with the mask words expanded into NOT-NULL bitmaps first.
-int32_t tq_agg_merge_regions(tq_agg *a, int32_t n_regions, const void *slots, int64_t region_cap, const tq_column *regions) {
+// The GROUP BY receive (both entry points): one host read of the slots (queued behind tq_region_wait on the compute stream),
+// then per region the mask words expanded into NOT-NULL bitmaps, every var-len partial column encoded into this handle's
+// dictionary of the input column it came from (one read of the region's byte total each), and the rows merged in place.
+static int32_t agg_merge_body(tq_agg *a, const char *fn, bool var_ok, int32_t n_regions, const void *slots, int64_t region_cap,
+                              const tq_column *regions) {
   if (!a) return TQ_ERR_INVALID_ARG;
   TQ_TRY(ensure_init());
-  const char *fn = "tq_agg_merge_regions";
   if (a->final_mode) { set_error("a FinalMode handle takes its partial rows through tq_agg_put"); return TQ_ERR_STATE; }
-  if (agg_has_varlen(a)) { set_error("partial export / merge with var-len columns is not supported"); return TQ_ERR_UNSUPPORTED_TYPE; }
+  if (!var_ok && agg_has_varlen(a)) { set_error("partial export / merge with var-len columns is not supported"); return TQ_ERR_UNSUPPORTED_TYPE; }
   if (a->eof) { set_error("put after eof"); return TQ_ERR_STATE; }
   if (a->raw_mode_seen) { set_error("one handle cannot mix raw rows and partial rows"); return TQ_ERR_STATE; }
   const int w = partial_width(a), nw = w + 1;
@@ -1568,8 +1601,12 @@ int32_t tq_agg_merge_regions(tq_agg *a, int32_t n_regions, const void *slots, in
     set_error("%s: 1..8 regions with their slots, 1 <= region_cap < 2^32", fn);
     return TQ_ERR_INVALID_ARG;
   }
-  for (int k = 0; k < n_regions * nw; k++)
+  int src[64];
+  partial_var_src(a, src);
+  for (int k = 0; k < n_regions * nw; k++) {
     if (!regions[k].data) { set_error("%s: region %d has no data for wire column %d", fn, k / nw, k % nw); return TQ_ERR_INVALID_ARG; }
+    if (k % nw < w && src[k % nw] >= 0 && !regions[k].offsets) { set_error("%s: region %d has no offsets for var-len column %d", fn, k / nw, k % nw); return TQ_ERR_INVALID_ARG; }
+  }
   Runtime &r = rt();
   std::lock_guard<std::recursive_mutex> lk(r.mu);
   cudaStream_t s = r.compute;
@@ -1590,6 +1627,7 @@ int32_t tq_agg_merge_regions(tq_agg *a, int32_t n_regions, const void *slots, in
   if (most == 0) return TQ_OK;
   TQ_TRY(agg_flush_stage(a, true, w));
   if ((int)a->region_bm.size() < w) a->region_bm.resize(w);
+  if ((int)a->region_ids.size() < w) a->region_ids.resize(w);
   for (int c = 0; c < w; c++) TQ_TRY(a->region_bm[c].reserve(bitmap_alloc_bytes(most)));
   std::vector<uint32_t *> bm(w);
   for (int c = 0; c < w; c++) bm[c] = a->region_bm[c].as<uint32_t>();
@@ -1598,11 +1636,42 @@ int32_t tq_agg_merge_regions(tq_agg *a, int32_t n_regions, const void *slots, in
     if (rows[g] == 0) continue;
     const tq_column *reg = regions + (size_t)g * nw;
     TQ_TRY(expand_null_mask((const uint64_t *)reg[w].data, rows[g], w, bm.data(), s));
-    for (int c = 0; c < w; c++) view[c] = DCol{(const uint64_t *)reg[c].data, a->region_bm[c].as<uint32_t>()};
+    for (int c = 0; c < w; c++) {
+      view[c] = DCol{(const uint64_t *)reg[c].data, a->region_bm[c].as<uint32_t>()};
+      if (src[c] < 0) continue;
+      // the region's cells as a device var-len column, as tq_agg_put(TQ_MEM_DEVICE) takes one (offsets from 0)
+      int64_t b0 = 0, b1 = 0;
+      TQ_TRY(device_cell_span(reg[c].offsets, rows[g], &b0, &b1, s));
+      StrView v;
+      v.off = reg[c].offsets;
+      v.base = 0;
+      v.bytes = reg[c].data;
+      TQ_TRY(a->region_ids[c].reserve((size_t)rows[g] * 8));
+      TQ_TRY(a->sd[src[c]].encode(v, bm[c], rows[g], b1 - b0, /*insert=*/true, a->region_ids[c].as<uint64_t>(), nullptr, s));
+      view[c].data = a->region_ids[c].as<uint64_t>();
+    }
     a->rows_total += rows[g];
     TQ_TRY(agg_update_device(a, view.data(), w, rows[g], true));   // in stream order after the expansion; it synchronises
   }
   return TQ_OK;
+}
+
+int32_t tq_agg_push_partial(tq_agg *a, int32_t n_parts, void *const *dest_data, void *const *dest_counts, int64_t region_cap, int32_t slot,
+                            uint64_t epoch) {
+  return agg_push_body(a, "tq_agg_push_partial", false, n_parts, dest_data, dest_counts, region_cap, nullptr, slot, epoch);
+}
+
+int32_t tq_agg_push_partial_var(tq_agg *a, int32_t n_parts, void *const *dest_data, void *const *dest_counts, int64_t region_cap,
+                                const int64_t *byte_cap, int32_t slot, uint64_t epoch) {
+  return agg_push_body(a, "tq_agg_push_partial_var", true, n_parts, dest_data, dest_counts, region_cap, byte_cap, slot, epoch);
+}
+
+int32_t tq_agg_merge_regions(tq_agg *a, int32_t n_regions, const void *slots, int64_t region_cap, const tq_column *regions) {
+  return agg_merge_body(a, "tq_agg_merge_regions", false, n_regions, slots, region_cap, regions);
+}
+
+int32_t tq_agg_merge_regions_var(tq_agg *a, int32_t n_regions, const void *slots, int64_t region_cap, const tq_column *regions) {
+  return agg_merge_body(a, "tq_agg_merge_regions_var", true, n_regions, slots, region_cap, regions);
 }
 
 int32_t tq_agg_stats(tq_agg *a, int64_t *s) {

@@ -54,20 +54,34 @@ struct RegionParams {
   uint32_t *counts;
   DCol in[REGION_MAXW];
   const uint8_t *dest;
-  uint64_t *const *out;  // DEVICE table: out[q * (n_cols + 1) + c] = destination q's region of wire column c, the mask word last
+  uint64_t *const *out;  // DEVICE table: out[q * n_areas + a] = destination q's area a: wire columns, the mask word, byte areas
   uint32_t cap;          // rows per region: a row at or past it is not written (the push publishes ~0)
+  int n_areas;           // n_cols + 1 + n_var
+  // var-len wire columns (scatter_to_regions_var): their words are not copied, k_region_scatter_var writes offsets and cells
+  int n_var;
+  uint64_t var_mask;     // bit c: wire column c is var-len
+  RegionVar var[REGION_MAXV];
+  uint32_t *bcounts;     // [(v * n_parts + q) * n_chunks + chunk] cell bytes, scanned in place
+  unsigned long long *btotal;  // [v * n_parts + q] cell bytes of the region, exact
 
   __device__ __forceinline__ int dest_of(int64_t r) const { return dest[r]; }
   __device__ __forceinline__ uint32_t run_base(int q) const { return counts[(int64_t)q * n_chunks]; }
   __device__ __forceinline__ void store(int64_t r, int q, uint32_t pos) const {
     if (pos >= cap) return;
-    uint64_t *const *o = out + (int64_t)q * (n_cols + 1);
+    uint64_t *const *o = out + (int64_t)q * n_areas;
     uint64_t m = 0;
     for (int c = 0; c < n_cols; c++) {
-      o[c][pos] = in[c].data[r];
+      if (!((var_mask >> c) & 1)) o[c][pos] = in[c].data[r];
       m |= (uint64_t)tqd::bm_not_null(in[c].bm, r) << c;
     }
     o[n_cols][pos] = m;
+  }
+  // bytes of row r's cell in var-len column v (0 for NULL)
+  __device__ __forceinline__ uint64_t cell_len(int v, int64_t r) const {
+    const DCol &c = in[var[v].col];
+    if (!tqd::bm_not_null(c.bm, r)) return 0;
+    const uint64_t id = c.data[r];
+    return (uint64_t)(var[v].off[id + 1] - var[v].off[id]);
   }
 };
 
@@ -215,6 +229,7 @@ struct GroupDestParams {
   int n_items, n_parts;
   uint32_t real_mask;  // bit g: item g is REAL
   DCol item[GROUP_MAX_ITEMS];
+  const uint64_t *hash[GROUP_MAX_ITEMS];  // var-len item: the content hash of each dictionary id
   int64_t n;
   uint8_t *dest;
 };
@@ -226,7 +241,8 @@ __global__ void __launch_bounds__(256) k_group_dest(const GroupDestParams p) {
       uint64_t v = GROUP_NULL_WORD;
       if (tqd::bm_not_null(p.item[g].bm, r)) {
         v = p.item[g].data[r];
-        if (((p.real_mask >> g) & 1) && v == 0x8000000000000000ull) v = 0;  // -0.0 and +0.0 are one group
+        if (p.hash[g]) v = p.hash[g][v];                                      // a string id: its content hash
+        else if (((p.real_mask >> g) & 1) && v == 0x8000000000000000ull) v = 0;  // -0.0 and +0.0 are one group
       }
       h = tqd::mix64(h ^ v);
     }
@@ -235,12 +251,20 @@ __global__ void __launch_bounds__(256) k_group_dest(const GroupDestParams p) {
 }
 
 int32_t group_dest(const DCol *items, int n_items, uint32_t real_mask, int64_t n, int n_parts, uint8_t *dest, cudaStream_t s) {
+  return group_dest(items, nullptr, n_items, real_mask, n, n_parts, dest, s);
+}
+
+int32_t group_dest(const DCol *items, const uint64_t *const *hashes, int n_items, uint32_t real_mask, int64_t n, int n_parts, uint8_t *dest,
+                   cudaStream_t s) {
   if (n_items < 0 || n_items > GROUP_MAX_ITEMS || n_parts < 1 || n_parts > 8 || n < 1) { set_error("internal: group_dest arguments"); return TQ_ERR_INVALID_ARG; }
   GroupDestParams p{};
   p.n_items = n_items;
   p.n_parts = n_parts;
   p.real_mask = real_mask;
-  for (int g = 0; g < n_items; g++) p.item[g] = items[g];
+  for (int g = 0; g < n_items; g++) {
+    p.item[g] = items[g];
+    p.hash[g] = hashes ? hashes[g] : nullptr;
+  }
   p.n = n;
   p.dest = dest;
   const int64_t blocks = (n + 255) / 256, cap = (int64_t)rt().sm_count * 8;
@@ -264,32 +288,7 @@ __global__ void k_region_rows(const uint32_t *scanned, int64_t n_chunks, int n_p
 
 int32_t scatter_to_regions(const DCol *cols, int n_cols, const uint8_t *dest, int64_t n, int n_parts, uint64_t *const *out, int64_t cap,
                            uint32_t *rows, unsigned long long *overflow, RegionScratch &sc, cudaStream_t s) {
-  if (n_cols < 1 || n_cols > REGION_MAXW || n_parts < 1 || n_parts > 8 || n < 1 || n > 0xFFFFFFF0ll || cap < 1 || cap > 0xFFFFFFF0ll) {
-    set_error("internal: scatter_to_regions arguments");
-    return TQ_ERR_INVALID_ARG;
-  }
-  RegionParams p{};
-  p.n_cols = n_cols;
-  p.n_parts = n_parts;
-  p.n = n;
-  p.n_chunks = (n + PART_CHUNK - 1) / PART_CHUNK;
-  for (int c = 0; c < n_cols; c++) p.in[c] = cols[c];
-  p.dest = dest;
-  p.out = out;
-  p.cap = (uint32_t)cap;
-  const int64_t n_counts = p.n_chunks * n_parts;
-  TQ_TRY(sc.hist.reserve((size_t)n_counts * 4));
-  TQ_TRY(sc.total.reserve(8));
-  p.counts = sc.hist.as<uint32_t>();
-  const unsigned blocks = (unsigned)((p.n_chunks + 7) / 8);
-  TQ_LAUNCH(k_part_hist<RegionParams>, blocks, 256, 0, s, p);
-  count_launch();
-  TQ_TRY(check_launch("k_part_hist(regions)"));
-  TQ_TRY(exclusive_scan_u32(p.counts, 1, p.counts, 1, n_counts, sc.total.as<uint64_t>(), sc.scan, s));
-  TQ_LAUNCH(k_region_rows, 1, 32, 0, s, p.counts, p.n_chunks, n_parts, sc.total.as<uint64_t>(), p.cap, rows, overflow);
-  TQ_LAUNCH(k_part_scatter<RegionParams>, blocks, 256, 0, s, p);
-  count_launch(2);
-  return check_launch("k_part_scatter(regions)");
+  return scatter_to_regions_var(cols, n_cols, nullptr, 0, dest, n, n_parts, out, cap, rows, overflow, sc, s);
 }
 
 struct ExpandParams {
@@ -377,27 +376,34 @@ __device__ __forceinline__ void bcast_words(const BcastParams &p, int c, int kin
   }
 }
 
-// The cells [off0, off0 + len) of a BYTES column to the start of each byte area.  Destination chunk i needs source bytes
-// [16 i, 16 i + 16): read as the aligned 8-byte words that hold them (each holds at least one of the column's bytes, so no read
-// leaves the cells' allocation), shifted into place.
+// Up to 16 bytes (cnt, 1..16) from s into x (bytes 0..7) and y (8..15), read as the aligned 8-byte words that hold them: each
+// holds at least one of the bytes, so no read leaves the bytes' allocation.
+__device__ __forceinline__ void load_chunk16(const uint8_t *s, uint64_t cnt, uint64_t &x, uint64_t &y) {
+  const unsigned a = (unsigned)((uintptr_t)s & 7);
+  const uint64_t *w = reinterpret_cast<const uint64_t *>(s - a);
+  const unsigned last = (unsigned)((a + cnt - 1) >> 3);
+  const uint64_t w0 = w[0], w1 = last >= 1 ? w[1] : 0, w2 = last >= 2 ? w[2] : 0;
+  x = a ? (w0 >> (8 * a)) | (w1 << (64 - 8 * a)) : w0;
+  y = a ? (w1 >> (8 * a)) | (w2 << (64 - 8 * a)) : w1;
+}
+
+// The cnt bytes of (x, y) to d: one 16-byte store where d is aligned and the chunk is whole, byte stores otherwise.
+__device__ __forceinline__ void store_chunk16(uint8_t *d, uint64_t cnt, uint64_t x, uint64_t y) {
+  if (cnt == 16 && ((uintptr_t)d & 15) == 0) {
+    bcast_store16(reinterpret_cast<uint64_t *>(d), x, y);
+  } else {
+    for (unsigned b = 0; b < cnt; b++) d[b] = (uint8_t)((b < 8 ? x >> (8 * b) : y >> (8 * (b - 8))) & 0xFF);
+  }
+}
+
+// The cells [off0, off0 + len) of a BYTES column to the start of each byte area: destination chunk i gets source bytes
+// [16 i, 16 i + 16).
 __device__ __forceinline__ void bcast_cells(const BcastParams &p, int c, const uint8_t *src, uint64_t len, int64_t t, int64_t stride) {
   for (uint64_t i = (uint64_t)t; 16 * i < len; i += (uint64_t)stride) {
     const uint64_t lo = 16 * i, cnt = len - lo < 16 ? len - lo : 16;
-    const uint8_t *s = src + lo;
-    const unsigned a = (unsigned)((uintptr_t)s & 7);
-    const uint64_t *w = reinterpret_cast<const uint64_t *>(s - a);
-    const unsigned last = (unsigned)((a + cnt - 1) >> 3);
-    const uint64_t w0 = w[0], w1 = last >= 1 ? w[1] : 0, w2 = last >= 2 ? w[2] : 0;
-    const uint64_t x = a ? (w0 >> (8 * a)) | (w1 << (64 - 8 * a)) : w0;
-    const uint64_t y = a ? (w1 >> (8 * a)) | (w2 << (64 - 8 * a)) : w1;
-    for (int q = 0; q < p.n_parts; q++) {
-      uint8_t *d = p.dst_cells[q][c] + lo;
-      if (cnt == 16 && ((uintptr_t)d & 15) == 0) {
-        bcast_store16(reinterpret_cast<uint64_t *>(d), x, y);
-      } else {
-        for (unsigned b = 0; b < cnt; b++) d[b] = (uint8_t)((b < 8 ? x >> (8 * b) : y >> (8 * (b - 8))) & 0xFF);
-      }
-    }
+    uint64_t x, y;
+    load_chunk16(src + lo, cnt, x, y);
+    for (int q = 0; q < p.n_parts; q++) store_chunk16(p.dst_cells[q][c] + lo, cnt, x, y);
   }
 }
 
@@ -456,6 +462,176 @@ int32_t broadcast_rows(int n_cols, const tq_column *cols, const int32_t *types, 
   TQ_LAUNCH(k_broadcast, (unsigned)(blocks < 1 ? 1 : (blocks < cap ? blocks : cap)), 256, 0, s, p);
   count_launch();
   return check_launch("k_broadcast");
+}
+
+// ---- the var-len wire columns of the GROUP BY push (scatter_to_regions_var): the cells follow their rows in the same stable
+// order, each region's byte positions from a per-(column, destination, chunk) byte count and its scan
+
+// One warp per chunk: the cell bytes each destination gets from it, per var-len column; also summed per region, exactly.
+__global__ void __launch_bounds__(256) k_region_var_hist(const RegionParams p) {
+  const int lane = threadIdx.x & 31;
+  const int64_t chunk = ((int64_t)blockIdx.x * blockDim.x + threadIdx.x) >> 5;
+  if (chunk >= p.n_chunks) return;
+  const int64_t lo = chunk * PART_CHUNK;
+  const int64_t hi = lo + PART_CHUNK < p.n ? lo + PART_CHUNK : p.n;
+  for (int v = 0; v < p.n_var; v++) {
+    uint64_t acc[8] = {0, 0, 0, 0, 0, 0, 0, 0};
+    for (int64_t r = lo + lane; r < hi; r += 32) {
+      const int q = p.dest[r];
+      const uint64_t len = p.cell_len(v, r);
+#pragma unroll
+      for (int k = 0; k < 8; k++) acc[k] += k == q ? len : 0;
+    }
+#pragma unroll
+    for (int q = 0; q < 8; q++) {
+      if (q >= p.n_parts) break;
+      uint64_t b = acc[q];
+#pragma unroll
+      for (int d = 16; d > 0; d >>= 1) b += __shfl_xor_sync(0xffffffffu, b, d);
+      if (lane == 0) {
+        // a chunk's count past 32 bits means a region past its byte cap (< 2^32): the push publishes ~0 and writes no cell
+        p.bcounts[((int64_t)v * p.n_parts + q) * p.n_chunks + chunk] = b > 0xFFFFFFFFull ? 0xFFFFFFFFu : (uint32_t)b;
+        if (b) atomicAdd(p.btotal + v * p.n_parts + q, (unsigned long long)b);
+      }
+    }
+  }
+}
+
+// After k_region_rows: a region past its byte cap sets the overflow; offsets entry 0 of every var-len area is 0.
+__global__ void k_region_bytes(const RegionParams p, unsigned long long *overflow) {
+  if (threadIdx.x != 0) return;
+  bool ovf = false;
+  for (int v = 0; v < p.n_var; v++)
+    for (int q = 0; q < p.n_parts; q++) {
+      ovf |= p.btotal[v * p.n_parts + q] > p.var[v].byte_cap;
+      p.out[(int64_t)q * p.n_areas + p.var[v].col][0] = 0;
+    }
+  if (ovf) *overflow = 1;
+}
+
+// k_part_scatter with var-len columns: the row's words and mask as RegionParams::store, then per var-len column the row's
+// byte position (the chunk's scanned base for its destination + the cells of the earlier rows of the same destination), its
+// offset, and its cell, copied by the whole warp one cell at a time in 16-byte chunks.  Positions are exact modulo 2^32, so
+// a region whose cells exceed its byte cap (< 2^32) gets no offset and no cell.
+__global__ void __launch_bounds__(256) k_region_scatter_var(const RegionParams p) {
+  __shared__ uint32_t s_base[8][8];
+  __shared__ uint32_t s_bpos[8][REGION_MAXV][8];
+  const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
+  const int64_t chunk = (int64_t)blockIdx.x * 8 + warp;
+  if (chunk >= p.n_chunks) return;
+  for (int i = lane; i < p.n_parts; i += 32) s_base[warp][i] = p.counts[(int64_t)i * p.n_chunks + chunk] - p.run_base(i);
+  for (int k = lane; k < p.n_var * p.n_parts; k += 32)
+    s_bpos[warp][k / p.n_parts][k % p.n_parts] = p.bcounts[(int64_t)k * p.n_chunks + chunk] - p.bcounts[(int64_t)k * p.n_chunks];
+  __syncwarp();
+  const int64_t lo = chunk * PART_CHUNK;
+  const int64_t hi = lo + PART_CHUNK < p.n ? lo + PART_CHUNK : p.n;
+  for (int64_t r0 = lo; r0 < hi; r0 += 32) {
+    const int64_t r = r0 + lane;
+    const bool active = r < hi;
+    const int part = active ? p.dest_of(r) : -1;
+    const unsigned peers = __match_any_sync(0xffffffffu, part);
+    const unsigned rank = __popc(peers & ((1u << lane) - 1));
+    const bool last = rank == (unsigned)__popc(peers) - 1;
+    uint32_t pos = 0;
+    if (active) pos = s_base[warp][part] + rank;
+    __syncwarp();
+    if (active && last) s_base[warp][part] = pos + 1;
+    __syncwarp();
+    if (active) p.store(r, part, pos);
+    for (int v = 0; v < p.n_var; v++) {
+      const uint64_t len = active ? p.cell_len(v, r) : 0;
+      uint64_t pre = 0;   // cells of the earlier rows of this warp step that go to the same destination
+      for (int d = 0; d < 32; d++) {
+        const uint64_t l = __shfl_sync(0xffffffffu, len, d);
+        if (d < lane && ((peers >> d) & 1)) pre += l;
+      }
+      uint32_t bpos = 0;
+      if (active) bpos = s_bpos[warp][v][part] + (uint32_t)pre;
+      __syncwarp();
+      if (active && last) s_bpos[warp][v][part] = bpos + (uint32_t)len;
+      __syncwarp();
+      const bool fits = active && pos < p.cap && p.btotal[v * p.n_parts + part] <= p.var[v].byte_cap;
+      unsigned long long src = 0, dst = 0;
+      if (fits) {
+        uint64_t *const *o = p.out + (int64_t)part * p.n_areas;
+        o[p.var[v].col][pos + 1] = (uint64_t)bpos + len;
+        dst = (unsigned long long)(reinterpret_cast<uint8_t *>(o[p.n_cols + 1 + v]) + bpos);
+        if (len) src = (unsigned long long)(p.var[v].bytes + p.var[v].off[p.in[p.var[v].col].data[r]]);
+      }
+      const unsigned todo = __ballot_sync(0xffffffffu, fits && len > 0);
+      for (int j = 0; j < 32; j++) {
+        if (!((todo >> j) & 1)) continue;
+        const uint8_t *cs = reinterpret_cast<const uint8_t *>(__shfl_sync(0xffffffffu, src, j));
+        uint8_t *cd = reinterpret_cast<uint8_t *>(__shfl_sync(0xffffffffu, dst, j));
+        const uint64_t cl = __shfl_sync(0xffffffffu, len, j);
+        for (uint64_t b = 16 * (uint64_t)lane; b < cl; b += 16 * 32) {
+          const uint64_t cnt = cl - b < 16 ? cl - b : 16;
+          uint64_t x, y;
+          load_chunk16(cs + b, cnt, x, y);
+          store_chunk16(cd + b, cnt, x, y);
+        }
+      }
+    }
+  }
+}
+
+int32_t scatter_to_regions_var(const DCol *cols, int n_cols, const RegionVar *var, int n_var, const uint8_t *dest, int64_t n, int n_parts,
+                               uint64_t *const *out, int64_t cap, uint32_t *rows, unsigned long long *overflow, RegionScratch &sc,
+                               cudaStream_t s) {
+  if (n_cols < 1 || n_cols > REGION_MAXW || n_var < 0 || n_var > REGION_MAXV || (n_var && !var) || n_parts < 1 || n_parts > 8 || n < 1 ||
+      n > 0xFFFFFFF0ll || cap < 1 || cap > 0xFFFFFFF0ll) {
+    set_error("internal: scatter_to_regions arguments");
+    return TQ_ERR_INVALID_ARG;
+  }
+  RegionParams p{};
+  p.n_cols = n_cols;
+  p.n_parts = n_parts;
+  p.n = n;
+  p.n_chunks = (n + PART_CHUNK - 1) / PART_CHUNK;
+  for (int c = 0; c < n_cols; c++) p.in[c] = cols[c];
+  p.dest = dest;
+  p.out = out;
+  p.cap = (uint32_t)cap;
+  p.n_areas = n_cols + 1 + n_var;
+  p.n_var = n_var;
+  for (int v = 0; v < n_var; v++) {
+    if (var[v].col < 0 || var[v].col >= n_cols || ((p.var_mask >> var[v].col) & 1) || var[v].byte_cap < 1 || var[v].byte_cap > 0xFFFFFFF0ull) {
+      set_error("internal: scatter_to_regions var-len column %d", v);
+      return TQ_ERR_INVALID_ARG;
+    }
+    p.var[v] = var[v];
+    p.var_mask |= 1ull << var[v].col;
+  }
+  const int64_t n_counts = p.n_chunks * n_parts;
+  TQ_TRY(sc.hist.reserve((size_t)n_counts * 4));
+  TQ_TRY(sc.total.reserve(8));
+  p.counts = sc.hist.as<uint32_t>();
+  const unsigned blocks = (unsigned)((p.n_chunks + 7) / 8);
+  TQ_LAUNCH(k_part_hist<RegionParams>, blocks, 256, 0, s, p);
+  count_launch();
+  TQ_TRY(check_launch("k_part_hist(regions)"));
+  TQ_TRY(exclusive_scan_u32(p.counts, 1, p.counts, 1, n_counts, sc.total.as<uint64_t>(), sc.scan, s));
+  TQ_LAUNCH(k_region_rows, 1, 32, 0, s, p.counts, p.n_chunks, n_parts, sc.total.as<uint64_t>(), p.cap, rows, overflow);
+  count_launch();
+  if (n_var == 0) {
+    TQ_LAUNCH(k_part_scatter<RegionParams>, blocks, 256, 0, s, p);
+    count_launch();
+    return check_launch("k_part_scatter(regions)");
+  }
+  const int64_t n_bcounts = n_counts * n_var;
+  TQ_TRY(sc.bhist.reserve((size_t)n_bcounts * 4));
+  TQ_TRY(sc.btotal.reserve((size_t)n_var * n_parts * 8));
+  p.bcounts = sc.bhist.as<uint32_t>();
+  p.btotal = sc.btotal.as<unsigned long long>();
+  TQ_CUDA(cudaMemsetAsync(p.btotal, 0, (size_t)n_var * n_parts * 8, s));
+  TQ_LAUNCH(k_region_var_hist, blocks, 256, 0, s, p);
+  count_launch();
+  TQ_TRY(check_launch("k_region_var_hist"));
+  TQ_TRY(exclusive_scan_u32(p.bcounts, 1, p.bcounts, 1, n_bcounts, nullptr, sc.bscan, s));
+  TQ_LAUNCH(k_region_bytes, 1, 32, 0, s, p, overflow);
+  TQ_LAUNCH(k_region_scatter_var, blocks, 256, 0, s, p);
+  count_launch(2);
+  return check_launch("k_region_scatter_var");
 }
 
 }  // namespace tq

@@ -36,8 +36,13 @@ static constexpr int GROUP_MAX_ITEMS = 8;
 static constexpr uint64_t GROUP_NULL_WORD = 0x4E554C4C4E554C4Cull;
 // dest[r] for n >= 1 rows; items: the n_items GROUP BY columns (device), real_mask bit g = item g is REAL.  Enqueued on s.
 int32_t group_dest(const DCol *items, int n_items, uint32_t real_mask, int64_t n, int n_parts, uint8_t *dest, cudaStream_t s);
+// The same with var-len items: where hashes[g] is not null, item g holds string-dictionary ids and v_g = hashes[g][id] (the
+// dictionary's content hash of the cell, sd_warp_hash: the same bytes give the same word on every rank).
+int32_t group_dest(const DCol *items, const uint64_t *const *hashes, int n_items, uint32_t real_mask, int64_t n, int n_parts, uint8_t *dest,
+                   cudaStream_t s);
 struct RegionScratch {
   DevBuf hist, scan, total;
+  DevBuf bhist, bscan, btotal;   // var-len wire columns: cell bytes per (column, destination, chunk) and per (column, destination)
 };
 // Scatters n >= 1 rows of n_cols (1..63) 8-byte columns to destination dest[r] < n_parts (<= 8): row i of destination q's run
 // (input order) goes to out[q * (n_cols + 1) + c][i] for every column c, the mask word (bit c = column c is NOT NULL) to
@@ -45,6 +50,24 @@ struct RegionScratch {
 // *overflow (device u64) = 1 when some rows[q] > cap, 0 otherwise; rows at or past cap are not written.  Enqueued on s.
 int32_t scatter_to_regions(const DCol *cols, int n_cols, const uint8_t *dest, int64_t n, int n_parts, uint64_t *const *out, int64_t cap,
                            uint32_t *rows, unsigned long long *overflow, RegionScratch &sc, cudaStream_t s);
+// A var-len wire column of scatter_to_regions_var: column `col` holds ids into an arena of cells (id i = bytes
+// [off[i], off[i + 1]) of `bytes`); on the wire its area is the region's cap + 1 offsets and its cells go to a byte area of
+// byte_cap bytes.
+static constexpr int REGION_MAXV = 16;
+struct RegionVar {
+  int col;
+  const int64_t *off;
+  const uint8_t *bytes;
+  uint64_t byte_cap;
+};
+// scatter_to_regions with n_var (0..REGION_MAXV) var-len columns: destination q's areas are out[q * (n_cols + 1 + n_var) + a]:
+// areas 0..n_cols - 1 as above except that var-len column var[v].col gets offsets (entry 0 = 0, entry i + 1 = end of row i's
+// cell; a NULL cell is empty), the mask word at n_cols, then the n_var byte areas in var[] order holding the cells in row
+// order.  *overflow = 1 also when some region's cells of var[v] exceed var[v].byte_cap; no byte is written past a byte cap
+// and no offset past cap + 1 words.  1 <= byte_cap < 2^32.  Enqueued on s.
+int32_t scatter_to_regions_var(const DCol *cols, int n_cols, const RegionVar *var, int n_var, const uint8_t *dest, int64_t n, int n_parts,
+                               uint64_t *const *out, int64_t cap, uint32_t *rows, unsigned long long *overflow, RegionScratch &sc,
+                               cudaStream_t s);
 // The receiving side: bitmap bm[c] (a host array of n_cols <= 63 device bitmaps) gets bit c of mask[r] for the n >= 1 rows, whole 64-row
 // groups, 0 past the last row.  Enqueued on s.
 int32_t expand_null_mask(const uint64_t *mask, int64_t n, int n_cols, uint32_t *const *bm, cudaStream_t s);

@@ -870,7 +870,7 @@ class BroadcastJoin:
 def agg_drain(lib, L, h, n_funcs):
     """the finished groups of an aggregation handle after tq_agg_eof, as host Columns: tq_agg_next_device, and — when it has
     no groups — tq_agg_next, which returns the one default row of a scalar aggregate over no rows (COUNT 0, the rest NULL)"""
-    from .chunk import Column, device_to_host
+    from .chunk import Column, VarColumn, device_to_host, device_var_to_host
     types = []
     for i in range(n_funcs):
         t = C.c_int32(0)
@@ -880,34 +880,64 @@ def agg_drain(lib, L, h, n_funcs):
     rows, eof = C.c_int64(0), C.c_int32(0)
     L.check(lib.tq_agg_next_device(h, out, C.byref(rows), C.byref(eof)))
     if rows.value:
-        return [device_to_host(types[i], out[i].data, out[i].null_bitmap, rows.value) for i in range(n_funcs)]
+        return [device_var_to_host(out[i].data, out[i].offsets, out[i].null_bitmap, rows.value) if types[i] == L.TQ_TYPE_BYTES
+                else device_to_host(types[i], out[i].data, out[i].null_bitmap, rows.value) for i in range(n_funcs)]
     data = [np.zeros(1, np.uint64) for _ in range(n_funcs)]
     bms = [np.zeros(8, np.uint8) for _ in range(n_funcs)]
+    offs = [np.zeros(2, np.int64) for _ in range(n_funcs)]
     for i in range(n_funcs):
         out[i].data, out[i].null_bitmap, out[i].offsets = data[i].ctypes.data, bms[i].ctypes.data, None
+        if types[i] == L.TQ_TYPE_BYTES:
+            out[i].offsets = offs[i].ctypes.data
     L.check(lib.tq_agg_next(h, 1, out, C.byref(rows), C.byref(eof)))
     if rows.value == 0:
-        return [Column.empty(t, 0) for t in types]
-    return [Column(t, data[i].view(np.float64 if t == L.TQ_TYPE_FLOAT64 else (np.uint64 if t == L.TQ_TYPE_UINT64 else np.int64)),
+        return [(VarColumn if t == L.TQ_TYPE_BYTES else Column).empty(t, 0) for t in types]
+    return [VarColumn(t, [None if not bms[i][0] & 1 else b""]) if t == L.TQ_TYPE_BYTES else
+            Column(t, data[i].view(np.float64 if t == L.TQ_TYPE_FLOAT64 else (np.uint64 if t == L.TQ_TYPE_UINT64 else np.int64)),
                    np.array([bool(bms[i][0] & 1)])) for i, t in enumerate(types)]
+
+
+def partial_var_cols(types, group_by, funcs):
+    """the var-len (string) partial columns of a GROUP BY, as tq_agg_push_partial_var sends them: [(partial column, input
+    column)] for every GROUP BY item on a BYTES column and every MAX / MIN / FIRSTROW over a BYTES argument, in partial-column
+    order (the GROUP BY items, then one column per function, two for AVG)"""
+    from . import _lib
+    is_bytes = [(t & 0xFF) == _lib.TQ_TYPE_BYTES for t in types]
+    out, c = [], 0
+    for g in group_by:
+        if is_bytes[g]:
+            out.append((c, g))
+        c += 1
+    for f, a in funcs:
+        if f in (3, 4, 5) and a >= 0 and is_bytes[a]:         # TQ_AGG_MAX, TQ_AGG_MIN, TQ_AGG_FIRSTROW
+            out.append((c, a))
+        c += 2 if f == 2 else 1                              # TQ_AGG_AVG: (count, sum)
+    return out
 
 
 class RegionAgg:
     """The multi-GPU GROUP BY over a RegionExchange of one table: w + 1 wire columns (w = tq_agg_partial_width: the partial
-    row, then its NULL mask word).  One step:
+    row, then its NULL mask word), then one byte area per var-len (string) partial column.  One step:
 
-        this rank      Partial1 handle <- tq_agg_put(shard) -> eof -> tq_agg_push_partial        (push stream)
-        compute stream tq_region_wait -> Final handle <- tq_agg_merge_regions -> eof -> next_device
+        this rank      Partial1 handle <- tq_agg_put(shard) -> eof -> tq_agg_push_partial_var    (push stream)
+        compute stream tq_region_wait -> Final handle <- tq_agg_merge_regions_var -> eof -> next_device
 
-    A partial group travels to the rank its group names (tq_agg_push_partial: with one NOT NULL item the rank the join sends
-    that key to), so every group is finished on exactly one rank; a scalar aggregate is finished on rank 0 only, which returns
-    its one row even when every shard is empty.  Host synchronisation per step: the export's group count, the merge's slot
-    read, the result drain and ONE barrier at the end (nobody may push into a region a peer is still merging)."""
+    A partial group travels to the rank its group names (tq_agg_push_partial_var: with one NOT NULL 8-byte item the rank the
+    join sends that key to; a string item by the content hash of its bytes), so every group is finished on exactly one rank; a
+    scalar aggregate is finished on rank 0 only, which returns its one row even when every shard is empty.  A string partial
+    column travels as offsets plus its cells, which the receiver encodes into its own dictionary.  Without string columns the
+    wire format is tq_agg_push_partial's.  Host synchronisation per step: the export's group count, the merge's slot read (and
+    one byte-total read per string column and region), the result drain and ONE barrier at the end (nobody may push into a
+    region a peer is still merging)."""
 
-    def __init__(self, lib, L, world, rank, types, group_by, funcs, max_groups_per_rank, slack=1.25, est_groups=0, slot=0):
+    def __init__(self, lib, L, world, rank, types, group_by, funcs, max_groups_per_rank, slack=1.25, est_groups=0, slot=0, byte_caps=None,
+                 exchange=None):
         """types: TQ_TYPE_* per input column (| TQ_TYPE_NOT_NULL where declared so); group_by: input column indices;
-        funcs: [(TQ_AGG_*, arg_col)].  max_groups_per_rank: the most groups one rank's shard holds (every rank passes the same
-        numbers: the layout is shared)."""
+        funcs: [(TQ_AGG_*, arg_col)].  max_groups_per_rank: the most groups one rank's shard holds; byte_caps: per input
+        column, for a BYTES column the most cell bytes one rank's partial rows hold in one partial column of it (at most the
+        bytes of the shard's column), None for the others.  Every rank passes the same numbers: the layout is shared.
+        exchange: a RegionLayout with the attributes of a RegionExchange (rank, epoch, wait, next_epoch) holding
+        RegionAgg.table_of(...) as table 0; by default a RegionExchange over the ranks of the process group."""
         self.lib, self.L, self.world, self.rank, self.slot = lib, L, world, rank, slot
         self.types, self.group_by, self.funcs, self.est_groups = list(types), list(group_by), list(funcs), est_groups
         h, keep = self._create()
@@ -919,10 +949,33 @@ class RegionAgg:
         self.width = width.value
         if self.width + 1 > 64:
             raise ValueError(f"RegionAgg: {self.width} partial columns and the mask word exceed 64 words per row")
-        # a group lands on one rank by its hash: +25 % covers the imbalance between (source, destination) pairs
-        cap = 1 if not group_by else int(max_groups_per_rank / world * slack) + (1 << 14)
-        self.rx = RegionExchange(lib, L, world, rank, [(self.width + 1, cap)])
+        self.var_cols = partial_var_cols(self.types, self.group_by, self.funcs)
+        self.table, self.byte_cap = RegionAgg.table_of(world, self.width, self.var_cols, bool(group_by), max_groups_per_rank, byte_caps, slack)
+        self.rx = exchange if exchange is not None else RegionExchange(lib, L, world, rank, [self.table])
+        self._hp = None
         self.last_phase = {}
+
+    @staticmethod
+    def table_of(world, width, var_cols, grouped, max_groups_per_rank, byte_caps=None, slack=1.25):
+        """(the RegionLayout table, the byte cap of every var-len partial column): width + 1 word areas of cap rows (a var-len
+        column's area is cap + 1 offsets, rounded up to 16 bytes), then one byte area per var-len column.  Rows and bytes take
+        the same slack: a group lands on one rank by its hash, so +25 % (and a fixed margin) covers the imbalance between
+        (source, destination) pairs.  Without var-len columns it is (width + 1, cap)."""
+        cap = _round_up(1 if not grouped else int(max_groups_per_rank / world * slack) + (1 << 14), 4096)
+        if not var_cols:
+            return (width + 1, cap), []
+        byte_cap = []
+        for _, src in var_cols:
+            most = byte_caps[src] if byte_caps and src < len(byte_caps) else None
+            if most is None:
+                raise ValueError(f"RegionAgg: input column {src} is a string column and needs byte_caps[{src}]")
+            b = _round_up(int(int(most) / world * slack) + (1 << 14), 16)
+            if b >= 1 << 32:
+                raise ValueError(f"RegionAgg: {b} bytes per region for input column {src}: at most 2^32 - 16")
+            byte_cap.append(b)
+        var = {c for c, _ in var_cols}
+        words = [_round_up(cap + 1, 2) if c in var else cap for c in range(width)] + [cap] + [b // 8 for b in byte_cap]
+        return (len(words), cap, words), byte_cap
 
     def _create(self):
         L = self.L
@@ -937,26 +990,44 @@ class RegionAgg:
     def close(self):
         self.rx.close()
 
-    def step(self, cols, bitmaps=None, keep_result=False):
-        """cols: this rank's shard of every input column ((device pointer, rows)-like objects); bitmaps: a device NULL bitmap
-        pointer (or None) per column.  Returns (groups finished on this rank, result): result (keep_result) = host Columns of
-        the function outputs, None otherwise."""
-        lib, L, rx, w = self.lib, self.L, self.rx, self.world
-        n = int(cols[0].numel()) if cols else 0
-        rx.next_epoch()
-        hp, keep_p = self._create()
+    def merge_table(self, dst):
+        """destination dst's regions as tq_agg_merge_regions_var takes them: regions[g * (w + 1) + c], a var-len column with
+        .offsets = its word area and .data = its byte area"""
+        rx, nw = self.rx, self.width + 1
+        regs = (self.L.TQColumn * (self.world * nw))()
+        for g in range(self.world):
+            for c in range(nw):
+                regs[g * nw + c].length, regs[g * nw + c].data = rx.cap[0], rx.region_ptr(dst, 0, g, c)
+            for v, (c, _) in enumerate(self.var_cols):
+                regs[g * nw + c].offsets = regs[g * nw + c].data
+                regs[g * nw + c].data = rx.region_ptr(dst, 0, g, nw + v)
+        return regs
+
+    def push(self, cols, bitmaps=None):
+        """this rank's half of a step before the merge: aggregate the shard into a Partial1 handle and enqueue its push (push
+        stream) for the exchange's current epoch.  cols: this rank's shard of every input column ((device pointer,
+        rows)-like objects, or VarCol / DeviceVarColumn for BYTES); bitmaps: a device NULL bitmap pointer (or None) per
+        column.  The handle is read until tq_partition_push_sync(slot)."""
+        lib, L, rx = self.lib, self.L, self.rx
+        arr, n = _tq_device(L, cols, bitmaps)
+        hp, _ = self._create()
+        self._hp = hp
+        if n:
+            L.check(lib.tq_agg_put(hp, arr, L.TQ_MEM_DEVICE))
+        L.check(lib.tq_agg_eof(hp))
+        dest, cnts = rx.push_tables(0, self.rank)
+        caps = (C.c_int64 * max(len(self.byte_cap), 1))(*self.byte_cap)
+        L.check(lib.tq_agg_push_partial_var(hp, self.world, dest, cnts, rx.cap[0], caps, self.slot, rx.epoch))
+
+    def finish(self, keep_result=False):
+        """this rank's half after every rank's push was enqueued: wait, merge, finish.  Returns (groups finished on this rank,
+        result): result (keep_result) = host Columns of the function outputs, None otherwise.  A region past its row or byte
+        cap is TQ_ERR_OOM (RuntimeError)."""
+        lib, L, rx = self.lib, self.L, self.rx
         hf, keep_f = self._create()
         try:
-            if n:
-                arr = _tq_cols(L, cols, n)
-                for c, b in enumerate(bitmaps or []):
-                    arr[c].null_bitmap = b
-                L.check(lib.tq_agg_put(hp, arr, L.TQ_MEM_DEVICE))
-            L.check(lib.tq_agg_eof(hp))
-            dest, cnts = rx.push_tables(0, self.rank)
-            L.check(lib.tq_agg_push_partial(hp, w, dest, cnts, rx.cap[0], self.slot, rx.epoch))
             rx.wait(0)
-            L.check(lib.tq_agg_merge_regions(hf, w, C.c_void_p(rx.slot_ptr(self.rank, 0, 0)), rx.cap[0], rx.region_table(self.rank, 0)))
+            L.check(lib.tq_agg_merge_regions_var(hf, self.world, C.c_void_p(rx.slot_ptr(self.rank, 0, 0)), rx.cap[0], self.merge_table(self.rank)))
             L.check(lib.tq_agg_eof(hf))
             L.check(lib.tq_partition_push_sync(self.slot))     # the push reads the Partial1 handle's rows until it is done
             res, groups = None, 0
@@ -972,10 +1043,27 @@ class RegionAgg:
                 else:                                        # a scalar aggregate over no rows: the default row, unless all FIRSTROW
                     groups = int(any(f != 5 for f, _ in self.funcs))
         finally:
-            lib.tq_agg_destroy(hp)
+            if self._hp is not None:
+                lib.tq_partition_push_sync(self.slot)
+                lib.tq_agg_destroy(self._hp)
+                self._hp = None
             lib.tq_agg_destroy(hf)
-        dist.barrier()
         return groups, res
+
+    def step(self, cols, bitmaps=None, keep_result=False):
+        """one step on this rank: push, wait, merge, finish, then one barrier.  cols / bitmaps as push().  Returns (groups
+        finished on this rank, result) as finish()."""
+        self.rx.next_epoch()
+        try:
+            self.push(cols, bitmaps)
+            res = self.finish(keep_result)
+        finally:
+            if self._hp is not None:
+                self.lib.tq_partition_push_sync(self.slot)
+                self.lib.tq_agg_destroy(self._hp)
+                self._hp = None
+        dist.barrier()
+        return res
 
 
 def gen_dist_tables(rank, world, n_b, n_p):
