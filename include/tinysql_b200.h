@@ -495,12 +495,18 @@ int32_t tq_agg_merge_partial(tq_agg *a, const tq_column *cols, int32_t mem);
  *
  * tq_agg_merge_regions, on a handle created with the same desc that has taken no raw rows (queue tq_region_wait first):
  * reads the n_regions (1..8) consecutive slots at `slots` (one host read) and merges regions[g * (w + 1) + c] (wire column c
- * of region g) with tq_agg_merge_partial's semantics, reading the regions in place.  A slot above region_cap (or ~0) is
- * TQ_ERR_OOM and merges nothing.  Then tq_agg_eof / next as usual.
+ * of region g) with tq_agg_merge_partial's semantics, reading the regions in place.  A slot reading 0xFFFFFFFF00000000 | s
+ * (a failed push, below) returns status s and merges nothing, so every rank refuses a step one source could not push; any
+ * other slot above region_cap (or ~0) is TQ_ERR_OOM and merges nothing.  Then tq_agg_eof / next as usual: a merged total
+ * that leaves int64 is TQ_ERR_OVERFLOW_BIGINT from next / next_device on the rank that finishes the group.
  *
  * Both refuse what tq_agg_export_partial / tq_agg_merge_partial refuse (var-len columns: TQ_ERR_UNSUPPORTED_TYPE; a FinalMode
  * handle, or raw and partial rows on one handle: TQ_ERR_STATE), and check every argument before anything is enqueued: a
- * refused push writes no region and publishes no slot. */
+ * refused push writes no region and publishes no slot.  A push that fails after those checks — a group's partial SUM / AVG
+ * total on this rank leaves int64 (TQ_ERR_OVERFLOW_BIGINT, as tq_agg_export_partial), more than 2^32 - 16 partial rows, a
+ * failed allocation — writes no region row but still publishes {0xFFFFFFFF00000000 | status, epoch} in every destination's
+ * slot (waited for with tq_partition_push_sync(slot) as usual), so no tq_region_wait waits for it and every merge of the
+ * step returns that status.  tq_region_gather and dist.RegionLayout.counts refuse the marker as a count past the cap. */
 int32_t tq_agg_push_partial(tq_agg *a, int32_t n_parts, void *const *dest_data, void *const *dest_counts, int64_t region_cap,
                             int32_t slot, uint64_t epoch);
 int32_t tq_agg_merge_regions(tq_agg *a, int32_t n_regions, const void *slots, int64_t region_cap, const tq_column *regions);

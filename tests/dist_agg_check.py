@@ -70,6 +70,45 @@ def main():
     partial_fn, final_fn = D.gpu_agg_fns(lib, L, [I64, I64], 0, funcs)
     nccl = D.distributed_agg([tk, tv], world, rank, partial_fn, D.gpu_partition_fn(lib, L), final_fn)
     assert np.array_equal(RA.canon(res), RA.canon(nccl)), "RegionAgg and distributed_agg differ"
+
+    # ---- the int64 limits, four steps on one RegionAgg: exact; a merged total past INT64_MAX (its owner fails, the others
+    # are exact); a part past INT64_MAX on one rank (every rank fails); exact again.  Every rank builds every rank's shard
+    # from one seed, so each can name its own expected status and groups (region_agg_ref.expect_ranks).
+    import int_agg_ref as I
+    from tinysql_b200.chunk import Chunk, Column
+    lfuncs = [(COUNT, -1), (SUM, 1), (AVG, 1), (FIRSTROW, 0)]
+    ltypes = [I64, I64]
+    frng = np.random.default_rng(77)
+    fam = I.limits(frng, n_groups=200, hi=400)
+    past_twin = I.out_by_one(fam, I.INT64_MAX + 1, frng)
+    sizes, tot = np.bincount(fam.gid), I.group_totals(fam)
+    big = max((g for g in range(len(sizes)) if tot[g] >= 0), key=lambda g: sizes[g])
+    steps = [("limits", I.deal(frng, fam, world, rebuild=True)),
+             ("merged_past", I.deal(frng, past_twin, world, rebuild=True)),
+             ("part_past", I.deal(frng, fam, world, rebuild=True, past=(big, world - 1)) if world > 1 else I.deal(frng, past_twin, 1)),
+             ("clean", I.deal(frng, fam, world, rebuild=True))]
+    ra = D.RegionAgg(lib, L, world, rank, ltypes, [0], lfuncs, max_groups_per_rank=4096)
+    for name, dealt in steps:
+        rank_cols = [[I.key_column(d.gid) if len(d.gid) else Column(I64, np.zeros(0, np.int64), np.zeros(0, bool)), Column(I64, d.x)]
+                     for d in dealt]
+        exp = RA.expect_ranks(ltypes, rank_cols, [0], lfuncs, world)
+        assert {"limits": not exp.push_fail and not exp.dest_fail, "clean": not exp.push_fail and not exp.dest_fail,
+                "merged_past": bool(exp.push_fail) if world == 1 else (not exp.push_fail and len(exp.dest_fail) == 1),
+                "part_past": bool(exp.push_fail)}[name], (name, exp.push_fail, exp.dest_fail)
+        key, x = rank_cols[rank]
+        dk, dx, dbm = t(key.values), t(x.values), bm(key.not_null())
+        torch.cuda.synchronize()
+        try:
+            _, res = ra.step([dk, dx], [dbm.data_ptr(), None], keep_result=True)
+            status = L.TQ_OK
+        except L.TQError as e:
+            status, res = e.status, None
+        fails = bool(exp.push_fail) or rank in exp.dest_fail
+        assert status == (L.TQ_ERR_OVERFLOW_BIGINT if fails else L.TQ_OK), (name, rank, status)
+        if not fails:
+            bad = I.mismatches(I.result_rows(Chunk(res), [3]), exp.ranks[rank], lfuncs)
+            assert not bad, (name, rank, bad[:5])
+    ra.close()
     print(f"DIST_AGG_OK world={world} rank={rank} groups={res[0].length}", flush=True)
     dist.barrier()
     dist.destroy_process_group()

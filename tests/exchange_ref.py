@@ -123,10 +123,11 @@ def bitmap_words(nn):
 
 class Regions(RegionLayout):
     """W emulated ranks' receive buffers of one table (t = 0): slots start at zero (epoch 0: nothing published), regions and
-    guards at the sentinel."""
+    guards at the sentinel.  words: words per wire column when they are not cap each (dist.RegionAgg.table_of's var-len
+    layout)."""
 
-    def __init__(self, lib, world, ncols, cap, guard=64):
-        super().__init__(lib, L, world, [(ncols, cap)], pad_rows=guard)
+    def __init__(self, lib, world, ncols, cap, guard=64, words=None):
+        super().__init__(lib, L, world, [(ncols, cap) if words is None else (ncols, cap, words)], pad_rows=guard)
         self.buf = Buf(lib, world * self.bytes)
         self.bases = [self.buf.addr(d * self.bytes) for d in range(world)]
         for d in range(world):
@@ -154,8 +155,9 @@ class Regions(RegionLayout):
         return [(int(r), int(e)) for r, e in self.read_slots(dst)[0]]
 
     def region(self, dst, src, c):
-        """the region's cap rows followed by its guard rows"""
-        out = np.empty(self.cap[0] + self.pad_rows, np.uint64)
+        """the region's words (cap rows, unless the layout lists its own) followed by its guard rows"""
+        offs = self.col_off[0] + [self.stride[0]]
+        out = np.empty(offs[c + 1] - offs[c], np.uint64)
         L.check(self.lib.tq_memcpy_d2h(out.ctypes.data, C.c_void_p(self.region_ptr(dst, 0, src, c)), out.nbytes))
         return out
 

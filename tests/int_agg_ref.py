@@ -22,7 +22,7 @@ import numpy as np
 
 from float_agg_ref import group_rows, key_labels
 from hash_targets import EMPTY_KEY
-from tinysql_b200.chunk import INT64, UINT64, Chunk, Column
+from tinysql_b200.chunk import BYTES, INT64, UINT64, Chunk, Column, VarColumn
 
 COUNT, SUM, AVG, MAX, MIN, FIRSTROW = range(6)
 INT64_MIN, INT64_MAX = -(1 << 63), (1 << 63) - 1
@@ -79,9 +79,10 @@ def prefix_out_of_range(x):
 
 
 # ------------------------------------------------------------------ the reference
-Expected = namedtuple("Expected", "groups overflow")
+Expected = namedtuple("Expected", "groups overflow over", defaults=(frozenset(),))
 """groups: {group key tuple: [per function: int, None (= NULL) or, for FIRSTROW of a non-key column, a frozenset]};
-overflow: some group's SUM / AVG total leaves int64 (the aggregation must fail with ErrOverflow)"""
+overflow: some group's SUM / AVG total leaves int64 (the aggregation must fail with ErrOverflow); over: the key tuples of
+those groups (the rank that finishes one of them fails, the others do not)"""
 
 
 def _grouped(gid, n_groups, sel):
@@ -97,7 +98,7 @@ def expect(cols, group_by, funcs):
     gid, labels = group_rows([cols[g] for g in group_by], n)
     ng = len(labels)
     rows = [[None] * len(funcs) for _ in range(ng)]
-    overflow = False
+    over = set()
     for fi, (f, a) in enumerate(funcs):
         if a < 0:
             nn, x = np.ones(n, bool), np.ones(n, np.int64)
@@ -113,7 +114,8 @@ def expect(cols, group_by, funcs):
             for g in range(ng):
                 if cnt[g] == 0:
                     continue
-                overflow |= not in_range(sums[g])
+                if not in_range(sums[g]):
+                    over.add(labels[g])
                 rows[g][fi] = sums[g] if f == SUM else trunc_div(sums[g], int(cnt[g]))
         elif f in (MAX, MIN):
             v = x[order]
@@ -132,7 +134,7 @@ def expect(cols, group_by, funcs):
                 sets[g].add(v)
             for g in range(ng):
                 rows[g][fi] = frozenset(sets[g])
-    return Expected({lab: r for lab, r in zip(labels, rows)}, overflow)
+    return Expected({lab: r for lab, r in zip(labels, rows)}, bool(over), frozenset(over))
 
 
 def result_rows(chunk, key_idx):
@@ -217,20 +219,22 @@ def expect_final(pcols, group_by, ffuncs):
                 acc[g][fi] = (cur or 0) + (v if f == COUNT else as_i64(v))
             else:
                 acc[g][fi] = v if cur is None else (max(cur, v) if f == MAX else min(cur, v))
-    overflow = False
+    over = set()
     for g in range(len(labels)):
         for fi, (f, a, b) in enumerate(ffuncs):
             if f == COUNT:
                 acc[g][fi] = acc[g][fi] or 0
             elif f == SUM and acc[g][fi] is not None:
-                overflow |= not in_range(acc[g][fi])
+                if not in_range(acc[g][fi]):
+                    over.add(labels[g])
             elif f == AVG:
                 if cnt[g][fi] == 0:
                     acc[g][fi] = None
                 else:
-                    overflow |= not in_range(acc[g][fi])
+                    if not in_range(acc[g][fi]):
+                        over.add(labels[g])
                     acc[g][fi] = trunc_div(acc[g][fi], cnt[g][fi])
-    return Expected({lab: r for lab, r in zip(labels, acc)}, overflow)
+    return Expected({lab: r for lab, r in zip(labels, acc)}, bool(over), frozenset(over))
 
 
 def final_funcs(funcs, n_group_by):
@@ -244,7 +248,9 @@ def final_funcs(funcs, n_group_by):
 
 
 def column(tp, vals):
-    """a Column of Python ints / None (BIGINT UNSIGNED values in [0, 2^64))"""
+    """a Column of Python ints / None (BIGINT UNSIGNED values in [0, 2^64)), or a VarColumn of bytes / None"""
+    if tp == BYTES:
+        return VarColumn(BYTES, list(vals))
     nn = [v is not None for v in vals]
     dt = np.uint64 if tp == UINT64 else np.int64
     arr = np.array([0 if v is None else v for v in vals], dtype=object).astype(dt) if vals else np.zeros(0, dt)
@@ -524,3 +530,79 @@ def check_family(fam):
         assert set(v for v in vals_of if v is not None) == set(EXTREMES[fam.meta["tp"]])
         assert any(not fam.nn[fam.gid == g].all() for g in range(ng) if vals_of[g] is not None)
     return fam
+
+
+# ------------------------------------------------------------------ rows dealt to ranks (the GROUP BY across GPUs)
+Dealt = namedtuple("Dealt", "gid x nn parts")
+"""per rank: gid, x, nn (as a Family's) of the rows that rank holds; parts: {(group, rank): exact total of its non-NULL rows}"""
+
+
+def _part_targets(rng, total, k, past=False):
+    """k targets that add up to total, each in int64 except the first when past (INT64_MAX + 1); k = 1: [total]"""
+    if k == 1:
+        return [total]
+    for _ in range(10_000):
+        t = [INT64_MAX + 1] if past else []
+        while len(t) < k - 1:
+            t.append(TARGETS[int(rng.integers(len(TARGETS)))] if rng.random() < 0.5 else _random63(rng))
+        if in_range(total - sum(t)):
+            return t + [total - sum(t)]
+    raise ValueError(f"no {k} parts of {total} in range (a part past the limit on 2 ranks needs a total >= 0)")
+
+
+def _part_sum(x, nn):
+    return group_sums(np.zeros(len(x), np.int64), x, nn)[0] if len(x) else 0
+
+
+def deal(rng, fam, W, rebuild=False, whole=(), empty=(), past=None):
+    """the rows of a family dealt over W ranks (none on the ranks in `empty`), each rank's rows in random order.  A group of
+    at least 2 rows goes to 2 or more of the ranks that may hold rows, unless it is in `whole` (every group when whole is
+    True): those stay on one random rank, so partials whose in-order prefixes wrap travel as they are.
+    rebuild (families without NULLs): the values are replaced; each group keeps its size and total, every (group, rank) part
+    totals a target of its own (TARGETS or a random 63-bit value) and its terms come from group_terms, so the low word of
+    every part still wraps.  Without rebuild the values are kept, and a group is re-dealt until every part is in range (after
+    200 tries it stays on one rank).  past = (group, rank), with rebuild: that part totals INT64_MAX + 1 while the group's
+    total is unchanged (the group needs 3 rows, and a total >= 0 when it lands on 2 ranks)."""
+    ng = int(fam.gid.max()) + 1
+    ranks = [r for r in range(W) if r not in empty]
+    nn = np.asarray(fam.nn, bool)
+    assert not rebuild or (nn.all() and np.asarray(fam.x).dtype == np.int64)
+    totals = group_sums(fam.gid, fam.x, nn)
+    out_rank = np.empty(len(fam.gid), np.int64)
+    x = np.asarray(fam.x).copy()
+    parts = {}
+    for g in range(ng):
+        rows = np.nonzero(fam.gid == g)[0]
+        m = len(rows)
+        is_past = past is not None and past[0] == g
+        spread = not (whole is True or (whole is not False and g in whole)) and len(ranks) > 1 and m >= 2
+        for attempt in range(201):
+            if not spread or attempt == 200:
+                owners = [ranks[int(rng.integers(len(ranks)))]]
+            else:
+                most = min(len(ranks), m)   # a total past the limits needs enough in-range parts to reach it
+                least = min(most, max(2, -(-abs(totals[g]) // INT64_MAX))) if rebuild else 2
+                owners = [int(o) for o in rng.choice(ranks, int(rng.integers(least, most + 1)), replace=False)]
+            if is_past:
+                owners = [past[1]] + [o for o in owners if o != past[1]][: max(1, len(owners) - 1)]
+                assert len(owners) >= 2 and m >= 3
+            need = [2 if (is_past and i == 0) else 1 for i in range(len(owners))]
+            assign = np.concatenate([np.repeat(owners, need), rng.choice(owners, m - sum(need))])[rng.permutation(m)]
+            if rebuild:
+                tg = _part_targets(rng, totals[g], len(owners), is_past)
+                for o, t in zip(owners, tg):
+                    sel = rows[assign == o]
+                    x[sel] = np.array(group_terms(rng, len(sel), t), dtype=object).astype(np.int64)
+                break
+            if all(in_range(_part_sum(x[rows[assign == o]], nn[rows[assign == o]])) for o in owners):
+                break
+        out_rank[rows] = assign
+        for o in owners:
+            sel = rows[assign == o]
+            parts[(g, o)] = _part_sum(x[sel], nn[sel])
+    out = []
+    for r in range(W):
+        sel = np.nonzero(out_rank == r)[0]
+        sel = sel[rng.permutation(len(sel))]
+        out.append(Dealt(fam.gid[sel], x[sel], nn[sel], {k: v for k, v in parts.items() if k[1] == r}))
+    return out

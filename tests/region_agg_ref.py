@@ -4,14 +4,16 @@ it with every rank emulated in one process on exchange_ref's Regions, whose argu
 group_dest is the Python twin of the destination rule (include/tinysql_b200.h, csrc/scatter.cuh): h = 0, then per GROUP BY
 item h = mix64(h ^ v), v = the item's 8 bytes (REAL: -0.0 read as +0.0) or GROUP_NULL_WORD for NULL; rank = (h >> 40) % W."""
 import ctypes as C
+from collections import namedtuple
 
 import numpy as np
 
 import exchange_ref as X
+import int_agg_ref as I
 import oracle_py as O
 from tinysql_b200 import _lib as L
-from tinysql_b200.chunk import Column
-from tinysql_b200.dist import agg_drain, mix64_np
+from tinysql_b200.chunk import BYTES, Chunk, Column
+from tinysql_b200.dist import _tq_device, agg_drain, mix64_np, partial_var_cols
 
 GROUP_NULL_WORD = np.uint64(0x4E554C4C4E554C4C)
 NEG_ZERO = np.uint64(1 << 63)
@@ -58,9 +60,13 @@ def width(lib, d):
 
 
 def partial_handle(lib, d, src):
-    """a Partial1 handle fed one shard (an R.Source in device memory), eof'd"""
+    """a Partial1 handle fed one shard (an R.Source in device memory, or a list of DeviceColumn / DeviceVarColumn), eof'd"""
     h = create(lib, d)
-    if src.n:
+    if not hasattr(src, "ptrs"):
+        arr, n = _tq_device(L, src)
+        if n:
+            L.check(lib.tq_agg_put(h, arr, L.TQ_MEM_DEVICE))
+    elif src.n:
         arr = (L.TQColumn * len(src.ptrs))()
         for c in range(len(src.ptrs)):
             arr[c].length, arr[c].data, arr[c].null_bitmap = src.n, src.ptrs[c], src.bms[c]
@@ -69,28 +75,69 @@ def partial_handle(lib, d, src):
     return h
 
 
-def run(lib, W, types, group_by, funcs, shards, reg, epoch=1, not_null=()):
+def var_region_table(reg, dst, w, var_cols):
+    """destination dst's regions as tq_agg_merge_regions_var takes them (dist.RegionAgg.merge_table): a var-len column c has
+    .offsets = its word area and .data = its byte area (wire area w + 1 + v)"""
+    regs = reg.region_table(dst, 0)
+    nw, nc = w + 1, reg.ncols[0]
+    out = (L.TQColumn * (reg.world * nw))()
+    for g in range(reg.world):
+        for c in range(nw):
+            out[g * nw + c].length, out[g * nw + c].data = reg.cap[0], regs[g * nc + c].data
+        for v, (c, _) in enumerate(var_cols):
+            out[g * nw + c].offsets = out[g * nw + c].data
+            out[g * nw + c].data = regs[g * nc + nw + v].data
+    return out
+
+
+def run(lib, W, types, group_by, funcs, shards, reg, epoch=1, not_null=(), statuses=False, byte_cap=None):
     """one step: every source's Partial1 handle pushes (slot = source), every destination waits and merges into a Final handle.
-    shards: per source an R.Source.  Returns per destination (status of tq_agg_merge_regions, host Columns or None).  A scalar
-    aggregate is finished on destination 0 only (dist.RegionAgg): the others return None."""
+    shards: per source an R.Source (or a list of device columns).  Returns per destination (status of tq_agg_merge_regions,
+    host Columns or None).  A scalar aggregate is finished on destination 0 only (dist.RegionAgg): the others return None.
+    statuses: nothing raises on a failed push or drain; returns (the push status of every source, per destination (merge
+    status, status of tq_agg_next_device / tq_agg_next, host Columns or None)).  byte_cap: run the _var pair with these
+    byte caps on a reg laid out as dist.RegionAgg.table_of."""
     d, keep = desc(types, group_by, funcs, not_null)
-    hs = []
+    var = byte_cap is not None
+    if var:
+        w, var_cols = width(lib, d), partial_var_cols(types, group_by, funcs)
+        caps = (C.c_int64 * max(len(byte_cap), 1))(*byte_cap)
+    hs, pushed = [], []
     try:
         for s in range(W):
             hs.append(partial_handle(lib, d, shards[s]))
             dest, cnts = reg.push_tables(0, s)
-            L.check(lib.tq_agg_push_partial(hs[-1], W, dest, cnts, reg.cap[0], s, epoch))
+            if var:
+                st = lib.tq_agg_push_partial_var(hs[-1], W, dest, cnts, reg.cap[0], caps, s, epoch)
+            else:
+                st = lib.tq_agg_push_partial(hs[-1], W, dest, cnts, reg.cap[0], s, epoch)
+            if not statuses:
+                L.check(st)
+            pushed.append(st)
         out = []
         for q in range(W):
             L.check(reg.wait(q, epoch))                      # queued after every push that satisfies it
             hf = create(lib, d)
             try:
-                st = lib.tq_agg_merge_regions(hf, W, C.c_void_p(reg.slot_ptr(q, 0, 0)), reg.cap[0], reg.region_table(q, 0))
+                slots = C.c_void_p(reg.slot_ptr(q, 0, 0))
+                if var:
+                    st = lib.tq_agg_merge_regions_var(hf, W, slots, reg.cap[0], var_region_table(reg, q, w, var_cols))
+                else:
+                    st = lib.tq_agg_merge_regions(hf, W, slots, reg.cap[0], reg.region_table(q, 0))
                 if st != L.TQ_OK:
-                    out.append((st, None))
+                    out.append((st, None, None) if statuses else (st, None))
                     continue
                 L.check(lib.tq_agg_eof(hf))
-                out.append((st, agg_drain(lib, L, hf, len(funcs)) if group_by or q == 0 else None))
+                if not statuses:
+                    out.append((st, agg_drain(lib, L, hf, len(funcs)) if group_by or q == 0 else None))
+                    continue
+                nxt, cols = L.TQ_OK, None
+                if group_by or q == 0:
+                    try:
+                        cols = agg_drain(lib, L, hf, len(funcs))
+                    except L.TQError as e:
+                        nxt = e.status
+                out.append((st, nxt, cols))
             finally:
                 lib.tq_agg_destroy(hf)
         for s in range(W):
@@ -98,7 +145,7 @@ def run(lib, W, types, group_by, funcs, shards, reg, epoch=1, not_null=()):
     finally:
         for h in hs:
             lib.tq_agg_destroy(h)
-    return out
+    return (pushed, out) if statuses else out
 
 
 # ------------------------------------------------------------------------------------------------ comparison
@@ -130,3 +177,50 @@ def oracle(types, shards_host, group_by, funcs):
     rc, want = O.hash_agg(types, cols, group_by, funcs)
     assert rc == 0, rc
     return want
+
+
+# ------------------------------------------------------------------------------------------------ expectations per rank
+def key_dest(labels, key_types, W):
+    """the rank the destination twin names for each group key tuple of int_agg_ref.expect (None = NULL, bytes for a BYTES
+    item: its dictionary content hash); rank 0 for a scalar aggregate"""
+    import dict_targets as D
+    n = len(labels)
+    if not key_types:
+        return np.zeros(n, np.int64)
+    items, nns = [], []
+    for i, t in enumerate(key_types):
+        vals = [lab[i] for lab in labels]
+        nns.append(np.array([v is not None for v in vals], bool))
+        if (t & 0xFF) == BYTES:
+            items.append(D.sd_hashes([b"" if v is None else v for v in vals]))
+        elif (t & 0xFF) == L.TQ_TYPE_FLOAT64:
+            items.append(np.array([0.0 if v is None else v for v in vals], np.float64).view(np.uint64))
+        else:
+            items.append(np.array([0 if v is None else v % (1 << 64) for v in vals], dtype=object).astype(np.uint64))
+    return group_dest(n, items, nns, [(t & 0xFF) == L.TQ_TYPE_FLOAT64 for t in key_types], W)
+
+
+RankExpect = namedtuple("RankExpect", "push_fail dest_fail ranks")
+"""push_fail: the sources whose push must fail (a partial total of theirs leaves int64: int_agg_ref.expect_partial raises),
+and then every destination's merge fails; dest_fail (no push failing): the ranks that finish a group whose merged total
+leaves int64, whose next fails; ranks[q]: int_agg_ref.Expected of the groups rank q finishes"""
+
+
+def expect_ranks(types, rank_cols, group_by, funcs, W):
+    """where every failure of one step lands, and the exact groups of every other rank.  rank_cols: per source its input
+    Columns (BIGINT / BIGINT UNSIGNED arguments, keys of any type)"""
+    push_fail = set()
+    for r, cols in enumerate(rank_cols):
+        if cols[0].length:
+            try:
+                I.expect_partial(types, cols, group_by, funcs)
+            except OverflowError:
+                push_fail.add(r)
+    full = Chunk.concat([Chunk(c) for c in rank_cols], types).cols
+    want = I.expect(full, group_by, funcs)
+    labels = list(want.groups)
+    d = key_dest(labels, [types[g] for g in group_by], W)
+    owner = dict(zip(labels, d.tolist()))
+    dest_fail = set() if push_fail else {owner[k] for k in want.over}
+    ranks = [I.Expected({k: v for k, v in want.groups.items() if owner[k] == q}, False) for q in range(W)]
+    return RankExpect(push_fail, dest_fail, ranks)

@@ -167,3 +167,111 @@ def test_key_column_keeps_the_edge_keys_apart():
     vals = k.tolist()
     assert vals[:6] == R.EDGE_KEYS + [None]
     assert len(set(vals)) == 40
+
+
+# ------------------------------------------------------------------ rows dealt to ranks (the GROUP BY across GPUs)
+def _big_group(fam):
+    """the largest group whose total is >= 0: it can hold a part past INT64_MAX on any number of ranks"""
+    sizes = np.bincount(fam.gid)
+    tot = R.group_totals(fam)
+    return max((g for g in range(len(sizes)) if tot[g] >= 0), key=lambda g: sizes[g])
+
+
+def _dealt_cols(d, tp=INT64):
+    return [R.key_column(d.gid) if len(d.gid) else Column(INT64, np.zeros(0, np.int64)), Column(tp, d.x, d.nn)]
+
+
+@pytest.mark.parametrize("W", [1, 2, 3, 8])
+@pytest.mark.parametrize("name", ["limits", "out_by_one", "unsigned", "prefix_wraps"])
+def test_deal_hits_its_aims(name, W):
+    """every part in range (but the one aimed past the limit), part totals add up to the family's targets, groups spread over
+    ranks (prefix_wraps: whole), the empty rank holds nothing, and a rebuilt part's low word still wraps"""
+    rng = np.random.default_rng(60 + W)
+    fam = R.limits(rng) if name != "unsigned" else R.unsigned(rng)
+    if name == "prefix_wraps":
+        fam = R.prefix_wraps(rng)
+    if name == "out_by_one":
+        fam = R.check_family(R.out_by_one(fam, R.TWINS["max_plus_1"], rng))
+    empty = (1,) if W >= 3 else ()
+    rebuild = name in ("limits", "out_by_one")
+    past = (_big_group(fam), 0) if name == "limits" and W > 1 else None
+    dealt = R.deal(rng, fam, W, rebuild=rebuild, whole=name == "prefix_wraps", empty=empty, past=past)
+    ng = int(fam.gid.max()) + 1
+    totals = R.group_totals(fam)
+    parts = {}
+    for r, d in enumerate(dealt):
+        assert r not in empty or len(d.gid) == 0
+        for (g, rr), t in d.parts.items():
+            assert rr == r
+            parts.setdefault(g, []).append(t)
+            rows = d.gid == g
+            assert t == R.group_sums(np.zeros(int(rows.sum()), np.int64), d.x[rows], d.nn[rows])[0]
+            # out of range only where aimed: the part past the limit, or a whole out_by_one group on its one rank
+            assert R.in_range(t) or (past == (g, r) and t == R.INT64_MAX + 1) or (t == totals[g] and rows.sum() == (fam.gid == g).sum())
+            if rebuild and rows.sum() >= 64:
+                with np.errstate(over="ignore"):
+                    assert R._carries(d.x[rows]) >= rows.sum() // 8, (g, r)
+    assert [sum(parts[g]) for g in range(ng)] == totals
+    sizes = np.bincount(fam.gid, minlength=ng)
+    holders = [len(parts[g]) for g in range(ng)]
+    free = W - len(empty)
+    if name == "prefix_wraps" or free == 1:
+        assert max(holders) == 1
+    elif name != "unsigned":
+        assert all(h >= 2 for h, m in zip(holders, sizes) if m >= free)
+    else:
+        assert sum(h >= 2 for h, m in zip(holders, sizes) if m >= free) >= 0.9 * sum(m >= free for m in sizes)
+    assert sorted(np.concatenate([d.gid for d in dealt]).tolist()) == sorted(fam.gid.tolist())
+
+
+@pytest.mark.parametrize("W", [2, 3, 8])
+@pytest.mark.parametrize("name", ["limits", "unsigned", "avg_trunc", "extremes_only"])
+def test_final_over_dealt_partials_equals_the_whole(name, W):
+    """with no part past the limit, FinalMode over every rank's Partial1 rows (expect_final of expect_partial) is the
+    reference over all rows: the same groups, counts, totals, averages and extremes; FIRSTROW picks are values of the group"""
+    rng = np.random.default_rng(80 + W)
+    fam = R.make(name, rng)
+    tp = UINT64 if fam.x.dtype == np.uint64 else INT64
+    dealt = R.deal(rng, fam, W, rebuild=name == "limits")
+    funcs = [f for f in FUNCS if f != (FIRSTROW, 0)]
+    types = [INT64, tp]
+    pt, chunks = None, []
+    for d in dealt:
+        if len(d.gid):
+            pt, ch = R.expect_partial(types, _dealt_cols(d, tp), [0], funcs)
+            chunks.append(ch)
+    pcols = R.Chunk.concat(chunks, pt).cols
+    ff, gb = R.final_funcs(funcs, 1)
+    got = R.expect_final(pcols, gb, ff)
+    every = R.Dealt(*[np.concatenate([getattr(d, f) for d in dealt]) for f in ("gid", "x", "nn")], {})
+    whole = R.expect(_dealt_cols(every, tp), [0], funcs)
+    assert not got.overflow and not whole.overflow and set(got.groups) == set(whole.groups)
+    for k, w in whole.groups.items():
+        for fi, (wv, gv) in enumerate(zip(w, got.groups[k])):
+            if isinstance(wv, frozenset):
+                assert gv <= wv, (k, fi)
+            else:
+                assert gv == wv, (k, fi, wv, gv)
+
+
+def test_expect_names_the_groups_past_the_limit():
+    """expect's per-group overflow set holds exactly the out_by_one group, and expect_final finds the same over the dealt
+    partials; a part past the limit makes expect_partial raise on that rank only"""
+    rng = np.random.default_rng(91)
+    fam = R.limits(rng)
+    twin = R.out_by_one(fam, R.TWINS["min_minus_1"], rng)
+    g = twin.meta["group"]
+    key = R.key_column(twin.gid)
+    want = R.expect([key, Column(INT64, twin.x)], [0], [(SUM, 1)])
+    assert want.overflow and want.over == {(R.key_labels(key, [np.nonzero(twin.gid == g)[0][0]])[0],)}
+    dealt = R.deal(rng, twin, 3, rebuild=True)
+    chunks = [R.expect_partial([INT64, INT64], _dealt_cols(d), [0], [(SUM, 1)])[1] for d in dealt]
+    got = R.expect_final(R.Chunk.concat(chunks, [INT64, INT64]).cols, [1], [(SUM, 0, -1)])
+    assert got.over == want.over
+    dealt = R.deal(rng, fam, 3, rebuild=True, past=(_big_group(fam), 2))
+    for r, d in enumerate(dealt):
+        if r == 2:
+            with pytest.raises(OverflowError):
+                R.expect_partial([INT64, INT64], _dealt_cols(d), [0], [(SUM, 1)])
+        else:
+            R.expect_partial([INT64, INT64], _dealt_cols(d), [0], [(SUM, 1)])

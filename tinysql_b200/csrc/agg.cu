@@ -1526,33 +1526,17 @@ int32_t tq_agg_export_partial(tq_agg *a, tq_column *out_cols, int64_t *n_rows) {
   return TQ_OK;
 }
 
-// The GROUP BY push (both entry points): every argument is checked before anything is enqueued (a refused push writes no
-// region and publishes no slot); then the export (one host read of the group count, on the compute stream, which it also
-// drains), and on the push stream the destination of every partial row, the scatter into the regions and k_publish_counts.
-// var_ok: the handle may have var-len partial columns, whose cells travel in byte areas of byte_cap[v] bytes.
-static int32_t agg_push_body(tq_agg *a, const char *fn, bool var_ok, int32_t n_parts, void *const *dest_data, void *const *dest_counts,
-                             int64_t region_cap, const int64_t *byte_cap, int32_t slot, uint64_t epoch) {
-  if (!a) return TQ_ERR_INVALID_ARG;
-  TQ_TRY(ensure_init());
-  if (a->final_mode) { set_error("%s: a FinalMode handle takes partial rows, it does not make them", fn); return TQ_ERR_STATE; }
-  if (a->merge_mode_seen) { set_error("%s: the handle has merged partial rows; push from a handle fed raw rows", fn); return TQ_ERR_STATE; }
-  if (!var_ok && agg_has_varlen(a)) { set_error("partial export / merge with var-len columns is not supported"); return TQ_ERR_UNSUPPORTED_TYPE; }
-  const int w = partial_width(a), nw = w + 1;
-  if (nw > 64) { set_error("%s: %d partial columns and the mask word exceed 64 words per row", fn, w); return TQ_ERR_INVALID_ARG; }
-  int src[64];
-  const int n_var = partial_var_src(a, src);
-  if (n_var > REGION_MAXV) { set_error("%s: %d var-len partial columns, at most %d", fn, n_var, REGION_MAXV); return TQ_ERR_INVALID_ARG; }
-  if (n_var && !byte_cap) { set_error("%s: %d var-len partial columns need byte_cap", fn, n_var); return TQ_ERR_INVALID_ARG; }
-  for (int v = 0; v < n_var; v++)
-    if (byte_cap[v] < 1 || byte_cap[v] > 0xFFFFFFF0ll) { set_error("%s: byte_cap[%d] = %lld: 1 <= byte_cap < 2^32", fn, v, (long long)byte_cap[v]); return TQ_ERR_INVALID_ARG; }
-  TQ_TRY(push_check_dests(fn, n_parts, nw + n_var, dest_data, dest_counts, region_cap, slot));
-  Runtime &r = rt();
-  std::lock_guard<std::recursive_mutex> lk(r.mu);
+// What the GROUP BY push does once its arguments are checked (caller holds the runtime lock): the export (one host read of the
+// group count, on the compute stream, which it also drains), and on the push stream s the destination of every partial row, the
+// scatter into the regions and k_publish_counts.
+static int32_t agg_push_rows(tq_agg *a, const char *fn, int w, int n_var, const int *src, int32_t n_parts, void *const *dest_data,
+                             void *const *dest_counts, int64_t region_cap, const int64_t *byte_cap, int32_t slot, uint64_t epoch,
+                             cudaStream_t s) {
+  const int nw = w + 1;
   if (!a->eof) TQ_TRY(tq_agg_eof(a));
   TQ_TRY(agg_finalize(a, true, a->result, w));   // synchronises the compute stream: the partial rows are complete
   const int64_t n = a->result.n;
   if (n > 0xFFFFFFF0ll) { set_error("%s: %lld partial rows", fn, (long long)n); return TQ_ERR_INVALID_ARG; }
-  cudaStream_t s = r.h2d;   // the push stream, as tq_partition_push_regions
   PushSlot *ps = nullptr;
   TQ_TRY(push_begin(slot, n_parts, dest_counts, nullptr, s, &ps));
   if (n > 0) {
@@ -1582,6 +1566,35 @@ static int32_t agg_push_body(tq_agg *a, const char *fn, bool var_ok, int32_t n_p
                                   ps->cursor.as<uint32_t>(), ps->ovf.as<unsigned long long>(), ps->region, s));
   }
   return push_publish(*ps, n_parts, epoch, s);
+}
+
+// The GROUP BY push (both entry points): every argument is checked before anything is enqueued (a refused push writes no
+// region and publishes no slot); then agg_push_rows.  Any failure after the checks (a partial total past int64 in the export,
+// too many partial rows, a failed reserve) still publishes, PUSH_FAILED | status in every destination's slot under `epoch`, so
+// every receiver refuses the step instead of waiting for this source or merging an older count.
+// var_ok: the handle may have var-len partial columns, whose cells travel in byte areas of byte_cap[v] bytes.
+static int32_t agg_push_body(tq_agg *a, const char *fn, bool var_ok, int32_t n_parts, void *const *dest_data, void *const *dest_counts,
+                             int64_t region_cap, const int64_t *byte_cap, int32_t slot, uint64_t epoch) {
+  if (!a) return TQ_ERR_INVALID_ARG;
+  TQ_TRY(ensure_init());
+  if (a->final_mode) { set_error("%s: a FinalMode handle takes partial rows, it does not make them", fn); return TQ_ERR_STATE; }
+  if (a->merge_mode_seen) { set_error("%s: the handle has merged partial rows; push from a handle fed raw rows", fn); return TQ_ERR_STATE; }
+  if (!var_ok && agg_has_varlen(a)) { set_error("partial export / merge with var-len columns is not supported"); return TQ_ERR_UNSUPPORTED_TYPE; }
+  const int w = partial_width(a), nw = w + 1;
+  if (nw > 64) { set_error("%s: %d partial columns and the mask word exceed 64 words per row", fn, w); return TQ_ERR_INVALID_ARG; }
+  int src[64];
+  const int n_var = partial_var_src(a, src);
+  if (n_var > REGION_MAXV) { set_error("%s: %d var-len partial columns, at most %d", fn, n_var, REGION_MAXV); return TQ_ERR_INVALID_ARG; }
+  if (n_var && !byte_cap) { set_error("%s: %d var-len partial columns need byte_cap", fn, n_var); return TQ_ERR_INVALID_ARG; }
+  for (int v = 0; v < n_var; v++)
+    if (byte_cap[v] < 1 || byte_cap[v] > 0xFFFFFFF0ll) { set_error("%s: byte_cap[%d] = %lld: 1 <= byte_cap < 2^32", fn, v, (long long)byte_cap[v]); return TQ_ERR_INVALID_ARG; }
+  TQ_TRY(push_check_dests(fn, n_parts, nw + n_var, dest_data, dest_counts, region_cap, slot));
+  Runtime &r = rt();
+  std::lock_guard<std::recursive_mutex> lk(r.mu);
+  cudaStream_t s = r.h2d;   // the push stream, as tq_partition_push_regions
+  const int32_t st = agg_push_rows(a, fn, w, n_var, src, n_parts, dest_data, dest_counts, region_cap, byte_cap, slot, epoch, s);
+  if (st != TQ_OK) push_publish_failure(slot, n_parts, dest_counts, st, epoch, s);   // every destination refuses this step
+  return st;
 }
 
 // The GROUP BY receive (both entry points): one host read of the slots (queued behind tq_region_wait on the compute stream),
@@ -1616,6 +1629,11 @@ static int32_t agg_merge_body(tq_agg *a, const char *fn, bool var_ok, int32_t n_
   const unsigned long long *sl = a->region_slots.as<unsigned long long>();
   int64_t rows[8], most = 0;
   for (int g = 0; g < n_regions; g++) {
+    if (push_failed(sl[2 * g])) {   // the source failed after its checks: this step has no complete set of partial rows
+      const int32_t st = (int32_t)(uint32_t)sl[2 * g];
+      set_error("%s: source %d failed its push with status %d, so no destination can finish this step", fn, g, st);
+      return st;
+    }
     if (sl[2 * g] > (unsigned long long)region_cap) {
       set_error("%s: a region overflowed (its slot reads more than %lld rows)", fn, (long long)region_cap);
       return TQ_ERR_OOM;

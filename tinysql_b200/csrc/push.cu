@@ -17,6 +17,18 @@ __global__ void k_publish_counts(const uint32_t *cursor, const unsigned long lon
   }
 }
 
+// A push that failed after its arguments were checked: every slot gets {PUSH_FAILED | status, epoch}, in the same order and
+// with the same fence as k_publish_counts, so that no receiver waits for a count that will never come.
+__global__ void k_publish_failure(int n_parts, unsigned long long *const *dest_slots, unsigned long long word, unsigned long long epoch) {
+  const int q = threadIdx.x;
+  if (q < n_parts) {
+    volatile unsigned long long *slot = dest_slots[q];
+    slot[0] = word;
+    __threadfence_system();
+    slot[1] = epoch;
+  }
+}
+
 // Device-side wait for the peers: spins (bounded: ~4 s) until the n slots of this rank's table carry `epoch`.  Enqueued on the
 // compute stream in front of the kernels that read the regions, so the exchange needs no host barrier.
 __global__ void k_region_wait(const unsigned long long *slots, int n, unsigned long long epoch, unsigned *timed_out) {
@@ -73,6 +85,17 @@ int32_t push_publish(PushSlot &ps, int n_pub, uint64_t epoch, cudaStream_t s) {
   count_launch();
   TQ_TRY(check_launch("k_publish_counts"));
   TQ_CUDA(cudaEventRecord(ps.ev, s));
+  return TQ_OK;
+}
+
+int32_t push_publish_failure(int slot, int n_parts, void *const *dest_counts, int32_t status, uint64_t epoch, cudaStream_t s) {
+  PushSlot *ps = nullptr;
+  TQ_TRY(push_begin(slot, n_parts, dest_counts, nullptr, s, &ps));
+  TQ_CUDA(cudaMemcpyAsync(ps->counts_ptrs.p, ps->h_ptrs.p, 128, cudaMemcpyHostToDevice, s));
+  k_publish_failure<<<1, 32, 0, s>>>(n_parts, ps->counts_ptrs.as<unsigned long long *>(), PUSH_FAILED | (uint32_t)status, epoch);
+  count_launch();
+  TQ_TRY(check_launch("k_publish_failure"));
+  TQ_CUDA(cudaEventRecord(ps->ev, s));
   return TQ_OK;
 }
 

@@ -33,4 +33,12 @@ int32_t push_begin(int slot, int n_parts, void *const *dest_counts, void *extra_
 // the n_pub count-slot pointers of ps.h_ptrs to the device, and records ps.ev.
 int32_t push_publish(PushSlot &ps, int n_pub, uint64_t epoch, cudaStream_t s);
 
+// The rows word of a slot whose source failed after its arguments were checked: PUSH_FAILED | the status it returned.  Above
+// every region cap, like ~0 (a region overflow), so a reader that only checks the cap refuses it too.
+static constexpr uint64_t PUSH_FAILED = 0xFFFFFFFF00000000ull;
+static inline bool push_failed(uint64_t rows) { return rows != ~0ull && (rows & PUSH_FAILED) == PUSH_FAILED; }
+// Slot `slot` set up as push_begin does, then every count slot dest_counts[q] (q < n_parts) gets {PUSH_FAILED | status, epoch}
+// on s, and ps.ev is recorded.  Writes no region.
+int32_t push_publish_failure(int slot, int n_parts, void *const *dest_counts, int32_t status, uint64_t epoch, cudaStream_t s);
+
 }  // namespace tq

@@ -1052,7 +1052,9 @@ class RegionAgg:
 
     def step(self, cols, bitmaps=None, keep_result=False):
         """one step on this rank: push, wait, merge, finish, then one barrier.  cols / bitmaps as push().  Returns (groups
-        finished on this rank, result) as finish()."""
+        finished on this rank, result) as finish().  A step that fails on any rank raises on this one too when the failure
+        reaches it (a push that fails after its checks makes every merge refuse the step); the barrier is passed either way, so
+        the ranks leave a failed step together and the next step runs as usual."""
         self.rx.next_epoch()
         try:
             self.push(cols, bitmaps)
@@ -1062,7 +1064,7 @@ class RegionAgg:
                 self.lib.tq_partition_push_sync(self.slot)
                 self.lib.tq_agg_destroy(self._hp)
                 self._hp = None
-        dist.barrier()
+            dist.barrier()
         return res
 
 
