@@ -587,6 +587,14 @@ int32_t tq_sort_next_bytes(tq_sort *s, int64_t max_rows, int64_t *bytes_per_col)
 int32_t tq_sort_next(tq_sort *s, int64_t max_rows, tq_column *out_cols, int64_t *n_rows, int32_t *eof);
 /* device-chunk handles: the whole result at once as DEVICE columns, lent until tq_sort_destroy; then eof */
 int32_t tq_sort_next_device(tq_sort *s, tq_column *out_cols, int64_t *n_rows, int32_t *eof);
+/* The receiving side of the multi-GPU ORDER BY (tq_partition_push_ranges): puts the n_regions (1..8) regions that arrived on
+ * this rank, in source order, each as one device chunk.  Queue tq_region_wait first; slots = the n_regions consecutive
+ * {u64 rows, u64 epoch} slots, read once on the host.  regions[g * (n_cols + 1) + c] = wire column c of region g: an 8-byte
+ * column's values in .data; a BYTES column's offsets area (rows + 1 offsets from 0) in .offsets and its byte area in .data;
+ * the mask word (bit c = column c is NOT NULL) at c = n_cols, in .data.  A slot past region_cap (~0: an overflowed push) is
+ * TQ_ERR_OOM and a source that failed its push returns that push's status; either way nothing is put.  FLOAT32 columns are
+ * TQ_ERR_UNSUPPORTED_TYPE (the push carries none).  After it, tq_sort_eof and tq_sort_next_device run as for any device put. */
+int32_t tq_sort_put_regions(tq_sort *s, int32_t n_regions, const void *slots, int64_t region_cap, const tq_column *regions);
 /* [0] rows sorted, [1] device time of the sort phase in ns (CUDA events; upload and result gather excluded),
  * [2] kernel launches of tq_sort_eof, [3] radix digit passes that ran (constant digits are skipped) */
 int32_t tq_sort_stats(tq_sort *s, int64_t *stats4);
@@ -708,6 +716,38 @@ int32_t tq_partition_push_regions(int32_t n_cols, const tq_column *cols, int32_t
 int32_t tq_partition_push_broadcast(int32_t n_cols, const tq_column *cols, const int32_t *types, int32_t nullable, int64_t n, int32_t n_parts,
                                     void *const *dest_data, void *const *dest_counts, int64_t region_cap, const int64_t *byte_cap, int32_t slot,
                                     uint64_t epoch);
+/* The two pushes of the multi-GPU ORDER BY (dist.RegionSort): rank src_rank routes each row of its shard to the rank whose
+ * slice of the global order holds it.  The routing order is the ByItems' order followed by one more, ascending, word per
+ * row, the tie word (src_rank << 32) | row: a total order that agrees with the rank-major stable sort, so a run of equal
+ * keys may be split between ranks anywhere.  Both take 1..63 columns of TQ_TYPE_INT64, _UINT64, _FLOAT64 or _BYTES (any
+ * other type, FLOAT32 included, is TQ_ERR_UNSUPPORTED_TYPE), device memory, offsets exactly on the BYTES columns (they may
+ * start anywhere, as for a TQ_MEM_DEVICE put), NULL bitmaps where a column has NULLs; 0..8 ByItems by_cols[i] (Desc
+ * by_desc[i]: NULL first ascending, last descending, as tq_sort); 0 <= n < 2^32, src_rank >= 0; byte_cap[c], for each BYTES
+ * column c, the byte area of its cells per region, 1 <= byte_cap[c] < 2^32.  Every argument is checked before anything is
+ * enqueued: a refused push writes no region and publishes no slot.  A failure after the checks publishes that status in
+ * every slot, so every receiver refuses the step.  Both are enqueued on the push stream; tq_partition_push_sync(slot)
+ * waits for them.
+ * tq_partition_push_sample: the splitter sample.  m = min(n, n_samples) rows (1 <= n_samples <= 65536), row j taken at a
+ *   hashed position of (seed, src_rank, j) inside the stratum [j n / m, (j + 1) n / m) — distinct rows, and no aliasing
+ *   with a periodic input.  Their ByItem columns and their tie word (UINT64) are broadcast to the n_parts destinations in
+ *   tq_partition_push_broadcast's wire format with n_by + 1 columns (the nullable flag, byte_cap of each BYTES ByItem
+ *   column); m <= region_cap.  Each received sample region is a device chunk for tq_sort_put (TQ_MEM_DEVICE).
+ * tq_partition_push_ranges: the rows.  split_cols = the sorted sample's n_by + 1 device columns (ByItems, then the tie
+ *   word), split_rows its rows, split_pos the n_parts - 1 non-decreasing splitter rows; row r goes to the number of
+ *   splitters at or below it, comparing the sort's own key words most significant first (per ByItem the NULL flag, then the
+ *   value word or the 8-byte big-endian chunks and the length of a string, each inverted when Desc; the tie word last).
+ *   n_parts == 1 or split_rows == 0 reads no splitter and sends every row to destination 0.  The rows go out in the GROUP BY
+ *   push's wire format, in input order per destination: dest_data[q * (n_cols + 1 + n_bytes) + a] = n_cols word areas (a
+ *   BYTES column's is its region_cap + 1 offsets from 0), the mask word, then the byte area of each BYTES column in column
+ *   order.  n <= region_cap, so no region overflows on rows; a byte area past its cap makes every slot read ~0.  The
+ *   receiver is tq_sort_put_regions. */
+int32_t tq_partition_push_sample(int32_t n_cols, const tq_column *cols, const int32_t *types, int64_t n, int32_t n_by, const int32_t *by_cols,
+                                 int32_t nullable, int32_t src_rank, int32_t n_samples, uint64_t seed, int32_t n_parts, void *const *dest_data,
+                                 void *const *dest_counts, int64_t region_cap, const int64_t *byte_cap, int32_t slot, uint64_t epoch);
+int32_t tq_partition_push_ranges(int32_t n_cols, const tq_column *cols, const int32_t *types, int64_t n, int32_t n_by, const int32_t *by_cols,
+                                 const int32_t *by_desc, int32_t src_rank, int32_t n_parts, const tq_column *split_cols, int64_t split_rows,
+                                 const int64_t *split_pos, void *const *dest_data, void *const *dest_counts, int64_t region_cap,
+                                 const int64_t *byte_cap, int32_t slot, uint64_t epoch);
 int32_t tq_partition_push_sync(int32_t slot);
 /* Enqueues, on the compute stream, a kernel that waits (bounded) until the n_sources consecutive slots at `slots` (this rank's
  * own table) carry `epoch` — the device-side barrier between the peers' pushes and the kernels that read the regions; no host

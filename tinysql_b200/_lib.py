@@ -134,6 +134,7 @@ SYMBOLS = {
     "tq_sort_next_bytes": (_I32, [_P, _I64, C.POINTER(_I64)]),
     "tq_sort_next": (_I32, [_P, _I64, _COL, C.POINTER(_I64), C.POINTER(_I32)]),
     "tq_sort_next_device": (_I32, [_P, _COL, C.POINTER(_I64), C.POINTER(_I32)]),
+    "tq_sort_put_regions": (_I32, [_P, _I32, _P, _I64, _COL]),
     "tq_sort_stats": (_I32, [_P, C.POINTER(_I64)]),
     "tq_sort_destroy": (_I32, [_P]),
     "tq_mjoin_create": (_I32, [C.POINTER(TQMJoinDesc), C.POINTER(_P)]),
@@ -154,6 +155,10 @@ SYMBOLS = {
                                          _I64, _I32, C.c_uint64]),
     "tq_partition_push_broadcast": (_I32, [_I32, _COL, C.POINTER(_I32), _I32, _I64, _I32, C.POINTER(_P), C.POINTER(_P), _I64, C.POINTER(_I64),
                                            _I32, C.c_uint64]),
+    "tq_partition_push_sample": (_I32, [_I32, _COL, C.POINTER(_I32), _I64, _I32, C.POINTER(_I32), _I32, _I32, _I32, C.c_uint64, _I32,
+                                        C.POINTER(_P), C.POINTER(_P), _I64, C.POINTER(_I64), _I32, C.c_uint64]),
+    "tq_partition_push_ranges": (_I32, [_I32, _COL, C.POINTER(_I32), _I64, _I32, C.POINTER(_I32), C.POINTER(_I32), _I32, _I32, _COL, _I64,
+                                        C.POINTER(_I64), C.POINTER(_P), C.POINTER(_P), _I64, C.POINTER(_I64), _I32, C.c_uint64]),
     "tq_region_wait": (_I32, [_P, _I32, C.c_uint64]),
     "tq_region_gather": (_I32, [_I32, _P, _I64, _I32, _I32, _COL, _COL, _I64, C.POINTER(_I64)]),
     "tq_partition_push_sync": (_I32, [_I32]),

@@ -7,7 +7,10 @@
 // And the GROUP BY push's kernels (tq_agg_push_partial): the destination of a partial row from its group, the same histogram /
 // scan / scatter writing each destination's run column-wise into that destination's region with the mask word packed on the
 // way, and the mask word's expansion into NULL bitmaps on the receiving side.
+// And the ORDER BY range push's kernels (tq_partition_push_sample / _ranges): the sample gather and the destination of a row
+// from the sorted sample's splitters, on the sort's own key words (sortkey.cuh).
 #include "scatter.cuh"
+#include "sortkey.cuh"
 
 namespace tq {
 
@@ -44,8 +47,6 @@ struct PartParams {
   }
 };
 
-static constexpr int REGION_MAXW = 63;  // wire columns before the mask word: the mask's 64 bits cover them
-
 struct RegionParams {
   int n_cols;  // wire columns before the mask word
   int n_parts;
@@ -76,11 +77,16 @@ struct RegionParams {
     }
     o[n_cols][pos] = m;
   }
+  // the arena id of row r's cell in var-len column v: its id word, or r itself for a column without ids (a device column
+  // whose offsets are the arena, as the range push sends one)
+  __device__ __forceinline__ uint64_t cell_id(int v, int64_t r) const {
+    const DCol &c = in[var[v].col];
+    return c.data ? c.data[r] : (uint64_t)r;
+  }
   // bytes of row r's cell in var-len column v (0 for NULL)
   __device__ __forceinline__ uint64_t cell_len(int v, int64_t r) const {
-    const DCol &c = in[var[v].col];
-    if (!tqd::bm_not_null(c.bm, r)) return 0;
-    const uint64_t id = c.data[r];
+    if (!tqd::bm_not_null(in[var[v].col].bm, r)) return 0;
+    const uint64_t id = cell_id(v, r);
     return (uint64_t)(var[v].off[id + 1] - var[v].off[id]);
   }
 };
@@ -556,7 +562,7 @@ __global__ void __launch_bounds__(256) k_region_scatter_var(const RegionParams p
         uint64_t *const *o = p.out + (int64_t)part * p.n_areas;
         o[p.var[v].col][pos + 1] = (uint64_t)bpos + len;
         dst = (unsigned long long)(reinterpret_cast<uint8_t *>(o[p.n_cols + 1 + v]) + bpos);
-        if (len) src = (unsigned long long)(p.var[v].bytes + p.var[v].off[p.in[p.var[v].col].data[r]]);
+        if (len) src = (unsigned long long)(p.var[v].bytes + p.var[v].off[p.cell_id(v, r)]);
       }
       const unsigned todo = __ballot_sync(0xffffffffu, fits && len > 0);
       for (int j = 0; j < 32; j++) {
@@ -632,6 +638,177 @@ int32_t scatter_to_regions_var(const DCol *cols, int n_cols, const RegionVar *va
   TQ_LAUNCH(k_region_scatter_var, blocks, 256, 0, s, p);
   count_launch(2);
   return check_launch("k_region_scatter_var");
+}
+
+// ---- the range push of the multi-GPU ORDER BY (tq_partition_push_sample / _ranges, push.cu): the sample of a shard, and the
+// destination of a row from the sorted sample's splitters, compared on the sort's own key words (sortkey.cuh)
+
+struct SampleParams {
+  int n_by;
+  RangeBy by[RANGE_MAX_BY];
+  SampleOut out;
+  int64_t n, m;
+  uint64_t seed;
+  int src_rank;
+};
+
+// One CTA walks the m samples 256 at a time (a warp = 32 consecutive samples: one ballot = one bitmap word): positions, values,
+// bits and tie words; cell lengths into the offsets, scanned in place by the block; then the cells, when they fit.
+__global__ void __launch_bounds__(256) k_sample_gather(const SampleParams p) {
+  __shared__ uint64_t s_scan[256];
+  __shared__ uint64_t s_carry;
+  const int lane = threadIdx.x & 31;
+  const int64_t padded = (p.m + 255) & ~255ll;
+  for (int64_t j = threadIdx.x; j < padded; j += 256) {
+    const bool live = j < p.m;
+    const uint64_t pos = live ? range_sample_pos(p.seed, p.src_rank, j, p.n, p.m) : 0;
+    if (live) p.out.tie[j] = range_tie(p.src_rank, pos);
+    for (int b = 0; b < p.n_by; b++) {
+      const RangeBy &c = p.by[b];
+      const bool nn = live && tqd::bm_not_null(c.bm, (int64_t)pos);
+      if (live && c.type != TQ_TYPE_BYTES) p.out.data[b][j] = c.data[pos];
+      if (live && c.type == TQ_TYPE_BYTES) p.out.off[b][j + 1] = nn ? c.off[pos + 1] - c.off[pos] : 0;   // lengths, scanned below
+      if (p.out.bm[b]) {
+        const unsigned w = __ballot_sync(0xffffffffu, nn);
+        if (lane == 0) p.out.bm[b][j >> 5] = w;
+      }
+    }
+  }
+  for (int b = 0; b < p.n_by; b++) {
+    if (p.by[b].type != TQ_TYPE_BYTES) continue;
+    int64_t *off = p.out.off[b];
+    if (threadIdx.x == 0) { off[0] = 0; s_carry = 0; }
+    __syncthreads();
+    for (int64_t j0 = 0; j0 < p.m; j0 += 256) {   // inclusive scan of off[1..m], 256 entries per round
+      const int64_t j = j0 + threadIdx.x;
+      uint64_t v = j < p.m ? (uint64_t)off[j + 1] : 0;
+      s_scan[threadIdx.x] = v;
+      __syncthreads();
+      for (int d = 1; d < 256; d <<= 1) {
+        const uint64_t add = threadIdx.x >= (unsigned)d ? s_scan[threadIdx.x - d] : 0;
+        __syncthreads();
+        v += add;
+        s_scan[threadIdx.x] = v;
+        __syncthreads();
+      }
+      if (j < p.m) off[j + 1] = (int64_t)(s_carry + v);
+      __syncthreads();
+      if (threadIdx.x == 255) s_carry += v;
+      __syncthreads();
+    }
+    if ((uint64_t)off[p.m] > p.out.byte_cap[b]) continue;   // the broadcast finds the same total and publishes the overflow
+    for (int64_t j = threadIdx.x; j < p.m; j += 256) {
+      const uint64_t pos = range_sample_pos(p.seed, p.src_rank, j, p.n, p.m);
+      const int64_t len = off[j + 1] - off[j];
+      const uint8_t *src = p.by[b].bytes + (len ? p.by[b].off[pos] : 0);
+      for (int64_t k = 0; k < len; k++) p.out.bytes[b][off[j] + k] = src[k];
+    }
+  }
+}
+
+int32_t sample_rows(const RangeBy *by, int n_by, int64_t n, int64_t m, uint64_t seed, int src_rank, const SampleOut &out, cudaStream_t s) {
+  if (n_by < 0 || n_by > RANGE_MAX_BY || m < 1 || m > RANGE_MAX_SAMPLES || m > n || n > 0xFFFFFFF0ll) { set_error("internal: sample_rows arguments"); return TQ_ERR_INVALID_ARG; }
+  SampleParams p{};
+  p.n_by = n_by;
+  for (int b = 0; b < n_by; b++) p.by[b] = by[b];
+  p.out = out;
+  p.n = n;
+  p.m = m;
+  p.seed = seed;
+  p.src_rank = src_rank;
+  TQ_LAUNCH(k_sample_gather, 1, 256, 0, s, p);
+  count_launch();
+  return check_launch("k_sample_gather");
+}
+
+struct RangeParams {
+  int n_by, n_split, src_rank;
+  RangeBy row[RANGE_MAX_BY], spl[RANGE_MAX_BY];
+  const uint64_t *spl_tie;
+  uint32_t pos[7];
+  int64_t n;
+  uint8_t *dest;
+};
+
+__device__ __forceinline__ KeySrc range_key(const RangeBy &c, int mode, int word) {
+  KeySrc k{};
+  k.mode = mode;
+  k.type = c.type;
+  k.word = word;
+  k.desc = c.desc;
+  k.d8 = c.data;
+  k.off = c.off;
+  k.bytes = c.bytes;
+  k.base = 0;
+  k.bm = c.bm;
+  return k;
+}
+
+// -1 / 0 / +1: row r of the shard against splitter row s of the sorted sample, on the sort's key words most significant first
+// (per ByItem the NULL flag, then the value word or the string's chunks and length), then the tie words
+__device__ int range_cmp(const RangeParams &p, uint32_t r, uint32_t s) {
+  for (int b = 0; b < p.n_by; b++) {
+    const RangeBy &x = p.row[b], &y = p.spl[b];
+    uint64_t a = key_word(range_key(x, KS_NULL_FLAG, 0), r), c = key_word(range_key(y, KS_NULL_FLAG, 0), s);
+    if (a != c) return a < c ? -1 : 1;
+    if (x.type != TQ_TYPE_BYTES) {
+      a = key_word(range_key(x, KS_COL8, 0), r);
+      c = key_word(range_key(y, KS_COL8, 0), s);
+      if (a != c) return a < c ? -1 : 1;
+      continue;
+    }
+    const bool nn = tqd::bm_not_null(x.bm, r);   // equal flags: both NULL (every word 0 or ~0) or both NOT NULL
+    if (!nn) continue;
+    const int64_t lx = x.off[r + 1] - x.off[r], ly = y.off[s + 1] - y.off[s];
+    const int64_t chunks = ((lx > ly ? lx : ly) + 7) / 8;
+    for (int64_t w = 0; w < chunks; w++) {
+      a = key_word(range_key(x, KS_STR_CHUNK, (int)w), r);
+      c = key_word(range_key(y, KS_STR_CHUNK, (int)w), s);
+      if (a != c) return a < c ? -1 : 1;
+    }
+    a = key_word(range_key(x, KS_STR_LEN, 0), r);
+    c = key_word(range_key(y, KS_STR_LEN, 0), s);
+    if (a != c) return a < c ? -1 : 1;
+  }
+  const uint64_t t = range_tie(p.src_rank, r), u = p.spl_tie[s];
+  return t == u ? 0 : (t < u ? -1 : 1);
+}
+
+// dest[r] = the splitters at or below row r: a binary search over the n_split (<= 7) splitters
+__global__ void __launch_bounds__(256) k_range_dest(const RangeParams p) {
+  for (int64_t r = (int64_t)blockIdx.x * blockDim.x + threadIdx.x; r < p.n; r += (int64_t)gridDim.x * blockDim.x) {
+    int lo = 0, hi = p.n_split;
+    while (lo < hi) {
+      const int mid = (lo + hi) >> 1;
+      if (range_cmp(p, (uint32_t)r, p.pos[mid]) >= 0) lo = mid + 1;
+      else hi = mid;
+    }
+    p.dest[r] = (uint8_t)lo;
+  }
+}
+
+int32_t range_dest(const RangeBy *rows, const RangeBy *spl, int n_by, const uint64_t *spl_tie, const int64_t *pos, int n_split, int src_rank,
+                   int64_t n, uint8_t *dest, cudaStream_t s) {
+  if (n_by < 0 || n_by > RANGE_MAX_BY || n_split < 0 || n_split > 7 || n < 1 || n > 0xFFFFFFF0ll || (n_split && (!spl_tie || !pos))) {
+    set_error("internal: range_dest arguments");
+    return TQ_ERR_INVALID_ARG;
+  }
+  RangeParams p{};
+  p.n_by = n_by;
+  p.n_split = n_split;
+  p.src_rank = src_rank;
+  for (int b = 0; b < n_by; b++) {
+    p.row[b] = rows[b];
+    if (n_split) p.spl[b] = spl[b];
+  }
+  p.spl_tie = spl_tie;
+  for (int k = 0; k < n_split; k++) p.pos[k] = (uint32_t)pos[k];
+  p.n = n;
+  p.dest = dest;
+  const int64_t blocks = (n + 255) / 256, cap = (int64_t)rt().sm_count * 8;
+  TQ_LAUNCH(k_range_dest, (unsigned)(blocks < cap ? blocks : cap), 256, 0, s, p);
+  count_launch();
+  return check_launch("k_range_dest");
 }
 
 }  // namespace tq

@@ -1,5 +1,5 @@
-// push.cuh — what the region pushes share (push.cu): tq_partition_push_regions (join.cu), tq_agg_push_partial (agg.cu) and
-// tq_partition_push_broadcast (push.cu)
+// push.cuh — what the region pushes share (push.cu): tq_partition_push_regions (join.cu), tq_agg_push_partial (agg.cu),
+// tq_partition_push_broadcast, tq_partition_push_sample and tq_partition_push_ranges (push.cu)
 // check their destinations with push_check_dests, set up their slot with push_begin, scatter into per-source regions of the
 // peers' receive buffers on the push stream, then publish {rows, epoch} in each destination's slot with push_publish; the
 // receiver waits on those slots with tq_region_wait.  Where the regions and slots sit is the caller's (dist.RegionLayout).
@@ -14,7 +14,8 @@ static constexpr int PUSH_SLOTS = 16;
 // push of the same slot (and tq_partition_push_sync) waits on before it rewrites them.
 struct PushSlot {
   DevBuf cursor, lim, ovf, counts_ptrs, mask, sel;   // cursor: rows per destination (u32 x 16); ovf: u64, non-zero = overflow
-  DevBuf dest, out_ptrs;                             // the GROUP BY push: destination per row, the region pointer table
+  DevBuf dest, out_ptrs;                             // the GROUP BY and range pushes: destination per row, the region pointer table
+  DevBuf sample[RANGE_MAX_BY][3], sample_tie;        // the sample push: per ByItem its values or offsets, cells, bitmap words; tie words
   RegionScratch region;
   PinBuf h_lim, h_ptrs, h_out_ptrs;
   cudaEvent_t ev = nullptr;

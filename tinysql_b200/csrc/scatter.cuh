@@ -40,6 +40,7 @@ int32_t group_dest(const DCol *items, int n_items, uint32_t real_mask, int64_t n
 // dictionary's content hash of the cell, sd_warp_hash: the same bytes give the same word on every rank).
 int32_t group_dest(const DCol *items, const uint64_t *const *hashes, int n_items, uint32_t real_mask, int64_t n, int n_parts, uint8_t *dest,
                    cudaStream_t s);
+static constexpr int REGION_MAXW = 63;  // wire columns before the mask word: the mask's 64 bits cover them
 struct RegionScratch {
   DevBuf hist, scan, total;
   DevBuf bhist, bscan, btotal;   // var-len wire columns: cell bytes per (column, destination, chunk) and per (column, destination)
@@ -51,8 +52,9 @@ struct RegionScratch {
 int32_t scatter_to_regions(const DCol *cols, int n_cols, const uint8_t *dest, int64_t n, int n_parts, uint64_t *const *out, int64_t cap,
                            uint32_t *rows, unsigned long long *overflow, RegionScratch &sc, cudaStream_t s);
 // A var-len wire column of scatter_to_regions_var: column `col` holds ids into an arena of cells (id i = bytes
-// [off[i], off[i + 1]) of `bytes`); on the wire its area is the region's cap + 1 offsets and its cells go to a byte area of
-// byte_cap bytes.
+// [off[i], off[i + 1]) of `bytes`); a column whose DCol has no data is its own arena (row r's id is r: a device BYTES column,
+// whose offsets may start anywhere).  On the wire its area is the region's cap + 1 offsets and its cells go to a byte area
+// of byte_cap bytes.
 static constexpr int REGION_MAXV = 16;
 struct RegionVar {
   int col;
@@ -87,5 +89,47 @@ inline int broadcast_wire_areas(int n_cols, const int32_t *types, int nullable) 
 // then no destination gets that column's cells.  One launch, enqueued on s.
 int32_t broadcast_rows(int n_cols, const tq_column *cols, const int32_t *types, int nullable, int64_t n, int n_parts, void *const *dest_data,
                        const int64_t *byte_cap, uint32_t *rows, unsigned long long *overflow, cudaStream_t s);
+
+// ---- the range push of the multi-GPU ORDER BY (partition.cu; tq_partition_push_sample / _ranges in push.cu)
+// A ByItem of the range routing: an INT64 / UINT64 / FLOAT64 column (data) or a BYTES column (offsets into data, which may
+// start anywhere), its NOT-NULL bitmap or null, and its Desc flag.
+static constexpr int RANGE_MAX_BY = 8;
+static constexpr int RANGE_MAX_SAMPLES = 1 << 16;
+struct RangeBy {
+  int type, desc;
+  const uint64_t *data;
+  const int64_t *off;
+  const uint8_t *bytes;
+  const uint32_t *bm;
+};
+// The tie word of row r of rank src_rank's shard: the last, ascending ByItem of the routing order, which makes it a total
+// order that agrees with the global (rank-major, stable) sort order.
+__host__ __device__ __forceinline__ uint64_t range_tie(int src_rank, uint64_t r) { return ((uint64_t)src_rank << 32) | r; }
+// Row j (0 <= j < m = min(n, n_samples)) of the sample of a shard of n rows: a hashed position inside stratum
+// [j n / m, (j + 1) n / m), so the m positions are distinct (the sampled cells never exceed the shard's) and a periodic input
+// does not alias with the strata.
+__host__ __device__ __forceinline__ uint64_t range_sample_pos(uint64_t seed, int src_rank, int64_t j, int64_t n, int64_t m) {
+  const int64_t lo = (int64_t)((uint64_t)j * (uint64_t)n / (uint64_t)m);          // < 2^16 x 2^32: no overflow
+  const int64_t hi = (int64_t)((uint64_t)(j + 1) * (uint64_t)n / (uint64_t)m);
+  return (uint64_t)lo + tqd::mix64(seed ^ tqd::mix64(range_tie(src_rank, (uint64_t)j))) % (uint64_t)(hi - lo);
+}
+// The sample of a shard: for each sampled row j, every ByItem's value — out[b] = m words for an 8-byte item; for BYTES
+// out_off[b] = m + 1 offsets from 0 and out_bytes[b] its cells, which are written only when they fit byte_cap[b] — its
+// NOT-NULL bit (out_bm[b], 64-row words, written when the item has a bitmap) and its tie word (tie).  One CTA, enqueued on s;
+// 1 <= m <= RANGE_MAX_SAMPLES.
+struct SampleOut {
+  uint64_t *data[RANGE_MAX_BY];
+  int64_t *off[RANGE_MAX_BY];
+  uint8_t *bytes[RANGE_MAX_BY];
+  uint32_t *bm[RANGE_MAX_BY];
+  uint64_t byte_cap[RANGE_MAX_BY];
+  uint64_t *tie;
+};
+int32_t sample_rows(const RangeBy *by, int n_by, int64_t n, int64_t m, uint64_t seed, int src_rank, const SampleOut &out, cudaStream_t s);
+// dest[r] for the n >= 1 rows of rank src_rank's shard: the number of splitters at or below (row r, its tie word) in the
+// routing order.  The splitters are rows pos[0..n_split) (non-decreasing) of the sorted sample: its ByItem columns spl[] and
+// its tie words spl_tie.  n_split = 0 sends every row to 0.  Enqueued on s.
+int32_t range_dest(const RangeBy *rows, const RangeBy *spl, int n_by, const uint64_t *spl_tie, const int64_t *pos, int n_split, int src_rank,
+                   int64_t n, uint8_t *dest, cudaStream_t s);
 
 }  // namespace tq

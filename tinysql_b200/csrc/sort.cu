@@ -28,6 +28,8 @@
 
 #include "common.cuh"
 #include "expr_prog.cuh"
+#include "push.cuh"
+#include "sortkey.cuh"
 #include "varlen.cuh"
 
 using namespace tq;
@@ -162,56 +164,7 @@ int grid_for(int64_t n) {
 }
 
 // ------------------------------------------------------------------------------------------------ order-preserving words
-// types.CompareInt64 / CompareUint64 / CompareFloat64 (types/compare.go) as unsigned comparisons of one word
-__device__ __forceinline__ uint64_t enc_word(uint64_t v, int type) {
-  if (type == TQ_TYPE_INT64) return v ^ 0x8000000000000000ull;
-  if (type == TQ_TYPE_FLOAT64) {
-    if ((v << 1) == 0) return 0x8000000000000000ull;          // -0.0 == +0.0
-    return (v >> 63) ? ~v : (v | 0x8000000000000000ull);
-  }
-  return v;  // BIGINT UNSIGNED
-}
-
-enum { KS_COL8 = 0, KS_F32 = 1, KS_STR_CHUNK = 2, KS_STR_LEN = 3, KS_NULL_FLAG = 4, KS_MIX_CLASS = 5, KS_MIX_VALUE = 6 };
-struct KeySrc {
-  int mode;             // KS_*
-  int type;             // KS_COL8 / KS_MIX_*: TQ_TYPE_* of the column
-  int word;             // KS_STR_CHUNK: which 8-byte chunk of the cell
-  int desc;             // ByItems.Desc: the word is inverted
-  const uint64_t *d8;   // 8-byte slots
-  const uint32_t *d4;   // FLOAT slots
-  const int64_t *off;   // var-len: offsets[n + 1] (relative to `base`) and bytes
-  const uint8_t *bytes;
-  int64_t base;
-  const uint32_t *bm;   // NOT-NULL bitmap or nullptr
-};
-
-__device__ __forceinline__ uint64_t key_word(const KeySrc &k, uint32_t r) {
-  const bool nn = tqd::bm_not_null(k.bm, r);
-  uint64_t w = 0;
-  switch (k.mode) {
-    case KS_COL8: if (nn) w = enc_word(k.d8[r], k.type); break;
-    case KS_F32: if (nn) w = enc_word((uint64_t)__double_as_longlong((double)__uint_as_float(k.d4[r])), TQ_TYPE_FLOAT64); break;
-    case KS_STR_CHUNK:
-      if (nn) {
-        const int64_t s0 = k.off[r] - k.base, len = k.off[r + 1] - k.off[r];
-        const int64_t b0 = (int64_t)k.word * 8;
-#pragma unroll
-        for (int j = 0; j < 8; j++) w = (w << 8) | (uint64_t)((b0 + j < len) ? k.bytes[s0 + b0 + j] : 0);
-      }
-      break;
-    case KS_STR_LEN: if (nn) w = (uint64_t)(k.off[r + 1] - k.off[r]); break;
-    case KS_NULL_FLAG: w = nn ? 1 : 0; break;
-    // a BIGINT compared with a BIGINT UNSIGNED (types.CompareInt with mixed flags): (class, value) pairs order and
-    // equate the two domains exactly — negative < [0, 2^63) < unsigned >= 2^63
-    case KS_MIX_CLASS:
-      if (nn) { const uint64_t v = k.d8[r]; w = (k.type == TQ_TYPE_INT64) ? ((v >> 63) ? 0 : 1) : ((v >> 63) ? 2 : 1); }
-      break;
-    default: if (nn) w = k.d8[r]; break;   // KS_MIX_VALUE: inside a class the raw two's-complement word orders both domains
-  }
-  return k.desc ? ~w : w;
-}
-
+// enc_word / KeySrc / key_word: sortkey.cuh (the range push routes rows by the same words)
 __global__ void __launch_bounds__(256) k_sort_keys(const KeySrc k, const uint32_t *__restrict__ perm, int64_t n, uint64_t *__restrict__ keys) {
   const int64_t stride = (int64_t)gridDim.x * blockDim.x;
   for (int64_t i = (int64_t)blockIdx.x * blockDim.x + threadIdx.x; i < n; i += stride) keys[i] = key_word(k, perm ? perm[i] : (uint32_t)i);
@@ -898,6 +851,7 @@ struct tq_sort {
   DevBuf keep_rows;            // device-chunk handles: row ids of the result window, kept for the lazy gathers
   ResultDev dev;
   int64_t launches = 0, passes = 0, sort_ns = 0;   // tq_sort_stats
+  std::vector<DevBuf> region_bm;                   // tq_sort_put_regions: a region's mask words expanded into NOT-NULL bitmaps
 };
 
 struct tq_mjoin {
@@ -954,6 +908,69 @@ int32_t tq_sort_put(tq_sort *h, const tq_column *cols, int32_t mem) {
   }
   if (mem != TQ_MEM_HOST) return TQ_ERR_INVALID_ARG;
   return h->rows.append(cols);
+}
+
+// The receiving side of the range push (tq_partition_push_ranges): one host read of the slots, then each source's region in
+// source order as one device chunk — its words as values, its mask word expanded into NOT-NULL bitmaps, a BYTES column's
+// offsets and byte area as a var-len device column (append_cells_device).
+int32_t tq_sort_put_regions(tq_sort *h, int32_t n_regions, const void *slots, int64_t region_cap, const tq_column *regions) {
+  if (!h) return TQ_ERR_INVALID_ARG;
+  TQ_TRY(ensure_init());
+  const char *fn = "tq_sort_put_regions";
+  if (h->eof) { set_error("put after eof"); return TQ_ERR_STATE; }
+  const int w = (int)h->rows.cols.size(), nw = w + 1;
+  if (nw > 64) { set_error("%s: %d columns and the mask word exceed 64 words per row", fn, w); return TQ_ERR_INVALID_ARG; }
+  if (n_regions < 1 || n_regions > 8 || !slots || region_cap < 1 || region_cap > 0xFFFFFFF0ll || !regions) {
+    set_error("%s: 1..8 regions with their slots, 1 <= region_cap < 2^32", fn);
+    return TQ_ERR_INVALID_ARG;
+  }
+  for (int c = 0; c < w; c++)
+    if (h->rows.cols[(size_t)c].kind == 1) { set_error("%s: column %d: the range push carries no FLOAT columns", fn, c); return TQ_ERR_UNSUPPORTED_TYPE; }
+  for (int k = 0; k < n_regions * nw; k++) {
+    const int c = k % nw;
+    const bool var = c < w && h->rows.cols[(size_t)c].kind == 2;
+    if (var ? !regions[k].offsets : !regions[k].data) { set_error("%s: region %d has no area for wire column %d", fn, k / nw, c); return TQ_ERR_INVALID_ARG; }
+  }
+  Runtime &r = rt();
+  std::lock_guard<std::recursive_mutex> lk(r.mu);
+  cudaStream_t s = r.compute;
+  unsigned long long sl[16];
+  TQ_CUDA(cudaMemcpyAsync(sl, slots, (size_t)n_regions * 16, cudaMemcpyDeviceToHost, s));
+  TQ_CUDA(cudaStreamSynchronize(s));
+  int64_t rows[8], most = 0;
+  for (int g = 0; g < n_regions; g++) {
+    if (push_failed(sl[2 * g])) {   // the source failed after its checks: this step has no complete set of rows
+      const int32_t st = (int32_t)(uint32_t)sl[2 * g];
+      set_error("%s: source %d failed its push with status %d, so no destination can finish this step", fn, g, st);
+      return st;
+    }
+    if (sl[2 * g] > (unsigned long long)region_cap) {
+      set_error("%s: a region overflowed (its slot reads more than %lld rows)", fn, (long long)region_cap);
+      return TQ_ERR_OOM;
+    }
+    rows[g] = (int64_t)sl[2 * g];
+    most = std::max(most, rows[g]);
+  }
+  if (most == 0) return TQ_OK;
+  if ((int)h->region_bm.size() < w) h->region_bm.resize((size_t)w);
+  std::vector<uint32_t *> bm((size_t)w);
+  for (int c = 0; c < w; c++) {
+    TQ_TRY(h->region_bm[(size_t)c].reserve(bitmap_alloc_bytes(most)));
+    bm[(size_t)c] = h->region_bm[(size_t)c].as<uint32_t>();
+  }
+  std::vector<tq_column> in((size_t)w);
+  for (int g = 0; g < n_regions; g++) {
+    if (rows[g] == 0) continue;
+    const tq_column *reg = regions + (size_t)g * nw;
+    TQ_TRY(expand_null_mask(reinterpret_cast<const uint64_t *>(reg[w].data), rows[g], w, bm.data(), s));
+    for (int c = 0; c < w; c++) {
+      in[(size_t)c] = reg[c];
+      in[(size_t)c].length = rows[g];
+      in[(size_t)c].null_bitmap = reinterpret_cast<uint8_t *>(bm[(size_t)c]);
+    }
+    TQ_TRY(h->rows.append_device(in.data(), s));   // in stream order after the expansion; it synchronises
+  }
+  return TQ_OK;
 }
 
 // fetchRowChunks is done: sort (sort.go:58-70) and materialise the rows the parent may ask for

@@ -1068,6 +1068,241 @@ class RegionAgg:
         return res
 
 
+class RegionSort:
+    """The multi-GPU ORDER BY and ORDER BY ... LIMIT over a RegionExchange of two tables: 0 = the splitter sample (the
+    broadcast's wire format: the ByItem columns, then the tie word), 1 = the rows (the GROUP BY push's wire format: one word
+    area per column, a BYTES column's being its offsets, the mask word, then one byte area per BYTES column).  Rank r holds
+    shard r; the global order is tq_sort of the shards concatenated in rank order (equal keys keep that order).
+
+    ORDER BY (limit_count < 0): rank d ends up with the d-th contiguous slice of the global order.
+
+        push stream    tq_partition_push_sample (min(n, n_samples) rows + tie words to every rank)
+        compute stream tq_region_wait | tq_sort of the W sample regions, by the ByItems then the tie word | splitters at
+                       rows floor(k m / W), k = 1 .. W - 1, of the m sample rows (the same on every rank, no host comparator)
+        push stream    tq_partition_push_ranges (row -> the splitters at or below (its keys, its tie word))
+        compute stream tq_region_wait | tq_sort_put_regions (sources in rank order) | eof | drain
+
+    The tie word (src_rank << 32) | row is the last, ascending ByItem of the routing only: it makes the routing order total
+    and equal to the global order, so a run of equal keys is split between ranks wherever the splitters fall (a column of one
+    value spreads evenly), and the rows a rank receives from the sources, put in rank order and sorted stably, are its slice.
+
+    ORDER BY ... LIMIT (limit_count >= 0): each rank sorts its shard with limit (0, limit_offset + limit_count) and pushes
+    that result to rank 0 (tq_partition_push_ranges, one destination); rank 0 sorts the W regions with the real limit and
+    holds rows [limit_offset, limit_offset + limit_count) of the global order, every other rank none.
+
+    Sizing: every (source, destination) region holds a whole shard (n_max rows) and each byte area a shard's cells
+    (byte_caps), so no push overflows on rows: the splitters decide only how evenly the work spreads.  The price is W x the
+    largest shard held per rank for the rows (the cost BroadcastJoin pays for its build side), plus a sample table of W x
+    min(n_max, n_samples) rows whose byte areas also take byte_caps (the sampled rows are distinct, so their cells never
+    exceed the shard's)."""
+
+    def __init__(self, lib, L, world, rank, types, by_cols, by_desc, n_max, byte_caps=None, nullable=False, limit_offset=0, limit_count=-1,
+                 n_samples=1024, slot=0, exchange=None, seed=0x5EED5EED):
+        """types: TQ_TYPE_INT64 / _UINT64 / _FLOAT64 / _BYTES per column; by_cols / by_desc: the 0..8 ByItems; n_max: the
+        largest shard; byte_caps: per column, for a BYTES column the most cell bytes one shard holds (None for the others);
+        nullable: the columns may carry NULL bitmaps (the sample then carries bitmap words).  Every rank passes the same
+        numbers: the layout is shared.  exchange: a RegionLayout with the attributes of a RegionExchange (rank, epoch, wait,
+        next_epoch) holding RegionSort.table_of(...) as tables 0 and 1; by default a RegionExchange over the process group."""
+        self.lib, self.L, self.world, self.rank, self.slot = lib, L, world, rank, slot
+        self.types, self.by_cols, self.by_desc = [t & 0xFF for t in types], list(by_cols), [int(bool(d)) for d in by_desc]
+        if len(self.by_cols) != len(self.by_desc) or len(self.by_cols) > 8:
+            raise ValueError("RegionSort: by_cols and by_desc name the same 0..8 ByItems")
+        self.nullable = int(bool(nullable))
+        self.limit_offset, self.limit_count = int(limit_offset), int(limit_count)
+        self.n_samples, self.seed = int(n_samples), int(seed)
+        self.byte_caps = [int((byte_caps or [None] * len(self.types))[c] or 0) for c in range(len(self.types))]
+        self.tables = RegionSort.table_of(self.types, self.by_cols, n_max, self.byte_caps, self.nullable, self.n_samples)
+        self.rx = exchange if exchange is not None else RegionExchange(lib, L, world, rank, self.tables, align_rows=1)
+        self._handles = []   # sort handles whose lent results a push may still read
+
+    @staticmethod
+    def table_of(types, by_cols, n_max, byte_caps, nullable, n_samples=1024):
+        """[the sample table, the rows table] as RegionLayout tables.  The sample is BroadcastJoin.table_of over the ByItem
+        columns and the tie word (UINT64) at min(n_max, n_samples) rows; the rows table has n_max rows per region: per column
+        n_max words (a BYTES column: n_max + 1 offsets), the mask word, then a byte area of byte_caps[c] bytes per BYTES
+        column, every area rounded up to 16 bytes."""
+        from . import _lib
+        types = [t & 0xFF for t in types]
+        is_b = [t == _lib.TQ_TYPE_BYTES for t in types]
+        caps = [int((byte_caps or [None] * len(types))[c] or 0) for c in range(len(types))]
+        for c in range(len(types)):
+            if is_b[c] and not 1 <= caps[c] < (1 << 32) - 16:
+                raise ValueError(f"RegionSort: BYTES column {c} needs 1 <= byte_caps[{c}] < 2^32 - 16")
+        sample = BroadcastJoin.table_of([types[b] for b in by_cols] + [_lib.TQ_TYPE_UINT64], min(max(int(n_max), 1), int(n_samples)),
+                                        [caps[b] for b in by_cols] + [None], nullable)
+        cap = _round_up(max(int(n_max), 1), 2)
+        words = [_round_up(cap + 1, 2) if b else cap for b in is_b] + [cap] + [_round_up(caps[c], 16) // 8 for c in range(len(types)) if is_b[c]]
+        return [sample, (len(words), cap, words)]
+
+    def close(self):
+        self.rx.close()
+
+    def _sample_areas(self, g, rows):
+        """source g's sample region on this rank as a tq_column chunk of `rows` rows (ByItem columns, then the tie word)"""
+        rx, L = self.rx, self.L
+        st = [self.types[b] for b in self.by_cols] + [L.TQ_TYPE_UINT64]
+        arr = (L.TQColumn * len(st))()
+        a = 0
+        for c, t in enumerate(st):
+            arr[c].length = rows
+            if t == L.TQ_TYPE_BYTES:
+                arr[c].offsets, arr[c].data = rx.region_ptr(rx.rank, 0, g, a), rx.region_ptr(rx.rank, 0, g, a + 1)
+                a += 2
+            else:
+                arr[c].data = rx.region_ptr(rx.rank, 0, g, a)
+                a += 1
+            if self.nullable:
+                arr[c].null_bitmap = rx.region_ptr(rx.rank, 0, g, a)
+                a += 1
+        return arr
+
+    def _published(self, t):
+        """one host read of this rank's slots of table t after its wait: a slot that does not carry this epoch (a peer that
+        never pushed) raises RuntimeError.  Returns the slots' rows words"""
+        rx = self.rx
+        self.L.check(self.lib.tq_compute_synchronize())
+        raw = rx.read_slots(rx.rank, t, 1)[0]
+        late = [g for g in range(self.world) if int(raw[g, 1]) != rx.epoch]
+        if late:
+            raise RuntimeError(f"RegionSort: sources {late} did not publish table {t} for epoch {rx.epoch}")
+        return [int(x) for x in raw[:, 0]]
+
+    def _sort(self, n_cols, types, by_cols, by_desc, limit_offset, limit_count):
+        L = self.L
+        tt = (C.c_int32 * n_cols)(*types)
+        bc, bd = (C.c_int32 * max(len(by_cols), 1))(*by_cols), (C.c_int32 * max(len(by_desc), 1))(*by_desc)
+        d = L.TQSortDesc(n_cols, tt, len(by_cols), bc, bd, limit_offset, limit_count)
+        h = C.c_void_p()
+        L.check(self.lib.tq_sort_create(C.byref(d), C.byref(h)))
+        self._handles.append(h)
+        return h
+
+    def _lend(self, h, n_cols):
+        out = (self.L.TQColumn * n_cols)()
+        rows, eof = C.c_int64(0), C.c_int32(0)
+        self.L.check(self.lib.tq_sort_next_device(h, out, C.byref(rows), C.byref(eof)))
+        return out, rows.value
+
+    def push_sample(self, cols, bitmaps=None):
+        """ORDER BY: enqueue the push of this rank's splitter sample (push stream) for the exchange's current epoch.  cols:
+        this rank's shard of every column ((device pointer, rows)-like objects, or VarCol / DeviceVarColumn for BYTES);
+        bitmaps: a device NULL bitmap pointer (or None) per column"""
+        L, rx = self.L, self.rx
+        arr, n = _tq_device(L, cols, bitmaps)
+        nb = len(self.by_cols)
+        types, by = (C.c_int32 * len(self.types))(*self.types), (C.c_int32 * max(nb, 1))(*self.by_cols)
+        caps = (C.c_int64 * len(self.byte_caps))(*self.byte_caps)
+        dest, cnts = rx.push_tables(0, self.rank)
+        L.check(self.lib.tq_partition_push_sample(len(self.types), arr, types, n, nb, by, self.nullable, self.rank, self.n_samples, self.seed,
+                                                  self.world, dest, cnts, rx.cap[0], caps, self.slot, rx.epoch))
+
+    def push_rows(self, cols, bitmaps=None):
+        """enqueue the push of this rank's rows (push stream): ORDER BY after every rank's push_sample (this waits for the
+        samples and sorts them), TopN on its own.  The shard (and the handles lent to the push) are read until
+        tq_partition_push_sync(slot)."""
+        L, lib, rx, w = self.L, self.lib, self.rx, self.world
+        arr, n = _tq_device(L, cols, bitmaps)
+        nc, nb = len(self.types), len(self.by_cols)
+        types, by = (C.c_int32 * nc)(*self.types), (C.c_int32 * max(nb, 1))(*self.by_cols)
+        desc = (C.c_int32 * max(nb, 1))(*self.by_desc)
+        caps = (C.c_int64 * nc)(*self.byte_caps)
+        split, m, pos = None, 0, None
+        if self.limit_count >= 0:                 # TopN: this shard's first limit_offset + limit_count rows, to rank 0
+            h = self._sort(nc, self.types, self.by_cols, self.by_desc, 0, self.limit_offset + self.limit_count)
+            if n:
+                L.check(lib.tq_sort_put(h, arr, L.TQ_MEM_DEVICE))
+            L.check(lib.tq_sort_eof(h))
+            arr, n = self._lend(h, nc)
+            if n == 0:
+                arr = _tq_device(L, cols, bitmaps)[0]
+            dest, cnts = rx.push_tables(1, self.rank)
+            n_parts = 1
+        else:                                     # ORDER BY: the splitters from the W samples, then every row to its rank
+            rx.wait(0)
+            self._published(0)
+            cnt = rx.counts(rx.rank, 0, 1)[0]          # a sample push that failed or overflowed raises here, on every rank
+            st = [self.types[b] for b in self.by_cols] + [L.TQ_TYPE_UINT64]
+            h = self._sort(nb + 1, st, list(range(nb + 1)), self.by_desc + [0], 0, -1)
+            for g in range(w):
+                if cnt[g]:
+                    L.check(lib.tq_sort_put(h, self._sample_areas(g, cnt[g]), L.TQ_MEM_DEVICE))
+            L.check(lib.tq_sort_eof(h))
+            split, m = self._lend(h, nb + 1)
+            pos = (C.c_int64 * max(w - 1, 1))(*[k * m // w for k in range(1, w)])
+            dest, cnts = rx.push_tables(1, self.rank)
+            n_parts = w
+        L.check(lib.tq_partition_push_ranges(nc, arr, types, n, nb, by, desc, self.rank, n_parts, split, m, pos, dest, cnts, rx.cap[1], caps,
+                                             self.slot, rx.epoch))
+
+    def finish(self, keep_result=False):
+        """this rank's half after every rank's push_rows: wait, put the regions in rank order, sort, drain.  Returns (rows on
+        this rank, result): result (keep_result) = host Columns of this rank's rows in order, None otherwise.  A region past
+        its byte cap, or a source whose push failed, raises (TQError) on every rank."""
+        lib, L, rx, w = self.lib, self.L, self.rx, self.world
+        nc = len(self.types)
+        try:
+            if self.limit_count >= 0 and self.rank != 0:
+                return 0, None
+            rx.wait(1)
+            self._published(1)                         # a failed or overflowed source: tq_sort_put_regions refuses the step
+            h = self._sort(nc, self.types, self.by_cols, self.by_desc, self.limit_offset if self.limit_count >= 0 else 0, self.limit_count)
+            regs = (L.TQColumn * (w * (nc + 1)))()
+            for g in range(w):
+                v = 0
+                for c in range(nc + 1):
+                    k = g * (nc + 1) + c
+                    regs[k].length, regs[k].data = rx.cap[1], rx.region_ptr(rx.rank, 1, g, c)
+                    if c < nc and self.types[c] == L.TQ_TYPE_BYTES:
+                        regs[k].offsets, regs[k].data = regs[k].data, rx.region_ptr(rx.rank, 1, g, nc + 1 + v)
+                        v += 1
+            L.check(lib.tq_sort_put_regions(h, w, C.c_void_p(rx.slot_ptr(rx.rank, 1, 0)), rx.cap[1], regs))
+            L.check(lib.tq_sort_eof(h))
+            out, rows = self._lend(h, nc)
+            res = None
+            if keep_result:
+                from .chunk import Column, VarColumn, device_to_host, device_var_to_host
+                res = ([device_var_to_host(out[c].data, out[c].offsets, out[c].null_bitmap, rows) if t == L.TQ_TYPE_BYTES
+                        else device_to_host(t, out[c].data, out[c].null_bitmap, rows) for c, t in enumerate(self.types)] if rows
+                       else [(VarColumn if t == L.TQ_TYPE_BYTES else Column).empty(t, 0) for t in self.types])
+            return rows, res
+        finally:
+            self.release()
+
+    def release(self):
+        """wait for this rank's pushes and free what they read"""
+        self.lib.tq_partition_push_sync(self.slot)
+        for h in self._handles:
+            self.lib.tq_sort_destroy(h)
+        self._handles = []
+
+    def step(self, cols, bitmaps=None, keep_result=False):
+        """one step on this rank: (sample push, splitters,) row push, wait, put, sort, drain, then one all-gather of the W row
+        counts and one barrier.  Returns (rows on this rank, global position of its first row, result) — for TopN rank 0's
+        position is limit_offset.  A step that fails on any rank fails on every rank (a push that fails after its checks
+        makes every receiver refuse the step); the barrier is passed either way, so the ranks leave a failed step together
+        and the next step reuses the regions."""
+        self.rx.next_epoch()
+        rows, res, err = 0, None, None
+        try:
+            if self.limit_count < 0:
+                self.push_sample(cols, bitmaps)
+            self.push_rows(cols, bitmaps)
+            rows, res = self.finish(keep_result)
+        except Exception as e:
+            err = e
+        finally:
+            self.release()
+            counts = [None] * self.world
+            dist.all_gather_object(counts, None if err is not None else rows)
+            dist.barrier()
+        if err is not None:
+            raise err
+        failed = [g for g, c in enumerate(counts) if c is None]
+        if failed:
+            raise RuntimeError(f"RegionSort: the step failed on ranks {failed}")
+        return rows, (self.limit_offset if self.limit_count >= 0 else 0) + sum(counts[:self.rank]), res
+
+
 def gen_dist_tables(rank, world, n_b, n_p):
     """this rank's shard of the C5 tables: B.k = the keys k with k % world == rank (shuffled), B.v = 7k + 1; probe row i of
     rank r has the global id g = r * n_p + i, P.v = g and P.k = mix64(g) % (n_b * world) — uniform keys, every probe row
